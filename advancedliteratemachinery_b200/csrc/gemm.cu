@@ -3,8 +3,10 @@
 // warp-specialised CTAs (one per SM):
 //
 //     warpgroup 0     : TMA producers      (warp 0: A tiles, warp 1: B tiles, one elected lane each)
-//     warpgroups 1, 2 : consumers          (64 rows of the 128-row tile each: wgmma main loop, then the fused
-//                                           bias / act / residual / scatter epilogue from the accumulator registers)
+//     warpgroups 1, 2 : consumers          (ping-pong: each owns every other tile of the CTA, all 128 rows: wgmma
+//                                           main loop, then the fused bias / act / residual / scatter epilogue from
+//                                           the accumulator registers while the other warpgroup runs the MMAs of
+//                                           the next tile)
 //
 // Precision: the reference computes in fp32 (SURVEY.md 8).  bf16 tensor-core operands alone would miss the
 // "logits within 1e-3" bar, so every fp32 matrix is carried as a (hi, lo) bf16 pair with hi + lo == x to
@@ -14,6 +16,7 @@
 // Every linear layer of Swin-B / the decoder / ViT, the FPN 1x1 convolutions, the decoder cross-attention
 // (Q K^T and P V as batched GEMMs) and the vocabulary heads go through this one kernel.
 #include <algorithm>
+#include <type_traits>
 
 #include "alm_internal.h"
 #include "ptx.cuh"
@@ -26,8 +29,8 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle-128B row
 constexpr int WGMMA_K = 16;
 constexpr int kThreads = 384;  // warpgroup 0 TMA, warpgroups 1 and 2 MMA + epilogue
-constexpr int kConsumers = 2;
 constexpr int kMaxStages = 16;
+constexpr uint32_t kOrderBar = 1;  // named barriers kOrderBar + c: consumer c may start its next main loop
 
 struct GemmParams {
   int M, N, K;
@@ -200,12 +203,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     } else trace_slot = -1;
   }
 
+  // every CTA has at most one tile (grid-uniform): the two consumers share it instead of taking turns
+  const bool coop = p.num_tiles <= gridDim.x;
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tm_a);
     ptx::prefetch_tmap(&tm_b);
     for (int s = 0; s < p.stages; ++s) {
       ptx::mbar_init(&full_bar[s], 2);          // one arrive.expect_tx per producer warp (A tiles, B tiles)
-      ptx::mbar_init(&empty_bar[s], kConsumers);  // one arrival per consumer warpgroup
+      ptx::mbar_init(&empty_bar[s], coop ? 2 : 1);  // one arrival per consumer that reads the stage
     }
     ptx::fence_mbar_init();
   }
@@ -252,77 +257,121 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     }
   } else {
     // ===================================================================== consumers (2 warpgroups)
-    // Warpgroup c owns rows [64 c, 64 c + 64) of every 128-row tile: wgmma main loop into registers, then the fused
-    // epilogue straight from the accumulator fragment.  A warpgroup whose 64 rows are all past M multiplies the rows of
-    // warpgroup 0 instead and stores nothing: a branch around the wgmma would make ptxas serialise all of them.
+    // Ping-pong: consumer c owns the CTA's local tiles c, c + 2, c + 4, ... whole: both 64-row halves of the 128-row
+    // tile, one m64 accumulator each, wgmma main loop into registers, then the fused epilogue straight from the
+    // accumulator fragments.  The main loops take turns through the named barriers kOrderBar + c, so while one consumer
+    // runs the epilogue of its tile the other issues the MMAs of the next one.  The producers fill the ring in tile order,
+    // so each consumer steps its stage / phase over the k-blocks of the other's tiles.
+    // Cooperative (every CTA has one tile: the few-tile decode GEMMs): consumer c multiplies and stores half c of that
+    // tile, so the second warpgroup does not idle; both consume every fill.
+    // A 64-row half that lies past M multiplies the rows of half 0 instead and stores nothing: a branch around the wgmma
+    // would make ptxas serialise all of them.
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int cw = wg - 1;
     const bool leader = (threadIdx.x & 127) == 0;
     const Epilogue& e = p.e;
-    float acc[BLOCK_N / 2];
+    float acc[2][BLOCK_N / 2];
+    // local tiles of this CTA: blockIdx.x + j * gridDim.x for j < n_local
+    const long n_local = (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
     int stage = 0;
     uint32_t phase = 0;
-    for (long tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int batch = static_cast<int>(tile / tiles_per_batch);
-      const int rem = static_cast<int>(tile % tiles_per_batch);
-      const int m_blk = rem / p.n_blocks, n_blk = rem % p.n_blocks;
-      const int b0 = batch % p.nb0, b1 = batch / p.nb0;
-      const int row_base = m_blk * BLOCK_M + cw * 64;
-      const bool live = row_base < p.M;   // warpgroup-uniform
-      const uint32_t a_row_off = live ? cw * 64 * 128 : 0;
+    auto skip_tile = [&]() {  // the k-blocks of one tile of the other consumer
+      stage += p.k_blocks;
+      phase ^= (stage / p.stages) & 1;
+      stage %= p.stages;
+    };
+    // one tile's main loop over A rows a_off0 (-> acc[0]) and, with two halves, a_off1 (-> acc[1]); returns the stage of
+    // the last k-block, still in flight
+    auto main_loop = [&](auto halves, uint32_t a_off0, uint32_t a_off1) {
+      constexpr bool kTwo = decltype(halves)::value == 2;
       int prev = -1;
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         ptx::mbar_wait_wg(&full_bar[stage], phase);
-        const uint32_t a_hi = ptx::smem_u32(stage_base + stage * p.stage_bytes) + a_row_off;
+        const uint32_t a_hi = ptx::smem_u32(stage_base + stage * p.stage_bytes);
         const uint32_t a_lo = a_hi + p.a_bytes;
-        const uint32_t b_hi = ptx::smem_u32(stage_base + stage * p.stage_bytes) + L::kNumA * p.a_bytes;
+        const uint32_t b_hi = a_hi + L::kNumA * p.a_bytes;
         const uint32_t b_lo = b_hi + L::kBBytes;
         ptx::wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
           const uint32_t koff = k * WGMMA_K * 2;  // bytes inside the 128 B swizzle row
-          const uint64_t da = ptx::make_kmajor_sw128_desc(a_hi + koff);
+          const uint64_t da0 = ptx::make_kmajor_sw128_desc(a_hi + a_off0 + koff);
+          const uint64_t da1 = ptx::make_kmajor_sw128_desc(a_hi + a_off1 + koff);
           const uint64_t db = ptx::make_kmajor_sw128_desc(b_hi + koff);
-          wgmma_tile<BLOCK_N>(acc, da, db, (kb | k) != 0);
+          wgmma_tile<BLOCK_N>(acc[0], da0, db, (kb | k) != 0);
+          if constexpr (kTwo) wgmma_tile<BLOCK_N>(acc[1], da1, db, (kb | k) != 0);
           if (NSPLIT == 3) {
-            wgmma_tile<BLOCK_N>(acc, ptx::make_kmajor_sw128_desc(a_lo + koff), db, 1);
-            wgmma_tile<BLOCK_N>(acc, da, ptx::make_kmajor_sw128_desc(b_lo + koff), 1);
+            wgmma_tile<BLOCK_N>(acc[0], ptx::make_kmajor_sw128_desc(a_lo + a_off0 + koff), db, 1);
+            if constexpr (kTwo) wgmma_tile<BLOCK_N>(acc[1], ptx::make_kmajor_sw128_desc(a_lo + a_off1 + koff), db, 1);
+            const uint64_t db_lo = ptx::make_kmajor_sw128_desc(b_lo + koff);
+            wgmma_tile<BLOCK_N>(acc[0], da0, db_lo, 1);
+            if constexpr (kTwo) wgmma_tile<BLOCK_N>(acc[1], da1, db_lo, 1);
           }
         }
         ptx::wgmma_commit();
         // the group of the previous k-block has retired -> its stage may be refilled
         ptx::wgmma_wait<1>();
-        ptx::wgmma_fence_operands(acc);
+        ptx::wgmma_fence_operands(acc[0]);
+        ptx::wgmma_fence_operands(acc[1]);
         ptx::mbar_arrive_if(&empty_bar[prev < 0 ? 0 : prev], leader && prev >= 0);
         prev = stage;
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
+      return prev;
+    };
+    if (cw == 1 && !coop) skip_tile();
+    for (long j = coop ? 0 : cw; j < n_local; j += 2) {
+      const long tile = blockIdx.x + j * gridDim.x;
+      const int batch = static_cast<int>(tile / tiles_per_batch);
+      const int rem = static_cast<int>(tile % tiles_per_batch);
+      const int m_blk = rem / p.n_blocks, n_blk = rem % p.n_blocks;
+      const int b0 = batch % p.nb0, b1 = batch / p.nb0;
+      const int row_base = m_blk * BLOCK_M;
+      // the other consumer has issued the MMAs of local tile j - 1
+      ptx::named_bar_sync_if(kOrderBar + cw, 2 * 128, j > 0);
+      int prev;
+      if (coop) {
+        prev = main_loop(std::integral_constant<int, 1>{}, row_base + 64 * cw < p.M ? cw * 64 * 128 : 0, 0);
+      } else {
+        prev = main_loop(std::integral_constant<int, 2>{}, 0, row_base + 64 < p.M ? 64 * 128 : 0);
+      }
+      // every MMA of tile j is issued: the other consumer may start local tile j + 1
+      ptx::named_bar_arrive_if(kOrderBar + (cw ^ 1), 2 * 128, j + 1 < n_local);
       ptx::wgmma_wait<0>();
-      ptx::wgmma_fence_operands(acc);
+      ptx::wgmma_fence_operands(acc[0]);
+      ptx::wgmma_fence_operands(acc[1]);
       ptx::mbar_arrive_if(&empty_bar[prev], leader);
-      if (!live) continue;
+      skip_tile();
 
-      // ---- epilogue: this thread holds rows r0, r0 + 8 and column pairs 8 j + 2 (lane % 4) of the tile
+      // ---- epilogue: this thread holds rows r0 + 8 q (q = 0..3: rows r0, r0 + 8 of half 0, then of half 1; in the
+      // cooperative schedule only the two of half c, in acc[0]) and column pairs 8 j + 2 (lane % 4) of the tile.  The row loop stays rolled, picking row q's values out of the fragment with
+      // selects: every epi_pair copy is tens of instructions, and a fully unrolled epilogue is large enough that
+      // instruction fetch, not the stores, sets its pace (measured: twice the time per tile).
       const long obatch = static_cast<long>(b0) * e.obs0 + static_cast<long>(b1) * e.obs1;
       const float* rbatch = e.resid ? e.resid + static_cast<long>(b0) * e.rbs0 + static_cast<long>(b1) * e.rbs1 : nullptr;
       const float* bias = e.bias ? e.bias + static_cast<long>(b0) * e.bias_bs0 : nullptr;
       const int r0 = row_base + (warp & 3) * 16 + (lane >> 2);
       const int cbase = n_blk * BLOCK_N + 2 * (lane & 3);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
+#pragma unroll 1
+      for (int q = coop ? 2 * cw : 0; q < (coop ? 2 * cw + 2 : 4); ++q) {
+        const int row = r0 + 64 * (q >> 1) + 8 * (q & 1);
+        const bool hi_acc = !coop && (q >> 1);  // row q's values sit in acc[1]
         if (row >= p.M) continue;
         const int orow = e.out_map ? e.out_map[row] : row;
         if (orow < 0) continue;
         const int rrow = e.resid_map ? e.resid_map[row] : orow;
         const float rbias = (bias && e.bias_mode == BIAS_ROW) ? bias[row] : 0.0f;
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int col = cbase + 8 * j;
+        for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
+          const int col = cbase + 8 * jj;
           if (col >= p.N) break;
           const int ncols = min(2, p.N - col);
-          epi_pair(e, obatch, rbatch, bias, orow, rrow, rbias, col, ncols, p.vec_ok && ncols == 2,
-                   acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          float v[2];
+#pragma unroll
+          for (int t = 0; t < 2; ++t)
+            v[t] = (q & 1) ? (hi_acc ? acc[1][4 * jj + 2 + t] : acc[0][4 * jj + 2 + t])
+                           : (hi_acc ? acc[1][4 * jj + t] : acc[0][4 * jj + t]);
+          epi_pair(e, obatch, rbatch, bias, orow, rrow, rbias, col, ncols, p.vec_ok && ncols == 2, v[0], v[1]);
         }
       }
     }
@@ -453,7 +502,7 @@ void launch_wgmma(Ctx* c, const Operand& A, const Operand& B, GemmParams& p) {
   p.n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
   p.num_tiles = static_cast<long>(p.m_blocks) * p.n_blocks * p.nb0 * p.nb1;
   // rows of A beyond M are never stored, so the TMA box only covers the live rows (multiple of 8 = one swizzle
-  // group); a consumer warpgroup may still read up to 64 rows of shared memory, the stale ones only feed discarded
+  // group); the second 64-row half of a tile may still read up to 64 rows of shared memory, the stale ones only feed discarded
   // accumulator rows (the stage layout keeps those reads inside the stage ring).
   const int a_rows = std::min(BLOCK_M, (p.M + 7) & ~7);
   p.a_bytes = a_rows * BLOCK_K * 2;

@@ -146,6 +146,20 @@ __device__ __forceinline__ void mbar_wait_wg(uint64_t* bar, uint32_t parity) {
       : "memory");
 }
 
+// ---------------------------------------------------------------- named barriers (barrier 0 is __syncthreads)
+// bar.sync blocks the calling warps until `count` threads have reached barrier `id`; bar.arrive adds the calling warps
+// without blocking.  Predicated instead of branched (see mbar_arrive_if); `pred` must be warp-uniform.
+__device__ __forceinline__ void named_bar_sync_if(uint32_t id, uint32_t count, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p bar.sync %0, %1;\n\t}" ::"r"(id), "r"(count),
+               "r"(static_cast<uint32_t>(pred))
+               : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive_if(uint32_t id, uint32_t count, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p bar.arrive %0, %1;\n\t}" ::"r"(id), "r"(count),
+               "r"(static_cast<uint32_t>(pred))
+               : "memory");
+}
+
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
