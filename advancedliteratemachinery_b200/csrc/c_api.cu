@@ -47,6 +47,18 @@ int guarded(alm_ctx* h, F&& f) {
   }
 }
 
+// for the entry points without a context: f returns the code
+template <class F>
+int guarded_free(F&& f) {
+  try {
+    return f();
+  } catch (const AlmError& e) {
+    return e.code;
+  } catch (...) {
+    return ALM_ERR_INVALID;
+  }
+}
+
 bool is_device_ptr(const void* p) {
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
@@ -54,6 +66,32 @@ bool is_device_ptr(const void* p) {
     return false;
   }
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+// every non-null pointer is device memory aligned to `align` bytes
+void require_device(std::initializer_list<const void*> ptrs, size_t align, const std::string& what) {
+  for (const void* p : ptrs)
+    ALM_REQUIRE(!p || (is_device_ptr(p) && reinterpret_cast<uintptr_t>(p) % align == 0), ALM_ERR_INVALID,
+                what + (align > 1 ? ": device pointers aligned to " + std::to_string(align) + " bytes required"
+                                  : std::string(": device pointers required")));
+}
+
+// milliseconds of `iters` calls of body() on the stream, after `warmup` untimed ones
+template <class F>
+float time_ms(Ctx* c, int warmup, int iters, F&& body) {
+  for (int i = 0; i < warmup; ++i) body();
+  cudaEvent_t e0, e1;
+  ALM_CHECK_CUDA(cudaEventCreate(&e0));
+  ALM_CHECK_CUDA(cudaEventCreate(&e1));
+  ALM_CHECK_CUDA(cudaEventRecord(e0, c->stream));
+  for (int i = 0; i < iters; ++i) body();
+  ALM_CHECK_CUDA(cudaEventRecord(e1, c->stream));
+  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+  float ms = 0;
+  ALM_CHECK_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  return ms;
 }
 
 // returns a device pointer for `p` (host buffers are copied into the context's staging slab on the stream)
@@ -69,6 +107,38 @@ const void* stage_input(alm_ctx* h, const void* p, size_t bytes, void** slab, si
   }
   ALM_CHECK_CUDA(cudaMemcpyAsync(*slab, p, bytes, cudaMemcpyHostToDevice, h->c.stream));
   return *slab;
+}
+
+// device copies of the caller's uint8 HWC images (host pointers are staged into the workspace on the stream)
+std::vector<PreImage> stage_images(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths, int n) {
+  Ctx* c = &h->c;
+  c->ensure_ws();
+  std::vector<PreImage> imgs(static_cast<size_t>(n));
+  for (int i = 0; i < n; ++i) {
+    ALM_REQUIRE(rgb[i] && heights[i] > 0 && widths[i] > 0, ALM_ERR_INVALID, "image pointer / size");
+    const size_t bytes = static_cast<size_t>(heights[i]) * widths[i] * 3;
+    const uint8_t* d = rgb[i];
+    if (!is_device_ptr(d)) {
+      uint8_t* slot = c->ws.get<uint8_t>(bytes);
+      ALM_CHECK_CUDA(cudaMemcpyAsync(slot, rgb[i], bytes, cudaMemcpyHostToDevice, c->stream));
+      d = slot;
+    }
+    imgs[static_cast<size_t>(i)] = PreImage{d, heights[i], widths[i], 0, 0};
+  }
+  return imgs;
+}
+
+// body(pages) on the caller's pages staged by stage_images, once every output is known to be device memory; the pages
+// live in the workspace until body returns
+template <class F>
+void with_pages(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths, int n,
+                std::initializer_list<const void*> outs, const char* what, F&& body) {
+  require_device(outs, 1, std::string(what) + " outputs");
+  Ctx* c = &h->c;
+  c->ensure_ws();
+  ArenaScope arena_scope(c->ws);
+  std::vector<PreImage> pages = stage_images(h, rgb, heights, widths, n);
+  body(pages);
 }
 
 void d2h(Ctx* c, void* dst, const void* src, size_t bytes) {
@@ -125,6 +195,39 @@ __global__ void op_join_kernel(const bf16* __restrict__ hi, const bf16* __restri
   if (i < n) out[i] = __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
 }
 unsigned blocks256(long n) { return static_cast<unsigned>((n + 255) / 256); }
+
+// The model's decoder caches for nimg_total images in the workspace: K (and V when v is given), with layer dl of images
+// img0..img0+nimg-1 scattered head-major from x [nimg_total][M][512].  Every element a call must not read holds NaN
+// (0xffff): other layers, other images, and the keys at or past key_len[i] of image i (when key_len is given).
+struct DecoderCache {
+  bf16 *kh = nullptr, *kl = nullptr, *vh = nullptr, *vl = nullptr;
+  long off = 0;  // elements from a plane's base to (img0, dl)
+};
+DecoderCache decoder_cache(Ctx* c, const float* k, const float* v, int nimg_total, int img0, int nimg, int M, int dl,
+                           const int* key_len) {
+  DecoderCache d;
+  const size_t cache = static_cast<size_t>(nimg_total) * 96 * M * 64;
+  d.kh = c->ws.get<bf16>(cache); d.kl = c->ws.get<bf16>(cache);
+  if (v) { d.vh = c->ws.get<bf16>(cache); d.vl = c->ws.get<bf16>(cache); }
+  for (bf16* p : {d.kh, d.kl, d.vh, d.vl})
+    if (p) ALM_CHECK_CUDA(cudaMemsetAsync(p, 0xff, cache * 2, c->stream));
+  d.off = (static_cast<long>(img0) * 96 + dl * 8) * M * 64;
+  const long nkv = static_cast<long>(nimg) * M * 512, in_off = static_cast<long>(img0) * M * 512;
+  op_head_major_kernel<<<blocks256(nkv), 256, 0, c->stream>>>(k + in_off, M, nkv, d.kh + d.off, d.kl + d.off);
+  if (v) op_head_major_kernel<<<blocks256(nkv), 256, 0, c->stream>>>(v + in_off, M, nkv, d.vh + d.off, d.vl + d.off);
+  check_launch("op_head_major");
+  for (int i = 0; key_len && i < nimg; ++i) {
+    const int n = key_len[img0 + i];
+    if (n == M) continue;
+    // rows n..M-1 of the 8 [M][64] head blocks of this image and layer
+    const long base = d.off + static_cast<long>(i) * 96 * M * 64 + static_cast<long>(n) * 64;
+    for (bf16* p : {d.kh, d.kl, d.vh, d.vl})
+      if (p)
+        ALM_CHECK_CUDA(cudaMemset2DAsync(p + base, static_cast<size_t>(M) * 128, 0xff, static_cast<size_t>(M - n) * 128, 8,
+                                         c->stream));
+  }
+  return d;
+}
 
 }  // namespace
 
@@ -193,16 +296,51 @@ void alm_free(alm_ctx* h) {
 
 const char* alm_last_error(const alm_ctx* h) { return h ? h->c.err.c_str() : "null context"; }
 
+namespace {
+
+// the integer options of alm_set_option
+enum OptionKind { OPT_ANY, OPT_FLAG, OPT_SET };  // stored as given / stored as 0 or 1 / one of the values in `accepted`
+struct IntOption {
+  const char* name;
+  int Ctx::*field;
+  OptionKind kind;
+  unsigned accepted;  // OPT_SET: bit v set when value v is accepted
+  const char* rule;   // OPT_SET: the accepted values, for the error message
+};
+const IntOption kIntOptions[] = {
+    {"nsplit", &Ctx::nsplit, OPT_SET, 0b1010, "1 or 3"},
+    {"gemm_impl", &Ctx::gemm_impl, OPT_SET, 0b11, "0 or 1"},
+    {"xattn_impl", &Ctx::xattn_impl, OPT_SET, 0b111, "0..2"},
+    {"fuse_ln_gemv", &Ctx::fuse_ln_gemv, OPT_FLAG, 0, nullptr},
+    {"kv_decoders", &Ctx::kv_decoders, OPT_SET, 0b1110, "1..3"},
+    {"attn_impl", &Ctx::attn_impl, OPT_SET, 0b11, "0 or 1"},
+    {"wattn_impl", &Ctx::wattn_impl, OPT_SET, 0b1011, "0, 1 or 3"},
+    {"enc_grid_cap", &Ctx::enc_grid_cap, OPT_ANY, 0, nullptr},
+    {"dec_grid_cap", &Ctx::dec_grid_cap, OPT_ANY, 0, nullptr},
+    {"xattn_ctas_per_sm", &Ctx::xattn_ctas_per_sm, OPT_SET, 0b1110, "1..3"},
+    {"xattn_wg", &Ctx::xattn_wg, OPT_SET, 0b110, "1 or 2"},
+    {"sattn_wide", &Ctx::sattn_wide, OPT_FLAG, 0, nullptr},
+    {"debug_skip", &Ctx::debug_skip, OPT_ANY, 0, nullptr},
+    {"decode_priority", &Ctx::decode_priority, OPT_FLAG, 0, nullptr},
+    {"small_grid_cap", &Ctx::small_grid_cap, OPT_ANY, 0, nullptr},
+    {"decode_streams", &Ctx::decode_streams, OPT_SET, 0b110, "1 or 2"},
+    {"use_graphs", &Ctx::use_graphs, OPT_FLAG, 0, nullptr},
+    {"profile_gemm", &Ctx::profile_gemm, OPT_FLAG, 0, nullptr},
+};
+
+}  // namespace
+
 int alm_set_option(alm_ctx* h, const char* key, long value) {
   return guarded(h, [&] {
     const std::string k = key ? key : "";
-    if (k == "nsplit") {
-      ALM_REQUIRE(value == 1 || value == 3, ALM_ERR_INVALID, "nsplit must be 1 or 3");
-      h->c.nsplit = static_cast<int>(value);
-    } else if (k == "gemm_impl") {
-      ALM_REQUIRE(value == 0 || value == 1, ALM_ERR_INVALID, "gemm_impl must be 0 or 1");
-      h->c.gemm_impl = static_cast<int>(value);
-    } else if (k == "trace_gemm") {
+    for (const IntOption& o : kIntOptions) {
+      if (k != o.name) continue;
+      ALM_REQUIRE(o.kind != OPT_SET || (value >= 0 && value < 32 && (o.accepted >> value & 1u)), ALM_ERR_INVALID,
+                  k + " must be " + o.rule);
+      h->c.*o.field = o.kind == OPT_FLAG ? (value ? 1 : 0) : static_cast<int>(value);
+      return;
+    }
+    if (k == "trace_gemm") {
       if (h->c.trace_buf) { cudaFree(h->c.trace_buf); cudaFree(h->c.trace_idx); h->c.trace_buf = nullptr; h->c.trace_idx = nullptr; }
       h->c.trace_cap = static_cast<int>(value);
       if (value > 0) {
@@ -210,45 +348,6 @@ int alm_set_option(alm_ctx* h, const char* key, long value) {
         ALM_CHECK_CUDA(cudaMalloc(&h->c.trace_idx, sizeof(int)));
         ALM_CHECK_CUDA(cudaMemset(h->c.trace_idx, 0, sizeof(int)));
       }
-    } else if (k == "xattn_impl") {
-      ALM_REQUIRE(value >= 0 && value <= 2, ALM_ERR_INVALID, "xattn_impl must be 0..2");
-      h->c.xattn_impl = static_cast<int>(value);
-    } else if (k == "fuse_ln_gemv") {
-      h->c.fuse_ln_gemv = value ? 1 : 0;
-    } else if (k == "kv_decoders") {
-      ALM_REQUIRE(value >= 1 && value <= 3, ALM_ERR_INVALID, "kv_decoders must be 1..3");
-      h->c.kv_decoders = static_cast<int>(value);
-    } else if (k == "attn_impl") {
-      ALM_REQUIRE(value == 0 || value == 1, ALM_ERR_INVALID, "attn_impl must be 0 or 1");
-      h->c.attn_impl = static_cast<int>(value);
-    } else if (k == "wattn_impl") {
-      ALM_REQUIRE(value == 0 || value == 1 || value == 3, ALM_ERR_INVALID, "wattn_impl must be 0, 1 or 3");
-      h->c.wattn_impl = static_cast<int>(value);
-    } else if (k == "enc_grid_cap") {
-      h->c.enc_grid_cap = static_cast<int>(value);
-    } else if (k == "dec_grid_cap") {
-      h->c.dec_grid_cap = static_cast<int>(value);
-    } else if (k == "xattn_ctas_per_sm") {
-      ALM_REQUIRE(value >= 1 && value <= 3, ALM_ERR_INVALID, "xattn_ctas_per_sm must be 1..3");
-      h->c.xattn_ctas_per_sm = static_cast<int>(value);
-    } else if (k == "xattn_wg") {
-      ALM_REQUIRE(value == 1 || value == 2, ALM_ERR_INVALID, "xattn_wg must be 1 or 2");
-      h->c.xattn_wg = static_cast<int>(value);
-    } else if (k == "sattn_wide") {
-      h->c.sattn_wide = value ? 1 : 0;
-    } else if (k == "debug_skip") {
-      h->c.debug_skip = static_cast<int>(value);
-    } else if (k == "decode_priority") {
-      h->c.decode_priority = value ? 1 : 0;
-    } else if (k == "small_grid_cap") {
-      h->c.small_grid_cap = static_cast<int>(value);
-    } else if (k == "decode_streams") {
-      ALM_REQUIRE(value == 1 || value == 2, ALM_ERR_INVALID, "decode_streams must be 1 or 2");
-      h->c.decode_streams = static_cast<int>(value);
-    } else if (k == "use_graphs") {
-      h->c.use_graphs = value ? 1 : 0;
-    } else if (k == "profile_gemm") {
-      h->c.profile_gemm = value ? 1 : 0;
     } else if (k == "workspace_mb") {
       ALM_REQUIRE(value >= 64 && h->c.ws.base == nullptr, ALM_ERR_STATE, "workspace_mb must be set before first use");
       h->c.ws_bytes = static_cast<size_t>(value) << 20;
@@ -313,18 +412,9 @@ int alm_bench_graph_floor(alm_ctx* h, int nodes, int iters, float* us_per_node) 
     ALM_CHECK_CUDA(cudaStreamEndCapture(c->stream, &g));
     ALM_CHECK_CUDA(cudaGraphInstantiate(&ge, g, 0));
     cudaGraphDestroy(g);
-    for (int i = 0; i < 3; ++i) ALM_CHECK_CUDA(cudaGraphLaunch(ge, c->stream));
-    cudaEvent_t e0, e1;
-    ALM_CHECK_CUDA(cudaEventCreate(&e0));
-    ALM_CHECK_CUDA(cudaEventCreate(&e1));
-    ALM_CHECK_CUDA(cudaEventRecord(e0, c->stream));
-    for (int i = 0; i < iters; ++i) ALM_CHECK_CUDA(cudaGraphLaunch(ge, c->stream));
-    ALM_CHECK_CUDA(cudaEventRecord(e1, c->stream));
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-    float ms = 0;
-    ALM_CHECK_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    const float ms = time_ms(c, 3, iters, [&] { ALM_CHECK_CUDA(cudaGraphLaunch(ge, c->stream)); });
     *us_per_node = ms * 1e3f / (static_cast<float>(iters) * nodes);
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaGraphExecDestroy(ge);
+    cudaGraphExecDestroy(ge);
   });
 }
 
@@ -351,19 +441,7 @@ int alm_bench_gemm_ex(alm_ctx* h, int M, int N, int K, int batch, int split_out,
     if (split_out) { e.out_hi = c->ws.get<bf16>(no); e.out_lo = c->ws.get<bf16>(no); }
     else e.out_f32 = c->ws.get<float>(no);
     e.ldo = ldo; e.obs0 = static_cast<long>(M) * ldo; e.act = act;
-    for (int i = 0; i < 3; ++i) gemm(c, a, b, e);
-    cudaEvent_t e0, e1;
-    ALM_CHECK_CUDA(cudaEventCreate(&e0));
-    ALM_CHECK_CUDA(cudaEventCreate(&e1));
-    ALM_CHECK_CUDA(cudaEventRecord(e0, c->stream));
-    for (int i = 0; i < iters; ++i) gemm(c, a, b, e);
-    ALM_CHECK_CUDA(cudaEventRecord(e1, c->stream));
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-    float ms = 0;
-    ALM_CHECK_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    *ms_per_launch = ms / iters;
+    *ms_per_launch = time_ms(c, 3, iters, [&] { gemm(c, a, b, e); }) / iters;
   });
 }
 
@@ -389,19 +467,7 @@ int alm_bench_gemm(alm_ctx* h, int M, int N, int K, int iters, float* ms_per_lau
     Epilogue e;
     e.out_f32 = c->ws.get<float>(static_cast<size_t>(M) * N);
     e.ldo = N;
-    for (int i = 0; i < 3; ++i) gemm(c, a, b, e);
-    cudaEvent_t e0, e1;
-    ALM_CHECK_CUDA(cudaEventCreate(&e0));
-    ALM_CHECK_CUDA(cudaEventCreate(&e1));
-    ALM_CHECK_CUDA(cudaEventRecord(e0, c->stream));
-    for (int i = 0; i < iters; ++i) gemm(c, a, b, e);
-    ALM_CHECK_CUDA(cudaEventRecord(e1, c->stream));
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-    float ms = 0;
-    ALM_CHECK_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    *ms_per_launch = ms / iters;
+    *ms_per_launch = time_ms(c, 3, iters, [&] { gemm(c, a, b, e); }) / iters;
   });
 }
 
@@ -487,14 +553,10 @@ int alm_stream_release(alm_ctx* h, void* consumer_stream) {
 
 int alm_comm_unique_id(void* id128) {
   if (!id128) return ALM_ERR_INVALID;
-  try {
+  return guarded_free([&] {
     comm_unique_id(id128);
     return ALM_OK;
-  } catch (const AlmError& e) {
-    return e.code;
-  } catch (...) {
-    return ALM_ERR_INVALID;
-  }
+  });
 }
 
 int alm_comm_init(alm_ctx* h, const void* id128, int rank, int world) {
@@ -514,29 +576,6 @@ int alm_gather_sequences(alm_ctx* h, const void* send, size_t bytes_per_rank, vo
 }
 
 // ------------------------------------------------------------------------------------------ pre-processing
-namespace {
-
-// device copies of the caller's uint8 HWC images (host pointers are staged into the workspace on the stream)
-std::vector<PreImage> stage_images(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths, int n) {
-  Ctx* c = &h->c;
-  c->ensure_ws();
-  std::vector<PreImage> imgs(static_cast<size_t>(n));
-  for (int i = 0; i < n; ++i) {
-    ALM_REQUIRE(rgb[i] && heights[i] > 0 && widths[i] > 0, ALM_ERR_INVALID, "image pointer / size");
-    const size_t bytes = static_cast<size_t>(heights[i]) * widths[i] * 3;
-    const uint8_t* d = rgb[i];
-    if (!is_device_ptr(d)) {
-      uint8_t* slot = c->ws.get<uint8_t>(bytes);
-      ALM_CHECK_CUDA(cudaMemcpyAsync(slot, rgb[i], bytes, cudaMemcpyHostToDevice, c->stream));
-      d = slot;
-    }
-    imgs[static_cast<size_t>(i)] = PreImage{d, heights[i], widths[i], 0, 0};
-  }
-  return imgs;
-}
-
-}  // namespace
-
 int alm_pre_omni_plan(const int* heights, const int* widths, int n, int test_min_size, int test_max_size, int* sizes,
                       int* Hmax, int* Wmax) {
   if (!heights || !widths || n < 0 || test_min_size <= 0 || !sizes || !Hmax || !Wmax) return ALM_ERR_INVALID;
@@ -552,11 +591,7 @@ int alm_pre_omni_plan(const int* heights, const int* widths, int n, int test_min
 }
 
 int alm_pre_coeffs(int in_size, int out_size, int filter, int* ksize, int* bounds, int* coefs, size_t cap_ints) {
-  try {
-    return pre_coeffs(in_size, out_size, filter, ksize, bounds, coefs, cap_ints);
-  } catch (...) {
-    return ALM_ERR_INVALID;
-  }
+  return guarded_free([&] { return pre_coeffs(in_size, out_size, filter, ksize, bounds, coefs, cap_ints); });
 }
 
 int alm_pre_omni_pages(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths, int n,
@@ -564,18 +599,15 @@ int alm_pre_omni_pages(alm_ctx* h, const uint8_t* const* rgb, const int* heights
   return guarded(h, [&] {
     ALM_REQUIRE(rgb && heights && widths && n > 0 && test_min_size > 0 && tensors && mask, ALM_ERR_INVALID,
                 "alm_pre_omni_pages arguments");
-    ALM_REQUIRE(is_device_ptr(tensors) && is_device_ptr(mask), ALM_ERR_INVALID, "outputs must be device buffers");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    std::vector<PreImage> imgs = stage_images(h, rgb, heights, widths, n);
-    int Hc = 0, Wc = 0;
-    for (auto& im : imgs) {
-      pre_omni_size(im.h, im.w, test_min_size, test_max_size, &im.oh, &im.ow);
-      Hc = std::max(Hc, im.oh);
-      Wc = std::max(Wc, im.ow);
-    }
-    pre_resize_batch(c, imgs, PRE_BILINEAR, true, tensors, Hc, Wc, mask);
+    with_pages(h, rgb, heights, widths, n, {tensors, mask}, "alm_pre_omni_pages", [&](std::vector<PreImage>& imgs) {
+      int Hc = 0, Wc = 0;
+      for (auto& im : imgs) {
+        pre_omni_size(im.h, im.w, test_min_size, test_max_size, &im.oh, &im.ow);
+        Hc = std::max(Hc, im.oh);
+        Wc = std::max(Wc, im.ow);
+      }
+      pre_resize_batch(&h->c, imgs, PRE_BILINEAR, true, tensors, Hc, Wc, mask);
+    });
   });
 }
 
@@ -584,13 +616,10 @@ int alm_pre_mgp_crops(alm_ctx* h, const uint8_t* const* rgb, const int* heights,
   return guarded(h, [&] {
     ALM_REQUIRE(rgb && heights && widths && n > 0 && imgH > 0 && imgW > 0 && out, ALM_ERR_INVALID,
                 "alm_pre_mgp_crops arguments");
-    ALM_REQUIRE(is_device_ptr(out), ALM_ERR_INVALID, "output must be a device buffer");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    std::vector<PreImage> imgs = stage_images(h, rgb, heights, widths, n);
-    for (auto& im : imgs) { im.oh = imgH; im.ow = imgW; }
-    pre_resize_batch(c, imgs, PRE_BICUBIC, false, out, imgH, imgW, nullptr);
+    with_pages(h, rgb, heights, widths, n, {out}, "alm_pre_mgp_crops", [&](std::vector<PreImage>& imgs) {
+      for (auto& im : imgs) { im.oh = imgH; im.ow = imgW; }
+      pre_resize_batch(&h->c, imgs, PRE_BICUBIC, false, out, imgH, imgW, nullptr);
+    });
   });
 }
 
@@ -598,7 +627,7 @@ int alm_pre_quad_plan(const int* heights, const int* widths, int n_pages, const 
                       float* ordered, float* corners, int* sizes, double* minv) {
   if (R == 0) return ALM_OK;
   if (!heights || !widths || n_pages < 1 || !quads || !page_index || R < 0) return ALM_ERR_INVALID;
-  try {
+  return guarded_free([&] {
     const std::vector<QuadPlan> plans = pre_quad_plan(heights, widths, n_pages, quads, page_index, R);
     for (int r = 0; r < R; ++r) {
       const QuadPlan& p = plans[static_cast<size_t>(r)];
@@ -608,11 +637,7 @@ int alm_pre_quad_plan(const int* heights, const int* widths, int n_pages, const 
       if (minv) std::copy(p.mi, p.mi + 9, minv + 9L * r);
     }
     return ALM_OK;
-  } catch (const AlmError& e) {
-    return e.code;
-  } catch (...) {
-    return ALM_ERR_INVALID;
-  }
+  });
 }
 
 int alm_pre_quad_crops(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths, int n_pages,
@@ -622,13 +647,9 @@ int alm_pre_quad_crops(alm_ctx* h, const uint8_t* const* rgb, const int* heights
     if (R == 0) return;
     ALM_REQUIRE(rgb && heights && widths && n_pages > 0 && quads && page_index && out, ALM_ERR_INVALID,
                 "alm_pre_quad_crops arguments");
-    ALM_REQUIRE(is_device_ptr(out), ALM_ERR_INVALID, "output must be a device buffer");
     const std::vector<QuadPlan> plans = pre_quad_plan(heights, widths, n_pages, quads, page_index, R);  // before any copy
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    std::vector<PreImage> pages = stage_images(h, rgb, heights, widths, n_pages);
-    pre_quad_crops(c, pages, plans, imgH, imgW, out);
+    with_pages(h, rgb, heights, widths, n_pages, {out}, "alm_pre_quad_crops",
+               [&](std::vector<PreImage>& pages) { pre_quad_crops(&h->c, pages, plans, imgH, imgW, out); });
   });
 }
 
@@ -636,7 +657,7 @@ int alm_pre_curve_plan(const int* heights, const int* widths, int n_pages, const
                        int R, double* ctrl, int* sizes) {
   if (R == 0) return ALM_OK;
   if (!heights || !widths || n_pages < 1 || !polys || !page_index || R < 0) return ALM_ERR_INVALID;
-  try {
+  return guarded_free([&] {
     const std::vector<CurvePlan> plans = pre_curve_plan(heights, widths, n_pages, polys, page_index, R);
     for (int r = 0; r < R; ++r) {
       const CurvePlan& p = plans[static_cast<size_t>(r)];
@@ -644,11 +665,7 @@ int alm_pre_curve_plan(const int* heights, const int* widths, int n_pages, const
       if (sizes) { sizes[2L * r] = p.cw; sizes[2L * r + 1] = p.ch; }
     }
     return ALM_OK;
-  } catch (const AlmError& e) {
-    return e.code;
-  } catch (...) {
-    return ALM_ERR_INVALID;
-  }
+  });
 }
 
 int alm_pre_curve_crops(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths, int n_pages,
@@ -658,13 +675,9 @@ int alm_pre_curve_crops(alm_ctx* h, const uint8_t* const* rgb, const int* height
     if (R == 0) return;
     ALM_REQUIRE(rgb && heights && widths && n_pages > 0 && polys && page_index && out, ALM_ERR_INVALID,
                 "alm_pre_curve_crops arguments");
-    ALM_REQUIRE(is_device_ptr(out), ALM_ERR_INVALID, "output must be a device buffer");
     const std::vector<CurvePlan> plans = pre_curve_plan(heights, widths, n_pages, polys, page_index, R);  // before any copy
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    std::vector<PreImage> pages = stage_images(h, rgb, heights, widths, n_pages);
-    pre_curve_crops(c, pages, plans, imgH, imgW, out);
+    with_pages(h, rgb, heights, widths, n_pages, {out}, "alm_pre_curve_crops",
+               [&](std::vector<PreImage>& pages) { pre_curve_crops(&h->c, pages, plans, imgH, imgW, out); });
   });
 }
 
@@ -691,21 +704,12 @@ int alm_pre_line_crops(alm_ctx* h, const uint8_t* const* rgb, const int* heights
     if (R == 0) return;
     ALM_REQUIRE(rgb && heights && widths && n_pages > 0 && regions && page_index && out, ALM_ERR_INVALID,
                 "alm_pre_line_crops arguments");
-    ALM_REQUIRE(is_device_ptr(out), ALM_ERR_INVALID, "output must be a device buffer");
-    Ctx* c = &h->c;
-    if (kind == ALM_BOX_QUAD) {
-      const std::vector<QuadPlan> plans = pre_quad_plan(heights, widths, n_pages, regions, page_index, R);
-      c->ensure_ws();
-      ArenaScope arena_scope(c->ws);
-      std::vector<PreImage> pages = stage_images(h, rgb, heights, widths, n_pages);
-      pre_line_crops(c, pages, plans, out);
-    } else {
-      const std::vector<CurvePlan> plans = pre_curve_plan(heights, widths, n_pages, regions, page_index, R);
-      c->ensure_ws();
-      ArenaScope arena_scope(c->ws);
-      std::vector<PreImage> pages = stage_images(h, rgb, heights, widths, n_pages);
-      pre_line_crops(c, pages, plans, out);
-    }
+    auto crops = [&](const auto& plans) {  // plans before any copy
+      with_pages(h, rgb, heights, widths, n_pages, {out}, "alm_pre_line_crops",
+                 [&](std::vector<PreImage>& pages) { pre_line_crops(&h->c, pages, plans, out); });
+    };
+    if (kind == ALM_BOX_QUAD) crops(pre_quad_plan(heights, widths, n_pages, regions, page_index, R));
+    else crops(pre_curve_plan(heights, widths, n_pages, regions, page_index, R));
   });
 }
 
@@ -750,30 +754,28 @@ int alm_pre_omni_tiles(alm_ctx* h, const uint8_t* const* rgb, const int* heights
     ALM_REQUIRE(rgb && pages_ok(heights, widths, n_pages) && tile_core::valid_layout(tile, overlap) &&
                     test_min_size > 0 && tensors && mask,
                 ALM_ERR_INVALID, "alm_pre_omni_tiles arguments");
-    ALM_REQUIRE(is_device_ptr(tensors) && is_device_ptr(mask), ALM_ERR_INVALID, "outputs must be device buffers");
     const std::vector<tile_core::Tile> tiles = page_tiles(heights, widths, n_pages, tile, overlap, 0.0);
     ALM_REQUIRE(first >= 0 && count >= 1 && static_cast<long>(first) + count <= static_cast<long>(tiles.size()),
                 ALM_ERR_INVALID, "alm_pre_omni_tiles: tile range outside the plan");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    std::vector<PreImage> pages = stage_images(h, rgb, heights, widths, n_pages);
-    std::vector<PreImage> imgs(static_cast<size_t>(count));
-    int Hc = 0, Wc = 0;
-    for (int k = 0; k < count; ++k) {  // one 2D copy per tile into a contiguous [h][w][3] buffer
-      const tile_core::Tile& t = tiles[static_cast<size_t>(first + k)];
-      const PreImage& pg = pages[static_cast<size_t>(t.page)];
-      uint8_t* dst = c->ws.get<uint8_t>(static_cast<size_t>(t.h) * t.w * 3);
-      const uint8_t* src = pg.dev_rgb + (static_cast<size_t>(t.y0) * pg.w + t.x0) * 3;
-      ALM_CHECK_CUDA(cudaMemcpy2DAsync(dst, static_cast<size_t>(t.w) * 3, src, static_cast<size_t>(pg.w) * 3,
-                                       static_cast<size_t>(t.w) * 3, t.h, cudaMemcpyDeviceToDevice, c->stream));
-      PreImage& im = imgs[static_cast<size_t>(k)];
-      im = PreImage{dst, t.h, t.w, 0, 0};
-      pre_omni_size(im.h, im.w, test_min_size, test_max_size, &im.oh, &im.ow);
-      Hc = std::max(Hc, im.oh);
-      Wc = std::max(Wc, im.ow);
-    }
-    pre_resize_batch(c, imgs, PRE_BILINEAR, true, tensors, Hc, Wc, mask);
+    with_pages(h, rgb, heights, widths, n_pages, {tensors, mask}, "alm_pre_omni_tiles", [&](std::vector<PreImage>& pages) {
+      Ctx* c = &h->c;
+      std::vector<PreImage> imgs(static_cast<size_t>(count));
+      int Hc = 0, Wc = 0;
+      for (int k = 0; k < count; ++k) {  // one 2D copy per tile into a contiguous [h][w][3] buffer
+        const tile_core::Tile& t = tiles[static_cast<size_t>(first + k)];
+        const PreImage& pg = pages[static_cast<size_t>(t.page)];
+        uint8_t* dst = c->ws.get<uint8_t>(static_cast<size_t>(t.h) * t.w * 3);
+        const uint8_t* src = pg.dev_rgb + (static_cast<size_t>(t.y0) * pg.w + t.x0) * 3;
+        ALM_CHECK_CUDA(cudaMemcpy2DAsync(dst, static_cast<size_t>(t.w) * 3, src, static_cast<size_t>(pg.w) * 3,
+                                         static_cast<size_t>(t.w) * 3, t.h, cudaMemcpyDeviceToDevice, c->stream));
+        PreImage& im = imgs[static_cast<size_t>(k)];
+        im = PreImage{dst, t.h, t.w, 0, 0};
+        pre_omni_size(im.h, im.w, test_min_size, test_max_size, &im.oh, &im.ow);
+        Hc = std::max(Hc, im.oh);
+        Wc = std::max(Wc, im.ow);
+      }
+      pre_resize_batch(c, imgs, PRE_BILINEAR, true, tensors, Hc, Wc, mask);
+    });
   });
 }
 
@@ -1046,13 +1048,49 @@ int alm_omni_decode_logits(alm_ctx* h, int image, int kind, const int64_t* seq, 
 }
 
 // ------------------------------------------------------------------------------------------ MGP-STR
+namespace {
+
+// the caller's [B][3][32][128] crop batch on the device
+const float* stage_crops(alm_ctx* h, const float* img, int B) {
+  return static_cast<const float*>(
+      stage_input(h, img, static_cast<size_t>(B) * 3 * 32 * 128 * sizeof(float), &h->dev_in, &h->dev_in_bytes));
+}
+
+// one attention-map plane per A^3 head of the loaded checkpoint
+void require_a3_heads(alm_ctx* h, int n_heads, const char* fn) {
+  int n_a3 = 0;
+  mgp_info(h->c.mgp, nullptr, nullptr, nullptr, &n_a3, nullptr);
+  ALM_REQUIRE(n_heads == n_a3, ALM_ERR_INVALID,
+              std::string(fn) + ": " + std::to_string(n_heads) + " head planes, but the checkpoint has " +
+                  std::to_string(n_a3) + " A^3 heads");
+}
+
+// the page geometry of R quad (9 values each) or curve (16 values each) regions, with their crop sizes
+std::vector<box_core::BoxGeom> region_geom(int kind, int R, const int* sizes, const double* geom, const char* fn) {
+  const int nv = kind == ALM_BOX_QUAD ? 9 : 16;
+  std::vector<box_core::BoxGeom> g(static_cast<size_t>(R));
+  for (int r = 0; r < R; ++r) {
+    box_core::BoxGeom& d = g[static_cast<size_t>(r)];
+    d.cw = sizes[2L * r];
+    d.ch = sizes[2L * r + 1];
+    ALM_REQUIRE(d.cw >= 1 && d.ch >= 1, ALM_ERR_INVALID,
+                std::string(fn) + ": region " + std::to_string(r) + ": crop size");
+    for (int i = 0; i < nv; ++i) {
+      d.g[i] = geom[static_cast<long>(nv) * r + i];
+      ALM_REQUIRE(isfinite(d.g[i]), ALM_ERR_INVALID,
+                  std::string(fn) + ": region " + std::to_string(r) + ": non-finite geometry");
+    }
+  }
+  return g;
+}
+
+}  // namespace
+
 int alm_mgpstr_forward(alm_ctx* h, const float* img, int B, float* attn, float* char_logits, float* bpe_logits,
                        float* wp_logits, int32_t* ids, float* prob) {
   return guarded(h, [&] {
     ALM_REQUIRE(img && B > 0, ALM_ERR_INVALID, "alm_mgpstr_forward arguments");
-    const float* dimg = static_cast<const float*>(
-        stage_input(h, img, static_cast<size_t>(B) * 3 * 32 * 128 * sizeof(float), &h->dev_in, &h->dev_in_bytes));
-    mgp_forward(&h->c, dimg, B, attn, char_logits, bpe_logits, wp_logits, ids, prob);
+    mgp_forward(&h->c, stage_crops(h, img, B), B, attn, char_logits, bpe_logits, wp_logits, ids, prob);
   });
 }
 
@@ -1061,9 +1099,7 @@ int alm_mgpstr_topk(alm_ctx* h, const float* img, int B, int k, int32_t* ids, fl
     ALM_REQUIRE(img && B > 0 && ids && probs, ALM_ERR_INVALID, "alm_mgpstr_topk arguments");
     ALM_REQUIRE(k >= 1 && k <= ALM_MAX_CANDIDATES, ALM_ERR_INVALID, "alm_mgpstr_topk: k must be 1..8");
     ALM_REQUIRE(h->c.mgp != nullptr, ALM_ERR_STATE, "alm_mgpstr_topk needs an MGP-STR checkpoint in this context");
-    const float* dimg = static_cast<const float*>(
-        stage_input(h, img, static_cast<size_t>(B) * 3 * 32 * 128 * sizeof(float), &h->dev_in, &h->dev_in_bytes));
-    mgp_forward(&h->c, dimg, B, nullptr, nullptr, nullptr, nullptr, ids, probs, k);
+    mgp_forward(&h->c, stage_crops(h, img, B), B, nullptr, nullptr, nullptr, nullptr, ids, probs, k);
   });
 }
 
@@ -1075,11 +1111,7 @@ int alm_mgpstr_forward_boxes(alm_ctx* h, const float* img, int B, int k, int geo
                 "alm_mgpstr_forward_boxes arguments");
     ALM_REQUIRE(k >= 0 && k <= ALM_MAX_CANDIDATES, ALM_ERR_INVALID, "alm_mgpstr_forward_boxes: k must be 0..8");
     ALM_REQUIRE(h->c.mgp != nullptr, ALM_ERR_STATE, "alm_mgpstr_forward_boxes needs an MGP-STR checkpoint in this context");
-    int n_a3 = 0;
-    mgp_info(h->c.mgp, nullptr, nullptr, nullptr, &n_a3, nullptr);
-    ALM_REQUIRE(n_heads == n_a3, ALM_ERR_INVALID,
-                "alm_mgpstr_forward_boxes: " + std::to_string(n_heads) + " head planes, but the checkpoint has " +
-                    std::to_string(n_a3) + " A^3 heads");
+    require_a3_heads(h, n_heads, "alm_mgpstr_forward_boxes");
     ALM_REQUIRE(geom_kind == ALM_BOX_CROP || geom_kind == ALM_BOX_QUAD || geom_kind == ALM_BOX_CURVE, ALM_ERR_INVALID,
                 "alm_mgpstr_forward_boxes: geom_kind must be 0 (crop), 1 (quad) or 2 (curve)");
     ALM_REQUIRE(n_geom == B, ALM_ERR_INVALID,
@@ -1088,25 +1120,10 @@ int alm_mgpstr_forward_boxes(alm_ctx* h, const float* img, int B, int k, int geo
     std::vector<box_core::BoxGeom> g;
     if (geom_kind != ALM_BOX_CROP) {
       ALM_REQUIRE(sizes && geom, ALM_ERR_INVALID, "alm_mgpstr_forward_boxes: quad / curve geometry needs sizes and geom");
-      const int nv = geom_kind == ALM_BOX_QUAD ? 9 : 16;
-      g.resize(static_cast<size_t>(B));
-      for (int r = 0; r < B; ++r) {
-        box_core::BoxGeom& d = g[static_cast<size_t>(r)];
-        d = box_core::BoxGeom{};
-        d.cw = sizes[2L * r];
-        d.ch = sizes[2L * r + 1];
-        ALM_REQUIRE(d.cw >= 1 && d.ch >= 1, ALM_ERR_INVALID, "alm_mgpstr_forward_boxes: region " + std::to_string(r) + ": crop size");
-        for (int i = 0; i < nv; ++i) {
-          d.g[i] = geom[static_cast<long>(nv) * r + i];
-          ALM_REQUIRE(isfinite(d.g[i]), ALM_ERR_INVALID,
-                      "alm_mgpstr_forward_boxes: region " + std::to_string(r) + ": non-finite geometry");
-        }
-      }
+      g = region_geom(geom_kind, B, sizes, geom, "alm_mgpstr_forward_boxes");
     }
-    const float* dimg = static_cast<const float*>(
-        stage_input(h, img, static_cast<size_t>(B) * 3 * 32 * 128 * sizeof(float), &h->dev_in, &h->dev_in_bytes));
     const MgpBoxes mb{geom_kind, g.empty() ? nullptr : g.data(), n, boxes, centres};
-    mgp_forward(&h->c, dimg, B, nullptr, nullptr, nullptr, nullptr, ids, probs, k, &mb);
+    mgp_forward(&h->c, stage_crops(h, img, B), B, nullptr, nullptr, nullptr, nullptr, ids, probs, k, &mb);
   });
 }
 
@@ -1117,31 +1134,17 @@ int alm_mgpstr_forward_lines(alm_ctx* h, const float* img, int B, int R, const i
     ALM_REQUIRE(img && B > 0 && R > 0 && windows && sizes && geom && ids && probs && n && boxes && centres,
                 ALM_ERR_INVALID, "alm_mgpstr_forward_lines arguments");
     ALM_REQUIRE(h->c.mgp != nullptr, ALM_ERR_STATE, "alm_mgpstr_forward_lines needs an MGP-STR checkpoint in this context");
-    int n_a3 = 0;
-    mgp_info(h->c.mgp, nullptr, nullptr, nullptr, &n_a3, nullptr);
-    ALM_REQUIRE(n_heads == n_a3, ALM_ERR_INVALID,
-                "alm_mgpstr_forward_lines: " + std::to_string(n_heads) + " head planes, but the checkpoint has " +
-                    std::to_string(n_a3) + " A^3 heads");
+    require_a3_heads(h, n_heads, "alm_mgpstr_forward_lines");
     ALM_REQUIRE(kind == ALM_BOX_QUAD || kind == ALM_BOX_CURVE, ALM_ERR_INVALID,
                 "alm_mgpstr_forward_lines: kind must be 1 (quad) or 2 (curve)");
-    const int nv = kind == ALM_BOX_QUAD ? 9 : 16;
-    std::vector<box_core::BoxGeom> g(static_cast<size_t>(R));
+    const std::vector<box_core::BoxGeom> g = region_geom(kind, R, sizes, geom, "alm_mgpstr_forward_lines");
     std::vector<line_core::LineWin> win;
     std::vector<int> wstart(static_cast<size_t>(R) + 1, 0);
     for (int r = 0; r < R; ++r) {
-      const std::string who = "alm_mgpstr_forward_lines: region " + std::to_string(r);
-      box_core::BoxGeom& d = g[static_cast<size_t>(r)];
-      d = box_core::BoxGeom{};
-      d.cw = sizes[2L * r];
-      d.ch = sizes[2L * r + 1];
-      ALM_REQUIRE(d.cw >= 1 && d.ch >= 1, ALM_ERR_INVALID, who + ": crop size");
-      for (int i = 0; i < nv; ++i) {
-        d.g[i] = geom[static_cast<long>(nv) * r + i];
-        ALM_REQUIRE(isfinite(d.g[i]), ALM_ERR_INVALID, who + ": non-finite geometry");
-      }
-      const line_core::Windows w = line_core::line_windows(d.cw, d.ch);
+      const line_core::Windows w = line_core::line_windows(g[static_cast<size_t>(r)].cw, g[static_cast<size_t>(r)].ch);
       ALM_REQUIRE(windows[r] == w.n, ALM_ERR_INVALID,
-                  who + ": " + std::to_string(windows[r]) + " windows, but its crop has " + std::to_string(w.n));
+                  "alm_mgpstr_forward_lines: region " + std::to_string(r) + ": " + std::to_string(windows[r]) +
+                      " windows, but its crop has " + std::to_string(w.n));
       ALM_REQUIRE(wstart[static_cast<size_t>(r)] + w.n <= B, ALM_ERR_INVALID,
                   "alm_mgpstr_forward_lines: the window counts exceed B = " + std::to_string(B));
       for (int i = 0; i < w.n; ++i) win.push_back(line_core::LineWin{r, w.x0[i], w.wn, 0});
@@ -1154,10 +1157,8 @@ int alm_mgpstr_forward_lines(alm_ctx* h, const float* img, int B, int R, const i
     c->ensure_ws();
     ALM_REQUIRE(mgp_lines_bytes(B, R) <= c->ws.cap, ALM_ERR_INVALID,
                 "alm_mgpstr_forward_lines: " + std::to_string(B) + " windows do not fit in the workspace");
-    const float* dimg = static_cast<const float*>(
-        stage_input(h, img, static_cast<size_t>(B) * 3 * 32 * 128 * sizeof(float), &h->dev_in, &h->dev_in_bytes));
     const MgpLines ml{kind, R, g.data(), win.data(), wstart.data(), ids, probs, n, boxes, centres};
-    mgp_forward(c, dimg, B, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, &ml);
+    mgp_forward(c, stage_crops(h, img, B), B, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, &ml);
   });
 }
 
@@ -1169,36 +1170,64 @@ int alm_mgpstr_info(alm_ctx* h, int* dim, int* depth, int* heads, int* n_a3, int
 }
 
 // ------------------------------------------------------------------------------------------ unit ops
+namespace {
+
+// fp32 x [nb][rows][K] as a split-bf16 operand in the workspace, its rows zero-padded to a multiple of 8 elements
+Operand split_operand(Ctx* c, const float* x, int rows, int K, int nb) {
+  const int Kp = (K + 7) & ~7;
+  const size_t n = static_cast<size_t>(nb) * rows * Kp;
+  bf16* hi = c->ws.get<bf16>(n);
+  bf16* lo = c->ws.get<bf16>(n);
+  if (Kp != K)
+    for (bf16* p : {hi, lo}) ALM_CHECK_CUDA(cudaMemsetAsync(p, 0, n * 2, c->stream));
+  split_rows(c, x, K, static_cast<long>(nb) * rows, K, hi, lo, Kp);
+  Operand o;
+  o.hi = hi; o.lo = lo; o.rows = rows; o.K = K; o.ld = Kp; o.nb0 = nb; o.bs0 = static_cast<long>(rows) * Kp;
+  return o;
+}
+
+// A [batch][M][K] times W [w_batch][N][K]^T, both fp32, through the engine's epilogue e
+void op_gemm(Ctx* c, const float* A, const float* W, int M, int N, int K, int batch, int w_batch, const Epilogue& e,
+             const char* fn) {
+  ALM_REQUIRE(K % 4 == 0, ALM_ERR_UNSUPPORTED, std::string(fn) + ": K must be a multiple of 4");
+  c->ensure_ws();
+  ArenaScope arena_scope(c->ws);
+  const Operand a = split_operand(c, A, M, K, batch), b = split_operand(c, W, N, K, w_batch);
+  gemm(c, a, b, e);  // its own checks reject the combinations the engine cannot run
+  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+}
+
+// the engine's epilogue for the caller's, once its values and pointers are checked
+Epilogue epilogue(const alm_gemm_epilogue& x, const char* fn) {
+  ALM_REQUIRE(x.ldo > 0 && x.obs0 >= 0 && x.obs1 >= 0 && x.bias_mode >= BIAS_NONE && x.bias_mode <= BIAS_ROW &&
+                  (x.bias != nullptr) == (x.bias_mode != BIAS_NONE) && x.act >= ACT_NONE && x.act <= ACT_RELU &&
+                  (!x.out_lo || x.out_hi) && (!x.resid || x.ldr > 0) && x.col_group >= 0,
+              ALM_ERR_INVALID, std::string(fn) + " epilogue");
+  require_device({x.out_f32, x.out_hi, x.out_lo, x.bias, x.resid, x.resid_map, x.out_map}, 1, fn);
+  Epilogue e;
+  e.out_f32 = x.out_f32;
+  e.out_hi = static_cast<bf16*>(x.out_hi);
+  e.out_lo = static_cast<bf16*>(x.out_lo);
+  e.ldo = x.ldo; e.obs0 = x.obs0; e.obs1 = x.obs1;
+  e.col_group = x.col_group; e.col_group_stride = x.col_group_stride;
+  e.bias = x.bias; e.bias_mode = x.bias_mode; e.bias_bs0 = x.bias_bs0;
+  e.resid = x.resid; e.ldr = x.resid ? x.ldr : 0; e.rbs0 = x.resid ? x.rbs0 : 0; e.rbs1 = x.resid ? x.rbs1 : 0;
+  e.out_map = x.out_map; e.resid_map = x.resid_map;
+  e.act = x.act; e.alpha = x.alpha;
+  return e;
+}
+
+}  // namespace
+
 int alm_op_linear(alm_ctx* h, const float* A, const float* W, const float* bias, float* C, int M, int N, int K, int act,
                   int batch) {
   return guarded(h, [&] {
     ALM_REQUIRE(A && W && C && M > 0 && N > 0 && K > 0 && batch > 0, ALM_ERR_INVALID, "alm_op_linear arguments");
-    ALM_REQUIRE(is_device_ptr(A) && is_device_ptr(W) && is_device_ptr(C), ALM_ERR_INVALID, "device pointers required");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    const int Kp = (K + 7) & ~7;
-    bf16* ah = c->ws.get<bf16>(static_cast<size_t>(batch) * M * Kp);
-    bf16* al = c->ws.get<bf16>(static_cast<size_t>(batch) * M * Kp);
-    bf16* wh = c->ws.get<bf16>(static_cast<size_t>(batch) * N * Kp);
-    bf16* wl = c->ws.get<bf16>(static_cast<size_t>(batch) * N * Kp);
-    if (Kp != K) {
-      ALM_CHECK_CUDA(cudaMemsetAsync(ah, 0, static_cast<size_t>(batch) * M * Kp * 2, c->stream));
-      ALM_CHECK_CUDA(cudaMemsetAsync(al, 0, static_cast<size_t>(batch) * M * Kp * 2, c->stream));
-      ALM_CHECK_CUDA(cudaMemsetAsync(wh, 0, static_cast<size_t>(batch) * N * Kp * 2, c->stream));
-      ALM_CHECK_CUDA(cudaMemsetAsync(wl, 0, static_cast<size_t>(batch) * N * Kp * 2, c->stream));
-    }
-    ALM_REQUIRE(K % 4 == 0, ALM_ERR_UNSUPPORTED, "alm_op_linear: K must be a multiple of 4");
-    split_rows(c, A, K, static_cast<long>(batch) * M, K, ah, al, Kp);
-    split_rows(c, W, K, static_cast<long>(batch) * N, K, wh, wl, Kp);
-    Operand a, b;
-    a.hi = ah; a.lo = al; a.rows = M; a.K = K; a.ld = Kp; a.nb0 = batch; a.bs0 = static_cast<long>(M) * Kp;
-    b.hi = wh; b.lo = wl; b.rows = N; b.K = K; b.ld = Kp; b.nb0 = batch; b.bs0 = static_cast<long>(N) * Kp;
+    require_device({A, W, C, bias}, 1, "alm_op_linear");
     Epilogue e;
     e.out_f32 = C; e.ldo = N; e.obs0 = static_cast<long>(M) * N;
     e.bias = bias; e.bias_mode = bias ? BIAS_COL : BIAS_NONE; e.act = act;
-    gemm(c, a, b, e);
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+    op_gemm(&h->c, A, W, M, N, K, batch, batch, e, "alm_op_linear");
   });
 }
 
@@ -1207,48 +1236,12 @@ int alm_op_gemm(alm_ctx* h, const float* A, const float* W, int M, int N, int K,
                 float alpha, int act, const float* resid, long ldr, long rbs0, const int* resid_map, const int* out_map,
                 int col_group, long col_group_stride) {
   return guarded(h, [&] {
-    ALM_REQUIRE(A && W && M > 0 && N > 0 && K > 0 && batch > 0 && (w_batch == 1 || w_batch == batch) && ldo > 0 &&
-                    obs0 >= 0 && bias_mode >= BIAS_NONE && bias_mode <= BIAS_ROW && (bias != nullptr) == (bias_mode != BIAS_NONE) &&
-                    act >= ACT_NONE && act <= ACT_RELU && (!out_lo || out_hi) && (!resid || ldr > 0) && col_group >= 0,
-                ALM_ERR_INVALID, "alm_op_gemm arguments");
-    for (const void* ptr : {static_cast<const void*>(A), static_cast<const void*>(W), static_cast<const void*>(out_f32),
-                            static_cast<const void*>(out_hi), static_cast<const void*>(out_lo),
-                            static_cast<const void*>(bias), static_cast<const void*>(resid),
-                            static_cast<const void*>(resid_map), static_cast<const void*>(out_map)})
-      ALM_REQUIRE(!ptr || is_device_ptr(ptr), ALM_ERR_INVALID, "device pointers required");
-    ALM_REQUIRE(K % 4 == 0, ALM_ERR_UNSUPPORTED, "alm_op_gemm: K must be a multiple of 4");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    const int Kp = (K + 7) & ~7;
-    const size_t na = static_cast<size_t>(batch) * M * Kp, nw = static_cast<size_t>(w_batch) * N * Kp;
-    bf16* ah = c->ws.get<bf16>(na);
-    bf16* al = c->ws.get<bf16>(na);
-    bf16* wh = c->ws.get<bf16>(nw);
-    bf16* wl = c->ws.get<bf16>(nw);
-    if (Kp != K) {
-      ALM_CHECK_CUDA(cudaMemsetAsync(ah, 0, na * 2, c->stream));
-      ALM_CHECK_CUDA(cudaMemsetAsync(al, 0, na * 2, c->stream));
-      ALM_CHECK_CUDA(cudaMemsetAsync(wh, 0, nw * 2, c->stream));
-      ALM_CHECK_CUDA(cudaMemsetAsync(wl, 0, nw * 2, c->stream));
-    }
-    split_rows(c, A, K, static_cast<long>(batch) * M, K, ah, al, Kp);
-    split_rows(c, W, K, static_cast<long>(w_batch) * N, K, wh, wl, Kp);
-    Operand a, b;
-    a.hi = ah; a.lo = al; a.rows = M; a.K = K; a.ld = Kp; a.nb0 = batch; a.bs0 = static_cast<long>(M) * Kp;
-    b.hi = wh; b.lo = wl; b.rows = N; b.K = K; b.ld = Kp; b.nb0 = w_batch; b.bs0 = w_batch > 1 ? static_cast<long>(N) * Kp : 0;
-    Epilogue e;
-    e.out_f32 = out_f32;
-    e.out_hi = static_cast<bf16*>(out_hi);
-    e.out_lo = static_cast<bf16*>(out_lo);
-    e.ldo = ldo; e.obs0 = obs0;
-    e.col_group = col_group; e.col_group_stride = col_group_stride;
-    e.bias = bias; e.bias_mode = bias_mode; e.bias_bs0 = bias_bs0;
-    e.resid = resid; e.ldr = resid ? ldr : 0; e.rbs0 = resid ? rbs0 : 0;
-    e.resid_map = resid_map; e.out_map = out_map;
-    e.act = act; e.alpha = alpha;
-    gemm(c, a, b, e);  // its own checks reject the combinations the engine cannot run
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+    ALM_REQUIRE(A && W && M > 0 && N > 0 && K > 0 && batch > 0 && (w_batch == 1 || w_batch == batch), ALM_ERR_INVALID,
+                "alm_op_gemm arguments");
+    require_device({A, W}, 1, "alm_op_gemm");
+    const alm_gemm_epilogue x{out_f32,   out_hi,   out_lo, ldo, obs0, /*obs1*/ 0, col_group, col_group_stride, bias,
+                              bias_mode, bias_bs0, resid,  ldr, rbs0, /*rbs1*/ 0, out_map, resid_map, act, alpha};
+    op_gemm(&h->c, A, W, M, N, K, batch, w_batch, epilogue(x, "alm_op_gemm"), "alm_op_gemm");
   });
 }
 
@@ -1259,40 +1252,20 @@ int alm_op_gemm_planes(alm_ctx* h, const alm_gemm_operand* A, const alm_gemm_ope
     for (int i = 0; i < 2; ++i) {
       const alm_gemm_operand& s = i == 0 ? *A : *B;
       const std::string who = i == 0 ? "alm_op_gemm_planes: A" : "alm_op_gemm_planes: B";
-      ALM_REQUIRE(s.hi && is_device_ptr(s.hi) && (!s.lo || is_device_ptr(s.lo)), ALM_ERR_INVALID,
-                  who + " planes must be device pointers");
+      ALM_REQUIRE(s.hi, ALM_ERR_INVALID, who + " hi plane is null");
+      require_device({s.hi, s.lo}, 16, who + " planes");
       ALM_REQUIRE(s.rows > 0 && s.K > 0 && s.ld >= s.K && s.nb0 > 0 && s.nb1 > 0 && s.bs0 >= 0 && s.bs1 >= 0,
                   ALM_ERR_INVALID, who + " extents");
       ALM_REQUIRE(s.ld % 8 == 0 && s.bs0 % 8 == 0 && s.bs1 % 8 == 0, ALM_ERR_INVALID,
                   who + " strides must be multiples of 8 elements");
-      const uintptr_t hi = reinterpret_cast<uintptr_t>(s.hi), lo = reinterpret_cast<uintptr_t>(s.lo);
-      ALM_REQUIRE(hi % 16 == 0 && lo % 16 == 0, ALM_ERR_INVALID, who + " planes must be 16-byte aligned");
-      ALM_REQUIRE(!s.lo || lo > hi, ALM_ERR_INVALID, who + " lo plane must lie after the hi plane");
+      ALM_REQUIRE(!s.lo || reinterpret_cast<uintptr_t>(s.lo) > reinterpret_cast<uintptr_t>(s.hi), ALM_ERR_INVALID,
+                  who + " lo plane must lie after the hi plane");
       op[i].hi = static_cast<const bf16*>(s.hi);
       op[i].lo = static_cast<const bf16*>(s.lo);
       op[i].rows = s.rows; op[i].K = s.K; op[i].ld = s.ld;
       op[i].nb0 = s.nb0; op[i].nb1 = s.nb1; op[i].bs0 = s.bs0; op[i].bs1 = s.bs1;
     }
-    const alm_gemm_epilogue& x = *epi;
-    ALM_REQUIRE(x.ldo > 0 && x.obs0 >= 0 && x.obs1 >= 0 && x.bias_mode >= BIAS_NONE && x.bias_mode <= BIAS_ROW &&
-                    (x.bias != nullptr) == (x.bias_mode != BIAS_NONE) && x.act >= ACT_NONE && x.act <= ACT_RELU &&
-                    (!x.out_lo || x.out_hi) && (!x.resid || x.ldr > 0) && x.col_group >= 0,
-                ALM_ERR_INVALID, "alm_op_gemm_planes epilogue");
-    for (const void* ptr : {static_cast<const void*>(x.out_f32), static_cast<const void*>(x.out_hi),
-                            static_cast<const void*>(x.out_lo), static_cast<const void*>(x.bias),
-                            static_cast<const void*>(x.resid), static_cast<const void*>(x.resid_map),
-                            static_cast<const void*>(x.out_map)})
-      ALM_REQUIRE(!ptr || is_device_ptr(ptr), ALM_ERR_INVALID, "device pointers required");
-    Epilogue e;
-    e.out_f32 = x.out_f32;
-    e.out_hi = static_cast<bf16*>(x.out_hi);
-    e.out_lo = static_cast<bf16*>(x.out_lo);
-    e.ldo = x.ldo; e.obs0 = x.obs0; e.obs1 = x.obs1;
-    e.col_group = x.col_group; e.col_group_stride = x.col_group_stride;
-    e.bias = x.bias; e.bias_mode = x.bias_mode; e.bias_bs0 = x.bias_bs0;
-    e.resid = x.resid; e.ldr = x.resid ? x.ldr : 0; e.rbs0 = x.resid ? x.rbs0 : 0; e.rbs1 = x.resid ? x.rbs1 : 0;
-    e.out_map = x.out_map; e.resid_map = x.resid_map;
-    e.act = x.act; e.alpha = x.alpha;
+    const Epilogue e = epilogue(*epi, "alm_op_gemm_planes");
     Ctx* c = &h->c;
     gemm(c, op[0], op[1], e);  // its own checks reject the batch extents and epilogues the engine cannot run
     ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
@@ -1302,7 +1275,7 @@ int alm_op_gemm_planes(alm_ctx* h, const alm_gemm_operand* A, const alm_gemm_ope
 int alm_op_attention(alm_ctx* h, const float* qkv, float* out, int B, int T, int H) {
   return guarded(h, [&] {
     ALM_REQUIRE(qkv && out && B > 0 && T > 0 && H > 0, ALM_ERR_INVALID, "alm_op_attention arguments");
-    ALM_REQUIRE(is_device_ptr(qkv) && is_device_ptr(out), ALM_ERR_INVALID, "device pointers required");
+    require_device({qkv, out}, 1, "alm_op_attention");
     Ctx* c = &h->c;
     c->ensure_ws();
     ArenaScope arena_scope(c->ws);
@@ -1320,6 +1293,7 @@ int alm_op_layernorm(alm_ctx* h, const float* x, const float* gamma, const float
                      int C) {
   return guarded(h, [&] {
     ALM_REQUIRE(x && gamma && beta && y && rows > 0, ALM_ERR_INVALID, "alm_op_layernorm arguments");
+    require_device({x, gamma, beta, y}, 1, "alm_op_layernorm");
     gather_ln(&h->c, x, C, nullptr, 1, C, rows, gamma, beta, eps, false, nullptr, 0, y, C, nullptr, nullptr, 0, nullptr,
               nullptr);
     ALM_CHECK_CUDA(cudaStreamSynchronize(h->c.stream));
@@ -1327,13 +1301,6 @@ int alm_op_layernorm(alm_ctx* h, const float* x, const float* gamma, const float
 }
 
 namespace {
-
-// every non-null pointer is device memory aligned to `align` bytes
-void require_device(std::initializer_list<const void*> ptrs, size_t align, const char* what) {
-  for (const void* p : ptrs)
-    ALM_REQUIRE(!p || (is_device_ptr(p) && reinterpret_cast<uintptr_t>(p) % align == 0), ALM_ERR_INVALID,
-                std::string(what) + ": device pointers aligned to " + std::to_string(align) + " bytes required");
-}
 
 void op_window_attention(alm_ctx* h, const float* qkv, const float* bias_table, float* out_f32, void* out_hi,
                          void* out_lo, int B, int nWh, int nWw, int C, int heads, int shift) {
@@ -1493,25 +1460,17 @@ void op_cross_attention(alm_ctx* h, const float* q, const float* k, const float*
                     M > 0 && dl >= 0 && dl < 12 && (q_split == 0 || q_split == 1) && launches >= 1,
                 ALM_ERR_INVALID, "alm_op_cross_attention arguments");
     ALM_REQUIRE(q_split == 1 || Ncap <= 16, ALM_ERR_INVALID, "alm_op_cross_attention: fp32 queries need Ncap <= 16");
-    ALM_REQUIRE(is_device_ptr(q) && is_device_ptr(k) && is_device_ptr(v) && is_device_ptr(out) && (!kpm || is_device_ptr(kpm)),
-                ALM_ERR_INVALID, "device pointers required");
+    require_device({q, k, v, out, kpm}, 1, "alm_op_cross_attention");
     Ctx* c = &h->c;
     const int impl = c->xattn_impl;
     ALM_REQUIRE(impl != 1 || Ncap == 1, ALM_ERR_UNSUPPORTED,
                 "alm_op_cross_attention: xattn_impl 1 has a fused kernel for one query per image only");
     c->ensure_ws();
     ArenaScope arena_scope(c->ws);
-    // the model's caches, every element this call must not read poisoned with NaN (0xffff)
-    const long slices = static_cast<long>(nimg_total) * 96;
-    const size_t cache = static_cast<size_t>(slices) * M * 64;
-    bf16* kh = c->ws.get<bf16>(cache); bf16* kl = c->ws.get<bf16>(cache);
-    bf16* vh = c->ws.get<bf16>(cache); bf16* vl = c->ws.get<bf16>(cache);
-    for (bf16* p : {kh, kl, vh, vl}) ALM_CHECK_CUDA(cudaMemsetAsync(p, 0xff, cache * 2, c->stream));
-    const long koff = (static_cast<long>(img0) * 96 + dl * 8) * M * 64;
+    const DecoderCache kv = decoder_cache(c, k, v, nimg_total, img0, nimg, M, dl, key_len);
+    const long slices = static_cast<long>(nimg_total) * 96, koff = kv.off;
+    bf16 *kh = kv.kh, *kl = kv.kl, *vh = kv.vh, *vl = kv.vl;
     const long nkv = static_cast<long>(nimg) * M * 512, in_off = static_cast<long>(img0) * M * 512;
-    op_head_major_kernel<<<blocks256(nkv), 256, 0, c->stream>>>(k + in_off, M, nkv, kh + koff, kl + koff);
-    op_head_major_kernel<<<blocks256(nkv), 256, 0, c->stream>>>(v + in_off, M, nkv, vh + koff, vl + koff);
-    check_launch("op_head_major");
     const int Mpad = (M + 7) & ~7;
     bf16 *vth = nullptr, *vtl = nullptr;
     const long voff = (static_cast<long>(img0) * 6144 + dl * 512) * Mpad;
@@ -1545,15 +1504,6 @@ void op_cross_attention(alm_ctx* h, const float* q, const float* k, const float*
       d_off = d_len + nimg;
       ALM_CHECK_CUDA(cudaMemcpyAsync(d_len, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream));
       ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));  // idx goes out of scope
-      for (int i = 0; i < nimg; ++i) {
-        const int n = key_len[img0 + i];
-        if (n == M) continue;
-        // rows n..M-1 of the 8 [M][64] head blocks of this image and layer
-        const long base = (static_cast<long>(img0 + i) * 96 + dl * 8) * M * 64 + static_cast<long>(n) * 64;
-        for (bf16* p : {kh, kl, vh, vl})
-          ALM_CHECK_CUDA(cudaMemset2DAsync(p + base, static_cast<size_t>(M) * 128, 0xff, static_cast<size_t>(M - n) * 128,
-                                           8, c->stream));
-      }
     }
     if (impl == 1) {
       const int ns = cross_attn_q1_splits(c, nimg, M);
@@ -1620,33 +1570,17 @@ int alm_op_rec_locations(alm_ctx* h, const float* q, const float* k, const uint8
     for (int i = 0; i < nimg; ++i)
       ALM_REQUIRE(mw[i] >= 1 && (!key_len || (key_len[i] >= 1 && key_len[i] <= M)), ALM_ERR_INVALID,
                   "alm_op_rec_locations: mw or key_len out of range");
-    ALM_REQUIRE(is_device_ptr(q) && is_device_ptr(k) && is_device_ptr(out) && (!kpm || is_device_ptr(kpm)),
-                ALM_ERR_INVALID, "device pointers required");
+    require_device({q, k, out, kpm}, 1, "alm_op_rec_locations");
     Ctx* c = &h->c;
     c->ensure_ws();
     ArenaScope arena_scope(c->ws);
-    // the model's K cache, every element this call must not read poisoned with NaN (0xffff)
-    const size_t cache = static_cast<size_t>(nimg) * 96 * M * 64;
-    bf16* kh = c->ws.get<bf16>(cache); bf16* kl = c->ws.get<bf16>(cache);
-    for (bf16* p : {kh, kl}) ALM_CHECK_CUDA(cudaMemsetAsync(p, 0xff, cache * 2, c->stream));
-    const long koff = static_cast<long>(11) * 8 * M * 64, nk = static_cast<long>(nimg) * M * 512;
-    op_head_major_kernel<<<blocks256(nk), 256, 0, c->stream>>>(k, M, nk, kh + koff, kl + koff);
-    check_launch("op_head_major");
+    const DecoderCache kc = decoder_cache(c, k, nullptr, nimg, 0, nimg, M, 11, key_len);  // the last decoder layer
     // per-image tables: key_len [nimg] (optional), grid widths [nimg]
     std::vector<int> idx(mw, mw + nimg);
     if (key_len) idx.insert(idx.end(), key_len, key_len + nimg);
     int* d_mw = c->ws.get<int>(idx.size());
     const int* d_len = key_len ? d_mw + nimg : nullptr;
     ALM_CHECK_CUDA(cudaMemcpyAsync(d_mw, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-    if (key_len)
-      for (int i = 0; i < nimg; ++i) {
-        const int n = key_len[i];
-        if (n == M) continue;
-        const long base = (static_cast<long>(i) * 96 + 88) * M * 64 + static_cast<long>(n) * 64;  // rows n..M-1, 8 heads
-        for (bf16* p : {kh, kl})
-          ALM_CHECK_CUDA(cudaMemset2DAsync(p + base, static_cast<size_t>(M) * 128, 0xff, static_cast<size_t>(M - n) * 128,
-                                           8, c->stream));
-      }
     const long nq = static_cast<long>(nimg) * Ncap * 512;
     bf16 *qh = nullptr, *ql = nullptr;
     if (q_split) {
@@ -1660,42 +1594,73 @@ int alm_op_rec_locations(alm_ctx* h, const float* q, const float* k, const uint8
     int* counters = c->ws.get<int>(groups);
     ALM_CHECK_CUDA(cudaMemsetAsync(partial, 0xff, pf * 4, c->stream));
     fill_i32(c, counters, groups, 0);
-    rec_locate(c, qh, ql, q_split ? nullptr : q, nimg, Ncap, kh + koff, kl + koff, kpm, M, d_len, d_mw, ks, partial,
+    rec_locate(c, qh, ql, q_split ? nullptr : q, nimg, Ncap, kc.kh + kc.off, kc.kl + kc.off, kpm, M, d_len, d_mw, ks, partial,
                counters, nullptr, 0, 1, out);
     ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
   });
 }
 
+namespace {
+
+// anc: null, or the ancestry of alm_op_self_attention_step_anc
+void op_self_attention_step(alm_ctx* h, const float* qkv, float* kc, float* vc, float* out, int S, int t, int Tmax,
+                            const int32_t* anc) {
+  ALM_REQUIRE(qkv && kc && vc && out && S > 0 && t >= 0 && t < Tmax && Tmax <= 1024, ALM_ERR_INVALID,
+              "alm_op_self_attention_step arguments");
+  require_device({qkv, kc, vc, out, anc}, 1, "alm_op_self_attention_step");
+  Ctx* c = &h->c;
+  c->ensure_ws();
+  ArenaScope arena_scope(c->ws);
+  int* tpos = c->ws.get<int>(1);
+  fill_i32(c, tpos, 1, t);
+  self_attn_step(c, qkv, qkv + 1024, kc, vc, S, tpos, Tmax, nullptr, nullptr, out, 1536, 1536, anc);
+  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+}
+
+// The decoder loop's token / probability buffers for one step with no prompt: the position counter is gen_index, the
+// token lands in column gen_index + 1 and its probability (NaN until written) in column gen_index.  Tmax > 0 adds an
+// identity ancestry.
+struct StepBuffers {
+  int* tokens;
+  float* probs;
+  int* anc;
+  int* tpos;
+  int tstride, pstride;
+};
+StepBuffers step_buffers(Ctx* c, int S, int gen_index, int Tmax) {
+  StepBuffers b;
+  b.tstride = gen_index + 2;
+  b.pstride = gen_index + 1;
+  b.tokens = c->ws.get<int>(static_cast<size_t>(S) * b.tstride);
+  b.probs = c->ws.get<float>(static_cast<size_t>(S) * b.pstride);
+  b.anc = Tmax > 0 ? c->ws.get<int>(static_cast<size_t>(S) * Tmax) : nullptr;
+  b.tpos = c->ws.get<int>(1);
+  fill_i32(c, b.tokens, static_cast<long>(S) * b.tstride, -1);
+  ALM_CHECK_CUDA(cudaMemsetAsync(b.probs, 0xff, static_cast<size_t>(S) * b.pstride * 4, c->stream));
+  if (b.anc) anc_identity(c, b.anc, S, Tmax);
+  fill_i32(c, b.tpos, 1, gen_index);
+  return b;
+}
+
+// the step's token and probability of each of the S rows, into the caller's device arrays
+void copy_step_out(Ctx* c, const StepBuffers& b, int S, int gen_index, int32_t* token, float* prob) {
+  ALM_CHECK_CUDA(cudaMemcpy2DAsync(token, sizeof(int32_t), b.tokens + gen_index + 1, b.tstride * sizeof(int), sizeof(int),
+                                   S, cudaMemcpyDeviceToDevice, c->stream));
+  ALM_CHECK_CUDA(cudaMemcpy2DAsync(prob, sizeof(float), b.probs + gen_index, b.pstride * sizeof(float), sizeof(float), S,
+                                   cudaMemcpyDeviceToDevice, c->stream));
+}
+
+}  // namespace
+
 int alm_op_self_attention_step(alm_ctx* h, const float* qkv, float* kc, float* vc, float* out, int S, int t, int Tmax) {
-  return guarded(h, [&] {
-    ALM_REQUIRE(qkv && kc && vc && out && S > 0 && t >= 0 && t < Tmax && Tmax <= 1024, ALM_ERR_INVALID,
-                "alm_op_self_attention_step arguments");
-    ALM_REQUIRE(is_device_ptr(qkv) && is_device_ptr(kc) && is_device_ptr(vc) && is_device_ptr(out), ALM_ERR_INVALID,
-                "device pointers required");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    int* tpos = c->ws.get<int>(1);
-    fill_i32(c, tpos, 1, t);
-    self_attn_step(c, qkv, qkv + 1024, kc, vc, S, tpos, Tmax, nullptr, nullptr, out, 1536, 1536);
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-  });
+  return guarded(h, [&] { op_self_attention_step(h, qkv, kc, vc, out, S, t, Tmax, nullptr); });
 }
 
 int alm_op_self_attention_step_anc(alm_ctx* h, const float* qkv, float* kc, float* vc, float* out, int S, int t, int Tmax,
                                    const int32_t* anc) {
   return guarded(h, [&] {
-    ALM_REQUIRE(qkv && kc && vc && out && anc && S > 0 && t >= 0 && t < Tmax && Tmax <= 1024, ALM_ERR_INVALID,
-                "alm_op_self_attention_step_anc arguments");
-    ALM_REQUIRE(is_device_ptr(qkv) && is_device_ptr(kc) && is_device_ptr(vc) && is_device_ptr(out) && is_device_ptr(anc),
-                ALM_ERR_INVALID, "device pointers required");
-    Ctx* c = &h->c;
-    c->ensure_ws();
-    ArenaScope arena_scope(c->ws);
-    int* tpos = c->ws.get<int>(1);
-    fill_i32(c, tpos, 1, t);
-    self_attn_step(c, qkv, qkv + 1024, kc, vc, S, tpos, Tmax, nullptr, nullptr, out, 1536, 1536, anc);
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+    ALM_REQUIRE(anc, ALM_ERR_INVALID, "alm_op_self_attention_step_anc: anc is null");
+    op_self_attention_step(h, qkv, kc, vc, out, S, t, Tmax, anc);
   });
 }
 
@@ -1704,10 +1669,7 @@ int alm_op_gemv(alm_ctx* h, const float* x, const float* x2, int n_split, const 
                 const float* pos, int pos_split) {
   return guarded(h, [&] {
     ALM_REQUIRE(x && W && out && N > 0 && act >= ACT_NONE && act <= ACT_RELU, ALM_ERR_INVALID, "alm_op_gemv arguments");
-    for (const void* p : {static_cast<const void*>(x), static_cast<const void*>(x2), static_cast<const void*>(W),
-                          static_cast<const void*>(bias), static_cast<const void*>(resid), static_cast<const void*>(out),
-                          static_cast<const void*>(ln_g), static_cast<const void*>(ln_b), static_cast<const void*>(pos)})
-      ALM_REQUIRE(!p || is_device_ptr(p), ALM_ERR_INVALID, "device pointers required");
+    require_device({x, x2, W, bias, resid, out, ln_g, ln_b, pos}, 1, "alm_op_gemv");
     Ctx* c = &h->c;
     gemv_rows(c, x, x2, n_split, K, W, bias, resid, N, out, N, M, N, K, act, ln_g, ln_b, 1e-5f, pos, pos_split);
     ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
@@ -1720,26 +1682,14 @@ int alm_op_head_select(alm_ctx* h, const float* logits, int S, int V, int nsoft,
     ALM_REQUIRE(logits && cfg && token && prob && S > 0 && V > 0 && nsoft > 0 && nsoft <= V && phase >= 0 && phase <= 2 &&
                     gen_index >= 0 && gen_index < (1 << 20) && (finished == nullptr) == (ntok == nullptr),
                 ALM_ERR_INVALID, "alm_op_head_select arguments");
-    ALM_REQUIRE(is_device_ptr(logits) && is_device_ptr(token) && is_device_ptr(prob) && (!finished || is_device_ptr(finished)) &&
-                    (!ntok || is_device_ptr(ntok)),
-                ALM_ERR_INVALID, "device pointers required");
+    require_device({logits, token, prob, finished, ntok}, 1, "alm_op_head_select");
     Ctx* c = &h->c;
     c->ensure_ws();
     ArenaScope arena_scope(c->ws);
-    // the pt loop's buffers with no prompt: position counter == gen_index, the token lands in column gen_index + 1
-    const int tstride = gen_index + 2, pstride = gen_index + 1;
-    int* tokens = c->ws.get<int>(static_cast<size_t>(S) * tstride);
-    float* probs = c->ws.get<float>(static_cast<size_t>(S) * pstride);
-    int* tpos = c->ws.get<int>(1);
-    fill_i32(c, tokens, static_cast<long>(S) * tstride, -1);
-    ALM_CHECK_CUDA(cudaMemsetAsync(probs, 0xff, static_cast<size_t>(S) * pstride * 4, c->stream));
-    fill_i32(c, tpos, 1, gen_index);
+    const StepBuffers b = step_buffers(c, S, gen_index, 0);  // the pt loop's
     const HeadCfg hc{cfg->num_bins, cfg->pt_eos, cfg->rec_eos, cfg->recog_pad, cfg->vie_categories};
-    head_select(c, logits, S, V, nsoft, phase, hc, tokens, tstride, tpos, 0, probs, pstride, finished, ntok, 1);
-    ALM_CHECK_CUDA(cudaMemcpy2DAsync(token, sizeof(int32_t), tokens + gen_index + 1, tstride * sizeof(int), sizeof(int), S,
-                                     cudaMemcpyDeviceToDevice, c->stream));
-    ALM_CHECK_CUDA(cudaMemcpy2DAsync(prob, sizeof(float), probs + gen_index, pstride * sizeof(float), sizeof(float), S,
-                                     cudaMemcpyDeviceToDevice, c->stream));
+    head_select(c, logits, S, V, nsoft, phase, hc, b.tokens, b.tstride, b.tpos, 0, b.probs, b.pstride, finished, ntok, 1);
+    copy_step_out(c, b, S, gen_index, token, prob);
     ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
   });
 }
@@ -1750,31 +1700,19 @@ int alm_op_beam_select(alm_ctx* h, const float* logits, int G, int W, int V, int
     ALM_REQUIRE(logits && cfg && score && len && token && parent && prob && G > 0 && W >= 1 && W <= ALM_MAX_BEAMS &&
                     V > 0 && nsoft > 0 && nsoft <= V && gen_index >= 0 && gen_index < 1024,
                 ALM_ERR_INVALID, "alm_op_beam_select arguments");
-    for (const void* p : {static_cast<const void*>(logits), static_cast<const void*>(score), static_cast<const void*>(len),
-                          static_cast<const void*>(token), static_cast<const void*>(parent), static_cast<const void*>(prob)})
-      ALM_REQUIRE(is_device_ptr(p), ALM_ERR_INVALID, "device pointers required");
+    require_device({logits, score, len, token, parent, prob}, 1, "alm_op_beam_select");
     Ctx* c = &h->c;
     c->ensure_ws();
     ArenaScope arena_scope(c->ws);
-    // the rec loop's buffers with no prompt: position counter == gen_index, the token lands in column gen_index + 1,
-    // the parent row in ancestry column gen_index
-    const int S = G * W, tstride = gen_index + 2, pstride = gen_index + 1, Tmax = gen_index + 1;
-    int* tokens = c->ws.get<int>(static_cast<size_t>(S) * tstride);
-    float* probs = c->ws.get<float>(static_cast<size_t>(S) * pstride);
-    int* anc = c->ws.get<int>(static_cast<size_t>(S) * Tmax);
-    int* tpos = c->ws.get<int>(1);
-    fill_i32(c, tokens, static_cast<long>(S) * tstride, -1);
-    anc_identity(c, anc, S, Tmax);
-    fill_i32(c, tpos, 1, gen_index);
+    // the rec loop's, the parent row in ancestry column gen_index
+    const int S = G * W, Tmax = gen_index + 1;
+    const StepBuffers b = step_buffers(c, S, gen_index, Tmax);
     const HeadCfg hc{cfg->num_bins, cfg->pt_eos, cfg->rec_eos, cfg->recog_pad, cfg->vie_categories};
-    beam_select(c, logits, G, W, V, nsoft, hc, tokens, tstride, tpos, 0, probs, pstride, score, len, anc, Tmax);
-    ALM_CHECK_CUDA(cudaMemcpy2DAsync(token, sizeof(int32_t), tokens + gen_index + 1, tstride * sizeof(int), sizeof(int), S,
-                                     cudaMemcpyDeviceToDevice, c->stream));
-    ALM_CHECK_CUDA(cudaMemcpy2DAsync(prob, sizeof(float), probs + gen_index, pstride * sizeof(float), sizeof(float), S,
-                                     cudaMemcpyDeviceToDevice, c->stream));
+    beam_select(c, logits, G, W, V, nsoft, hc, b.tokens, b.tstride, b.tpos, 0, b.probs, b.pstride, score, len, b.anc, Tmax);
+    copy_step_out(c, b, S, gen_index, token, prob);
     // the ancestry holds the parent's row; the op reports its slot within the group
     std::vector<int32_t> par(S);
-    ALM_CHECK_CUDA(cudaMemcpy2DAsync(par.data(), sizeof(int32_t), anc + gen_index, Tmax * sizeof(int), sizeof(int), S,
+    ALM_CHECK_CUDA(cudaMemcpy2DAsync(par.data(), sizeof(int32_t), b.anc + gen_index, Tmax * sizeof(int), sizeof(int), S,
                                      cudaMemcpyDeviceToHost, c->stream));
     ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
     for (int r = 0; r < S; ++r) par[r] -= r - r % W;
