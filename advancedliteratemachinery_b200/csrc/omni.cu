@@ -886,7 +886,7 @@ void run_steps(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens, in
                            reinterpret_cast<long>(u.x), reinterpret_cast<long>(tokens), tstride,
                            reinterpret_cast<long>(h.probs), reinterpret_cast<long>(h.finished), h.n_prompt_m1,
                            reinterpret_cast<long>(m->kc_hi), reinterpret_cast<long>(u.kc[3]), h.cfg.pt_eos, h.cfg.num_bins,
-                           h.cfg.rec_eos, h.cfg.recog_pad, reinterpret_cast<long>(c->trace_buf), h.nsoft, h.cfg.vie, c->xattn_impl, c->gemm_grid_cap, c->debug_skip, c->xattn_ctas_per_sm, c->sattn_wide, c->xattn_wg, c->fuse_ln_gemv,
+                           h.cfg.rec_eos, h.cfg.recog_pad, reinterpret_cast<long>(c->trace_buf), h.nsoft, h.cfg.vie, c->xattn_impl, c->gemm_grid_cap, c->small_grid_cap, c->debug_skip, c->xattn_ctas_per_sm, c->sattn_wide, c->xattn_wg, c->fuse_ln_gemv,
                            reinterpret_cast<long>(m->key_len), u.mq_grid, u.mq_parts, h.topk,
                            reinterpret_cast<long>(h.cand_ids), reinterpret_cast<long>(h.cand_probs), h.beams,
                            reinterpret_cast<long>(h.bscore), reinterpret_cast<long>(u.anc), reinterpret_cast<long>(u.loc)};
