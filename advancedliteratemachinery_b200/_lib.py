@@ -261,6 +261,11 @@ SIGNATURES = {
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_long]),
+    # ctx, n_words, rec_length, polys, rec, loc, frame_index, n_frames, frames, recog_pad_index, rec_eos_index, n_chars,
+    # step, centre, cov, box
+    'alm_omni_char_boxes': (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p]),
     # ctx, n_pages, page_count, page_offset, polys, cos_tol, height_ratio, max_offset, max_overlap, max_gap, n_lines,
     # line_offset, line_first, line_words, order, line_of, rank_of, line_polys, cap
     'alm_omni_group_lines': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double,

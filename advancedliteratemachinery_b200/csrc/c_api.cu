@@ -1034,6 +1034,35 @@ int alm_omni_merge_whole_page(alm_ctx* h, const int* heights, const int* widths,
   });
 }
 
+int alm_omni_char_boxes(alm_ctx* h, long n_words, int rec_length, const double* polys, const int64_t* rec,
+                        const float* loc, const int32_t* frame_index, int n_frames, const int32_t* frames,
+                        int recog_pad_index, int rec_eos_index, int32_t* n_chars, int32_t* step, double* centre,
+                        double* cov, double* box) {
+  return guarded(h, [&] {
+    const char* fn = "alm_omni_char_boxes";
+    ALM_REQUIRE(n_words >= 0 && rec_length >= 1 && rec_length <= rec_box_core::kMaxSteps, ALM_ERR_INVALID,
+                std::string(fn) + ": n_words must be >= 0 and rec_length in 1.." +
+                    std::to_string(rec_box_core::kMaxSteps));
+    if (n_words == 0) return;
+    ALM_REQUIRE(polys && rec && loc && frame_index && frames && n_chars && step && centre && cov && box,
+                ALM_ERR_INVALID, std::string(fn) + ": null argument");
+    ALM_REQUIRE(n_frames >= 1, ALM_ERR_INVALID, std::string(fn) + ": words need at least one frame");
+    std::vector<rec_box_core::Frame> fr(static_cast<size_t>(n_frames));
+    for (int k = 0; k < n_frames; ++k) {
+      const int32_t* v = frames + 7L * k;
+      fr[static_cast<size_t>(k)] = rec_box_core::Frame{v[0], v[1], v[2], v[3], v[4], v[5], v[6]};
+      ALM_REQUIRE(rec_box_core::valid_frame(fr[static_cast<size_t>(k)]), ALM_ERR_INVALID,
+                  std::string(fn) + ": frame " + std::to_string(k) +
+                      ": need positive sizes, a turn in 0..3 and the tile inside its turned page");
+    }
+    for (long n = 0; n < n_words; ++n)
+      ALM_REQUIRE(frame_index[n] >= 0 && frame_index[n] < n_frames, ALM_ERR_INVALID,
+                  std::string(fn) + ": word " + std::to_string(n) + ": frame index out of range");
+    char_boxes(&h->c, n_words, rec_length, n_frames, fr.data(), frame_index, polys, rec, loc, recog_pad_index,
+               rec_eos_index, n_chars, step, centre, cov, box);
+  });
+}
+
 int alm_omni_merge_kie_tiles(alm_ctx* h, const int* heights, const int* widths, int n_pages, const int32_t* turns,
                              int tile, int overlap, int n_tiles, const int* tile_page, const int* tile_origin,
                              const int32_t* n_tok, const int64_t* tokens, const float* tok_prob, int max_tok,

@@ -5,6 +5,7 @@
 #include "alm_internal.h"
 #include "group_core.h"
 #include "kie_tile_core.h"
+#include "rec_box_core.h"
 #include "tile_core.h"
 #include "whole_core.h"
 
@@ -124,6 +125,14 @@ void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, i
                const kie_tile_core::Entity* ents, int max_inst, const int64_t* poly, int num_bins, double margin,
                double iou, int* page_count, int* page_offset, int* cls_out, float* prob_out, int* word_offset,
                int* word_count, int* ent_src, double* rects, double* polys, int* word_src);
+
+// Character boxes in page pixels (tile_merge.cu; rule: rec_box_core.h, DESIGN 4.20).  Host inputs: N words' page
+// polygons [N][32], rec ids [N][L], locations [N][L][5] and frame index [N] (into frames [F], checked by the caller).
+// Host outputs: n_chars [N] and per slot [N][L] the step, centre [2], cov [3] and box [8]; slots past n_chars are 0.
+// One launch; none when N = 0.
+void char_boxes(Ctx* c, long N, int L, int F, const rec_box_core::Frame* frames, const int* frame_index,
+                const double* polys, const int64_t* rec, const float* loc, int64_t pad, int64_t eos, int* n_chars,
+                int* step, double* centre, double* cov, double* box);
 
 // Words -> text lines (group_core.h, line_group.cu): the N word polygons f64 [N][32] of n_pages pages (page p = rows
 // page_offset[p] .. + page_count[p] - 1, the rows of all pages partition [0, N); host buffers) grouped into lines.

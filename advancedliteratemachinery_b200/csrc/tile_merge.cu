@@ -41,12 +41,19 @@
 //                        the block's kept entities in slot order by a warp ballot and their words after a block scan
 //                        of the word counts (no atomics); words mapped back to the upright page as they are written;
 //                        the first block of a page writes its entity count and offset, the last block the word total
+//
+// Character boxes in page pixels of words read in tiles (rule: rec_box_core.h, DESIGN 4.20), one launch:
+//   rec_box_kernel       one warp per word: decode_seq's walk over the steps in chunks of 32, a lane per step, the
+//                        kept steps numbered by ballot prefix counts (no atomics: bit-reproducible), each kept step's
+//                        centre, covariance and box from the word's polygon staged in shared memory; slots past the
+//                        word's character count are zeroed
 #include <algorithm>
 #include <vector>
 
 #include "alm_internal.h"
 #include "pre.h"
 #include "kie_tile_core.h"
+#include "rec_box_core.h"
 #include "tile_core.h"
 #include "turn_core.h"
 #include "whole_core.h"
@@ -445,6 +452,48 @@ kie_compact_kernel(int max_ent, int max_inst, int nchunk, int num_bins, int n_pa
   }
 }
 
+// words per block of rec_box_kernel: one warp each
+constexpr int kBoxWords = kBlock / 32;
+
+__global__ void __launch_bounds__(kBlock)
+rec_box_kernel(long N, int L, const rec_box_core::Frame* __restrict__ frames, const int* __restrict__ frame_index,
+               const double* __restrict__ polys, const int64_t* __restrict__ rec, const float* __restrict__ loc,
+               int64_t pad, int64_t eos, int* __restrict__ n_chars, int* __restrict__ step,
+               double* __restrict__ centre, double* __restrict__ cov, double* __restrict__ box) {
+  __shared__ double spoly[kBoxWords][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long n = static_cast<long>(blockIdx.x) * kBoxWords + warp;
+  if (n >= N) return;  // uniform over the warp
+  spoly[warp][lane] = polys[32 * n + lane];
+  __syncwarp();
+  const rec_box_core::Frame f = frames[frame_index[n]];
+  const long row = n * L;
+  int kept = 0;
+  for (int j0 = 0; j0 < L; j0 += 32) {
+    const int j = j0 + lane;
+    const int kind = j < L ? rec_box_core::step_kind(rec[row + j], pad, eos) : rec_box_core::kStop;
+    const unsigned stops = __ballot_sync(0xffffffffu, kind == rec_box_core::kStop);
+    const unsigned before = stops ? (1u << (__ffs(stops) - 1)) - 1u : 0xffffffffu;  // lanes before the first stop
+    const bool kp = (before >> lane & 1u) && kind == rec_box_core::kKeep;
+    const unsigned km = __ballot_sync(0xffffffffu, kp);
+    if (kp) {
+      const long o = row + kept + __popc(km & ((1u << lane) - 1u));
+      step[o] = j;
+      rec_box_core::char_box(spoly[warp], f, loc + 5 * (row + j), centre + 2 * o, cov + 3 * o, box + 8 * o);
+    }
+    kept += __popc(km);
+    if (stops) break;  // uniform over the warp
+  }
+  for (int i = kept + lane; i < L; i += 32) {
+    const long o = row + i;
+    step[o] = 0;
+    for (int k = 0; k < 2; ++k) centre[2 * o + k] = 0.0;
+    for (int k = 0; k < 3; ++k) cov[3 * o + k] = 0.0;
+    for (int k = 0; k < 8; ++k) box[8 * o + k] = 0.0;
+  }
+  if (lane == 0) n_chars[n] = kept;
+}
+
 }  // namespace
 
 void tile_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, int max_inst, int L, int num_bins,
@@ -730,6 +779,43 @@ void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, i
   down(rects, o_rects, kept_words * 4 * sizeof(double));
   down(polys, o_polys, kept_words * 32 * sizeof(double));
   down(word_src, o_wsrc, kept_words * 2 * sizeof(int));
+  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+}
+
+void char_boxes(Ctx* c, long N, int L, int F, const rec_box_core::Frame* frames, const int* frame_index,
+                const double* polys, const int64_t* rec, const float* loc, int64_t pad, int64_t eos, int* n_chars,
+                int* step, double* centre, double* cov, double* box) {
+  if (N == 0) return;
+  c->ensure_ws();
+  ArenaScope arena_scope(c->ws);
+  Arena& ws = c->ws;
+  auto up = [&](const void* src, size_t bytes) {
+    void* d = ws.alloc(bytes);
+    ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
+    return d;
+  };
+  const size_t S = static_cast<size_t>(N) * L;
+  const auto* d_frames = static_cast<const rec_box_core::Frame*>(up(frames, F * sizeof(rec_box_core::Frame)));
+  const auto* d_fi = static_cast<const int*>(up(frame_index, N * sizeof(int)));
+  const auto* d_polys = static_cast<const double*>(up(polys, N * 32 * sizeof(double)));
+  const auto* d_rec = static_cast<const int64_t*>(up(rec, S * sizeof(int64_t)));
+  const auto* d_loc = static_cast<const float*>(up(loc, S * 5 * sizeof(float)));
+  int* o_n = ws.get<int>(N);
+  int* o_step = ws.get<int>(S);
+  double* o_centre = ws.get<double>(S * 2);
+  double* o_cov = ws.get<double>(S * 3);
+  double* o_box = ws.get<double>(S * 8);
+  rec_box_kernel<<<static_cast<unsigned>((N + kBoxWords - 1) / kBoxWords), kBlock, 0, c->stream>>>(
+      N, L, d_frames, d_fi, d_polys, d_rec, d_loc, pad, eos, o_n, o_step, o_centre, o_cov, o_box);
+  count_launch(c); check_launch("rec_box");
+  auto down = [&](void* dst, const void* src, size_t bytes) {
+    ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
+  };
+  down(n_chars, o_n, N * sizeof(int));
+  down(step, o_step, S * sizeof(int));
+  down(centre, o_centre, S * 2 * sizeof(double));
+  down(cov, o_cov, S * 3 * sizeof(double));
+  down(box, o_box, S * 8 * sizeof(double));
   ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
 }
 

@@ -218,6 +218,81 @@ def merge_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_inst,
     return out
 
 
+MAX_REC_LENGTH = 1021  # alm_omni_char_boxes' bound on rec_length, as alm_omni_decode's
+
+
+def char_boxes(ctx: _lib.Context, sizes, tiles, polys, rec, loc, tile_index, recog_pad_index: int, rec_eos_index: int,
+               turns=None) -> dict:
+    """One box per recognised character of words read in tiles, in page pixels, on the device
+    (``alm_omni_char_boxes``; rule: DESIGN 4.20): ``postprocess.rec_char_boxes`` for the words of ``merge_tiles``,
+    ``merge_turns`` and ``read_regions``.  sizes: the upright (h, w) of every page; tiles int [F, 5] = (page, y0, x0, h,
+    w) in the layout of ``preprocess.omni_tile_plan`` (a page read whole: (page, 0, 0, h, w) of its turned size); turns:
+    None, or int [P] in 0..3, page p read as ``np.rot90(page_p, turns[p])``.  Word n: polys f64 [N, 32] (its vertices
+    in page pixels), rec int64 [N, L], loc f32 [N, L, 5] (the locations of the tile instance it came from,
+    ``last_rec_locations``' layout) and tile_index int [N] into tiles.
+    Returns dict(n_chars int32 [N], step int32 [N, L], centre f64 [N, L, 2], cov f64 [N, L, 3] = (sxx, sxy, syy), box
+    f64 [N, L, 8] = four corners (x, y)): character i of word n is slot [n, i], the i-th step decode_seq keeps; slots
+    past n_chars are 0.  ValueError for shapes that do not match, a tile index out of range, a turn outside 0..3, a
+    non-positive size or a tile outside its turned page."""
+    from .preprocess import check_turns
+    P = len(sizes)
+    turns = np.zeros(P, np.int32) if turns is None else check_turns(turns, P)
+    tiles = np.asarray(tiles, dtype=np.int64).reshape(-1, 5)
+    rec = np.ascontiguousarray(rec, dtype=np.int64)
+    if rec.ndim != 2:
+        raise ValueError(f'char_boxes: rec must be [N, L], got {rec.shape}')
+    N, L = rec.shape
+    polys = np.ascontiguousarray(polys, dtype=np.float64)
+    loc = np.ascontiguousarray(loc, dtype=np.float32)
+    tile_index = np.asarray(tile_index).reshape(-1)
+    if polys.shape not in ((N, 32), (N, 16, 2)):
+        raise ValueError(f'char_boxes: polys must be [{N}, 32], got {polys.shape}')
+    if loc.shape != (N, L, 5) or len(tile_index) != N or not 1 <= L <= MAX_REC_LENGTH:
+        raise ValueError(f'char_boxes: rec {rec.shape} (rec_length in 1..{MAX_REC_LENGTH}), loc {loc.shape} and '
+                         f'tile_index {tile_index.shape} do not match')
+    if N and (tile_index.dtype.kind not in 'iu' or tile_index.min() < 0 or tile_index.max() >= len(tiles)):
+        raise ValueError(f'char_boxes: tile indices must be integers in 0 .. {len(tiles) - 1}')
+    if len(tiles) and (tiles[:, 0].min() < 0 or tiles[:, 0].max() >= P):
+        raise ValueError(f'char_boxes: tile pages must be in 0 .. {P - 1}')
+    hw = np.array([(int(h), int(w)) for h, w in sizes], dtype=np.int64).reshape(-1, 2)
+    frames = np.zeros((len(tiles), 7), np.int32)
+    if len(tiles):
+        p = tiles[:, 0]
+        frames[:] = np.stack([hw[p, 0], hw[p, 1], turns[p], tiles[:, 1], tiles[:, 2], tiles[:, 3], tiles[:, 4]], 1)
+        odd = turns[p] % 2 == 1
+        th, tw = np.where(odd, hw[p, 1], hw[p, 0]), np.where(odd, hw[p, 0], hw[p, 1])
+        ok = (hw[p] >= 1).all(1) & (tiles[:, 3] >= 1) & (tiles[:, 4] >= 1) & (tiles[:, 1] >= 0) & (tiles[:, 2] >= 0) & \
+            (tiles[:, 1] + tiles[:, 3] <= th) & (tiles[:, 2] + tiles[:, 4] <= tw)
+        if not ok.all():
+            raise ValueError(f'char_boxes: tile {int(np.argmin(ok))} is empty or outside its turned page')
+    out = dict(n_chars=np.zeros(N, np.int32), step=np.zeros((N, L), np.int32), centre=np.zeros((N, L, 2)),
+               cov=np.zeros((N, L, 3)), box=np.zeros((N, L, 8)))
+    if N == 0:
+        return out
+    fi = np.ascontiguousarray(tile_index, dtype=np.int32)
+    ctx.check(ctx.lib.alm_omni_char_boxes(ctx.h, N, L, polys.ctypes.data, rec.ctypes.data, loc.ctypes.data,
+                                          fi.ctypes.data, len(frames), frames.ctypes.data, int(recog_pad_index),
+                                          int(rec_eos_index), *[out[k].ctypes.data for k in
+                                                                ('n_chars', 'step', 'centre', 'cov', 'box')]))
+    return out
+
+
+def char_dicts(boxes: dict, rec, vocab) -> List[List[dict]]:
+    """``char_boxes``' result -> per word the list ``postprocess.rec_char_boxes`` gives: dict(char, centre [2], cov
+    [[sxx, sxy], [sxy, syy]], box [4, 2]) per character, in page pixels."""
+    rec = np.asarray(rec)
+    out = []
+    for n, k in enumerate(boxes['n_chars'].tolist()):
+        chars = []
+        for i in range(k):
+            sxx, sxy, syy = boxes['cov'][n, i]
+            chars.append({'char': vocab.chars[int(rec[n, boxes['step'][n, i]]) - vocab.num_bins],
+                          'centre': boxes['centre'][n, i].copy(), 'cov': np.array([[sxx, sxy], [sxy, syy]]),
+                          'box': boxes['box'][n, i].reshape(4, 2).copy()})
+        out.append(chars)
+    return out
+
+
 def orient_select(ctx: _lib.Context, n_inst, rec, prob, recog_pad_index: int, rec_eos_index: int):
     """Per page the turn its four probe readings choose, on the device (``alm_omni_orient_select``; rule: DESIGN
     4.14).  n_inst int [P, 4], rec int64 [P, 4, max_inst, L], prob f32 [..]: reading [p, k] = page p read whole at turn
@@ -1019,7 +1094,8 @@ class OmniParserB200:
 
     def spot_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                    band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200,
-                   test_max_size: int = 1920, orientation='upright', whole_page: bool = False) -> List[List[dict]]:
+                   test_max_size: int = 1920, orientation='upright', whole_page: bool = False,
+                   rec_locations: bool = False) -> List[List[dict]]:
         """Text spotting of pages larger than the model's input, read in overlapping tiles (rule: DESIGN 4.11).
         pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch).  Every page is cut into the tiles
         of ``preprocess.omni_tile_plan(sizes, tile, overlap)``; each tile goes through the reference's validation
@@ -1054,7 +1130,13 @@ class OmniParserB200:
         the tile words whose point lies inside one of them.  Such words come with 'tile' -1 and 'instance' their index
         in the whole-page decode, after the page's tile words; ``last_tiles`` gains 'whole' (the whole-page decode
         arrays, one row per page, or per reading for 'mixed') and 'whole_merge'.  A page that fits in one tile is not
-        read again and keeps what whole_page=False gives.  Text spotting only."""
+        read again and keeps what whole_page=False gives.  Text spotting only.
+        rec_locations (rule: DESIGN 4.20): every tile decode, and 'auto''s probes, also keep the character locations
+        (``decode``'s rec_locations); each kept word is followed back to its tile instance ('auto': a page that fits in
+        one tile, to its probe reading; 'mixed': through the turn merge to its reading's tile) and one ``char_boxes``
+        call for all pages gives each word 'chars', ``postprocess.rec_char_boxes``' list (char, centre, cov, box) in
+        pixels of the page as passed in.  ``last_tiles`` gains 'loc', every tile's locations.  Not together with
+        whole_page: whole-page readings go through ``decode_dense``, which has no locations."""
         from . import postprocess
         from . import preprocess as Pre
         v = self.vocab
@@ -1062,6 +1144,8 @@ class OmniParserB200:
             raise ValueError('spot_tiled reads text spotting checkpoints; this one is a KIE checkpoint')
         if int(max_batch) < 1:
             raise ValueError(f'max_batch must be >= 1, got {max_batch}')
+        if rec_locations and whole_page:
+            raise ValueError('rec_locations cannot be combined with whole_page: whole-page readings have no locations')
         auto = isinstance(orientation, str) and orientation == 'auto'
         if isinstance(orientation, str):
             if orientation not in ('upright', 'auto', 'mixed'):
@@ -1076,16 +1160,17 @@ class OmniParserB200:
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
         if isinstance(orientation, str) and orientation == 'mixed':
             return self._spot_mixed(pages, sizes, tile, overlap, max_batch, margin, band, iou, test_min_size,
-                                    test_max_size, whole_page)
+                                    test_max_size, whole_page, rec_locations)
+        decode = self._decode_loc_arrays if rec_locations else self._decode_arrays
         extra = {}
         if auto:
             Pre.omni_tile_plan(sizes, tile, overlap)  # a bad layout is refused before the probes run
             probe, turns, extra['page_scores'] = self._probe_turns(pages, sizes, max_batch, test_min_size, test_max_size,
-                                                                   self._decode_arrays)
+                                                                   decode)
             extra['probe'] = probe
-        plan, (n_inst, pt, poly, rec, prob) = self._read_tiles(pages, sizes, turns, extra.get('probe'), tile, overlap,
-                                                               max_batch, test_min_size, test_max_size,
-                                                               self._decode_arrays)
+        plan, (n_inst, pt, poly, rec, prob, *loc) = self._read_tiles(pages, sizes, turns, extra.get('probe'), tile,
+                                                                     overlap, max_batch, test_min_size, test_max_size,
+                                                                     decode)
         m = merge_tiles(self.ctx, sizes, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band, iou,
                         turns=turns)
         out, whole = m, None
@@ -1096,6 +1181,7 @@ class OmniParserB200:
                 whole = self._read_whole(pages, sizes, turns, tile, max_batch, test_min_size, test_max_size)
             out = merge_whole_page(self.ctx, sizes, tile, overlap, m, *whole, v.num_bins, margin, turns=turns)
         texts, scores = postprocess.rec_texts(out['rec'], out['prob'], v)
+        chars = self._tile_chars(sizes, plan, turns, out, out['source'], loc[0]) if rec_locations else None
         first_tile = np.searchsorted(plan[:, 0], np.arange(len(sizes)))
         results = []
         for p in range(len(sizes)):
@@ -1104,9 +1190,12 @@ class OmniParserB200:
             results.append([{'pts': [[float(out['pts'][r, 0]), float(out['pts'][r, 1])]], 'score': float(scores[r]),
                              'polys': out['polys'][r].reshape(-1, 2).tolist(), 'rec': texts[r],
                              'tile': _tile_of(out['source'][r, 0], first_tile[p]),
-                             'instance': int(out['source'][r, 1]), **turn}
+                             'instance': int(out['source'][r, 1]), **turn,
+                             **({} if chars is None else {'chars': chars[r]})}
                             for r in rows])
         self.last_tiles = dict(plan=plan, n_inst=n_inst, pt=pt, poly=poly, rec=rec, prob=prob, merged=m)
+        if rec_locations:
+            self.last_tiles.update(loc=loc[0])
         if whole is not None:
             self.last_tiles.update(whole=whole, whole_merge=out)
         if turns is not None:
@@ -1115,7 +1204,7 @@ class OmniParserB200:
 
     def read_regions(self, pages, regions, page_index, kind: str = 'quad', tile: int = 1200, overlap: int = 256,
                      max_batch: int = 16, test_min_size: int = 1200, test_max_size: int = 1920, rec_candidates: int = 0,
-                     rec_beams: int = 0, length_penalty: float = 1.0) -> List[dict]:
+                     rec_beams: int = 0, length_penalty: float = 1.0, rec_locations: bool = False) -> List[dict]:
         """Read caller-given regions of raw pages of any size (rule: DESIGN 4.19): OmniParser as the recogniser of
         another detector's regions, each word read in place on the page and returned with its 16-point polygon.
         pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch); regions of one kind, in page
@@ -1134,9 +1223,12 @@ class OmniParserB200:
         ``last_regions`` keeps the plan, the routing (plan index or -1 per region), the points and every chunk's
         tiles / pages and raw arrays.  rec_candidates / rec_beams / length_penalty: as in ``decode``, with
         ``last_rec_candidates`` (ids, probs [R, rec_length, k]) and ``last_rec_beams`` (ids, probs [R, W, rec_length],
-        scores [R, W]) in region order.
-        Not offered: character locations (they would be in each tile's frame), orientation, KIE checkpoints, and any
-        merge or dedupe of overlapping regions -- each region is read as given."""
+        scores [R, W]) in region order.  rec_locations (not together with rec_beams; rule: DESIGN 4.20): every chunk's
+        ``read_at`` also keeps the character locations, ``last_rec_locations`` [R, rec_length, 5] in region order (each
+        in its tile's or page's frame), and one ``char_boxes`` call gives each region 'chars', ``postprocess.
+        rec_char_boxes``' list (char, centre, cov, box) in page pixels.
+        Not offered: orientation, KIE checkpoints, and any merge or dedupe of overlapping regions -- each region is read
+        as given."""
         from . import postprocess
         from . import preprocess as Pre
         v = self.vocab
@@ -1155,7 +1247,7 @@ class OmniParserB200:
         pi = pi.astype(np.int64)
         for r in range(R):   # every point on its page (ValueError otherwise)
             postprocess.point_bins(centres[r], sizes[pi[r]], v.num_bins)
-        self._set_rec_candidates(rec_candidates, rec_beams, length_penalty)   # refused before any device work
+        self._set_rec_candidates(rec_candidates, rec_beams, length_penalty, rec_locations)   # refused before device work
         plan = Pre.omni_tile_plan(sizes, tile, overlap)
         route = route_regions(sizes, plan, region_boxes(regions, kind), pi)
         # the plan's tiles that hold a region, then the pages read whole, in chunks of their own kind
@@ -1171,6 +1263,7 @@ class OmniParserB200:
         cand = (np.zeros((R, L, K), np.int64), np.zeros((R, L, K), np.float32)) if K > 0 else None
         beams = (np.zeros((R, W, L), np.int64), np.zeros((R, W, L), np.float32), np.zeros((R, W), np.float32)) \
             if W > 0 else None
+        loc = np.zeros((R, L, 5), np.float32) if rec_locations else None
         chunks = []
         T_whole = max([64] + [max(sizes[p]) for _, p in whole])
         for chunk in [tiles[i:i + mb] for i in range(0, len(tiles), mb)] + \
@@ -1195,7 +1288,7 @@ class OmniParserB200:
                 self.encode_pages(nt.tensors, resized)
             local = [postprocess.point_bins(centres[r_] - np.array([f[1], f[0]]), f[2:], v.num_bins)
                      for f, r_ in zip(frames, rows)]
-            n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty)
+            n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty, rec_locations)
             for j, (f, r_) in enumerate(zip(frames, rows)):
                 k = len(r_)
                 rec[r_], prob[r_] = rc[j, :k], pb[j, :k]
@@ -1207,15 +1300,24 @@ class OmniParserB200:
                 if beams is not None:
                     for a, b in zip(beams, self.last_rec_beams):
                         a[r_] = b[j, :k]
+                if loc is not None:
+                    loc[r_] = self.last_rec_locations[j, :k]
             chunks.append(dict(kind=chunk[0][0], index=np.array([i for _, i in chunk]), n=n, pt=xy, poly=pl, rec=rc,
                                prob=pb))
         texts, scores = postprocess.rec_texts(rec, prob, v)
+        chars = None
+        if loc is not None:  # frames: the plan's tiles, then every page read whole
+            frames = np.concatenate([plan, [(p, 0, 0) + sizes[p] for p in range(len(sizes))]])
+            boxes = char_boxes(self.ctx, sizes, frames, polys, rec, loc, np.where(route >= 0, route, len(plan) + pi),
+                               v.recog_pad_index, v.rec_eos_index)
+            chars = char_dicts(boxes, rec, v)
         first_tile = np.searchsorted(plan[:, 0], np.arange(len(sizes)))
-        self.last_rec_candidates, self.last_rec_beams = cand, beams
+        self.last_rec_candidates, self.last_rec_beams, self.last_rec_locations = cand, beams, loc
         self.last_regions = dict(plan=plan, route=route, points=centres, chunks=chunks)
         return [{'pts': [pts[r].tolist()], 'score': float(scores[r]), 'polys': polys[r].reshape(16, 2).tolist(),
                  'rec': texts[r], 'page': int(pi[r]),
-                 'tile': int(route[r] - first_tile[pi[r]]) if route[r] >= 0 else -1} for r in range(R)]
+                 'tile': int(route[r] - first_tile[pi[r]]) if route[r] >= 0 else -1,
+                 **({} if chars is None else {'chars': chars[r]})} for r in range(R)]
 
     def kie_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                   band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200, test_max_size: int = 1920,
@@ -1349,7 +1451,7 @@ class OmniParserB200:
         return out
 
     def _spot_mixed(self, pages, sizes, tile, overlap, max_batch, margin, band, iou, test_min_size, test_max_size,
-                    whole_page=False):
+                    whole_page=False, rec_locations=False):
         """spot_tiled(orientation='mixed'): every page read in tiles at turns 0..3 (reading 4 p + k), one merge of the
         4 P readings, with whole_page each reading merged with its whole-page partner (merge_whole_page), then one
         merge of each page's four readings (merge_turns)."""
@@ -1360,8 +1462,9 @@ class OmniParserB200:
         t4 = np.tile(np.arange(4, dtype=np.int32), P)
         sizes4 = [s for s in sizes for _ in range(4)]
         plan = Pre.omni_tile_plan(Pre.turned_sizes(sizes4, t4), tile, overlap)
-        n_inst, pt, poly, rec, prob = self._decode_tiles([p for p in pages for _ in range(4)], plan, tile, overlap, t4,
-                                                         max_batch, test_min_size, test_max_size, self._decode_arrays)
+        n_inst, pt, poly, rec, prob, *loc = self._decode_tiles(
+            [p for p in pages for _ in range(4)], plan, tile, overlap, t4, max_batch, test_min_size, test_max_size,
+            self._decode_loc_arrays if rec_locations else self._decode_arrays)
         rd = merge_tiles(self.ctx, sizes4, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band,
                          iou, turns=t4)
         tiles_rd, whole = rd, None
@@ -1372,22 +1475,42 @@ class OmniParserB200:
         m = merge_turns(self.ctx, rd['count'], rd['offset'], rd['pts'], rd['polys'], rd['rec'], rd['prob'],
                         v.recog_pad_index, v.rec_eos_index, iou)
         texts, scores = postprocess.rec_texts(m['rec'], m['prob'], v)
+        # each kept row's (tile, instance) in the 4 P readings' plan, through its reading's row
+        page_of = np.repeat(np.arange(P), m['count'])
+        src = rd['source'][rd['offset'][4 * page_of + m['source'][:, 0]] + m['source'][:, 1]].reshape(-1, 2)
+        chars = self._tile_chars(sizes4, plan, t4, m, src, loc[0]) if rec_locations else None
         first_tile = np.searchsorted(plan[:, 0], np.arange(4 * P))
         results = []
         for p in range(P):
             page = []
             for r in range(int(m['offset'][p]), int(m['offset'][p]) + int(m['count'][p])):
-                k, i = int(m['source'][r, 0]), int(m['source'][r, 1])
-                src = rd['source'][int(rd['offset'][4 * p + k]) + i]  # (tile, instance) in the 4 P readings' plan
+                k = int(m['source'][r, 0])
                 page.append({'pts': [[float(m['pts'][r, 0]), float(m['pts'][r, 1])]], 'score': float(scores[r]),
                              'polys': m['polys'][r].reshape(-1, 2).tolist(), 'rec': texts[r],
-                             'tile': _tile_of(src[0], first_tile[4 * p + k]), 'instance': int(src[1]), 'turns': k})
+                             'tile': _tile_of(src[r, 0], first_tile[4 * p + k]), 'instance': int(src[r, 1]), 'turns': k,
+                             **({} if chars is None else {'chars': chars[r]})})
             results.append(page)
         self.last_tiles = dict(plan=plan, n_inst=n_inst, pt=pt, poly=poly, rec=rec, prob=prob, turns=t4,
                                readings=tiles_rd, turn_merge=m)
+        if rec_locations:
+            self.last_tiles.update(loc=loc[0])
         if whole is not None:
             self.last_tiles.update(whole=whole, whole_merge=rd)
         return results
+
+    def _decode_loc_arrays(self):
+        """``_decode_arrays`` with character locations on, the locations appended: (n_inst, pt, poly, rec, prob, loc f32
+        [B, max_inst, rec_length, 5])."""
+        return self._decode_arrays(rec_locations=True) + (self.last_rec_locations,)
+
+    def _tile_chars(self, sizes, plan, turns, rows, source, loc) -> List[List[dict]]:
+        """'chars' of merged rows (rows: a merge's dict, 'polys' and 'rec' in page pixels; source int [K, 2]: each row's
+        (tile, instance) in plan) from the tiles' locations loc [tiles, max_inst, L, 5]: one ``char_boxes`` call."""
+        v = self.vocab
+        source = np.asarray(source, dtype=np.int64).reshape(-1, 2)
+        boxes = char_boxes(self.ctx, sizes, plan, rows['polys'], rows['rec'], loc[source[:, 0], source[:, 1]],
+                           source[:, 0], v.recog_pad_index, v.rec_eos_index, turns=turns)
+        return char_dicts(boxes, rows['rec'], v)
 
     def _probe_turns(self, pages, sizes, max_batch, test_min_size, test_max_size, decode):
         """Every page read whole at turns 0..3 (reading 4 p + k; one tile no smaller than any page) by decode and the

@@ -963,6 +963,30 @@ ALM_API int alm_omni_merge_whole_page(alm_ctx* ctx, const int* heights, const in
                                       int cap_in, int rec_length, int32_t* page_count, int32_t* page_offset,
                                       double* pts_out, double* polys_out, int64_t* rec_out, float* prob_out,
                                       int32_t* source, long cap);
+/* One box per recognised character of words read in tiles, turned or not, in page pixels (DESIGN 4.20; the rule in
+ * full is in rec_box_core.h): the counterpart of postprocess.rec_char_boxes for spot_tiled and read_regions.  Inputs,
+ * HOST buffers, word n of n_words: polys f64 [n_words][32] (its 16 vertices in page pixels, as the merges return
+ * them), rec int64 [n_words][rec_length], loc f32 [n_words][rec_length][5] (the character locations of the tile
+ * instance it came from, (cx, cy, sxx, sxy, syy) normalised by that image's encoded size) and frame_index int32
+ * [n_words] into frames int32 [n_frames][7] = (H, W, turn, y0, x0, h, w): the upright page size, the turn the page was
+ * read at and the tile's origin and size in the turned page (a page read whole: 0, 0 and the page's size, turn 0).
+ *   centre  (x0 + cx w, y0 + cy h) in double, mapped to the upright page as alm_omni_merge_tiles_turned maps points;
+ *   cov     (sxx w w, sxy w h, syy h h), turned with the page: an odd turn swaps sxx and syy and negates sxy;
+ *   chars   the steps decode_seq keeps: stop at recog_pad_index or rec_eos_index, skip recog_pad_index - 1;
+ *   box     rec_char_boxes' rule on the page polygon: nearest point q of the centre line (P_i + P_{15-i}) / 2, unit
+ *           direction u of that segment, local height H, half-width a = sqrt(3) sqrt(u^T cov u); corners q -+ a u -+
+ *           (H / 2) v, v = (-u_y, u_x), top-left, top-right, bottom-right, bottom-left in reading direction.
+ * Every operation in double, rounded on its own; non-finite inputs propagate as NaN.  Outputs, HOST: n_chars int32
+ * [n_words]; per slot [n_words][rec_length] (character i of word n is slot i) step int32 (the rec step it came
+ * from), centre f64 [2], cov f64 [3] = (sxx, sxy, syy) and box f64 [8] = four corners (x, y); slots past n_chars are
+ * 0.  One kernel launch whatever n_words is (one warp per word, no atomics: bit-reproducible), none for n_words = 0.
+ * ALM_ERR_INVALID, before any device work, for n_words < 0, rec_length outside 1..1021, a null buffer or n_frames < 1
+ * (with n_words > 0), a frame index out of range, a turn outside 0..3, a non-positive size or a tile outside its
+ * turned page. */
+ALM_API int alm_omni_char_boxes(alm_ctx* ctx, long n_words, int rec_length, const double* polys, const int64_t* rec,
+                                const float* loc, const int32_t* frame_index, int n_frames, const int32_t* frames,
+                                int recog_pad_index, int rec_eos_index, int32_t* n_chars, int32_t* step,
+                                double* centre, double* cov, double* box);
 /* KIE on pages larger than the model's input or turned by quarter-turns: the entities decoded from every tile merged
  * into page coordinates on the device (DESIGN 4.18; the rule in full is in kie_tile_core.h).  Page p of upright size
  * heights[p] x widths[p], read as np.rot90(page, turns[p]) (turns null = all upright), tiled with (tile, overlap) as
