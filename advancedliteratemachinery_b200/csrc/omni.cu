@@ -321,9 +321,7 @@ OmniModel* omni_share(const OmniModel* owner) {
   m->kpm = nullptr;
   m->kc_hi = m->kc_lo = m->vc_hi = m->vc_lo = m->vt_hi = m->vt_lo = nullptr;
   m->page_mh.clear(); m->page_mw.clear(); m->page_keys.clear();
-  m->cand_ids.clear(); m->cand_probs.clear();
-  m->beam_ids.clear(); m->beam_probs.clear(); m->beam_scores.clear();
-  m->rec_loc.clear();
+  m->rec_lists = {};
   m->dense_loops.clear();
   m->mixed = false;
   m->key_len = m->kb_off = nullptr;
@@ -645,6 +643,8 @@ void omni_encode_pages(Ctx* c, const float* img, int B, int Hc, int Wc, const in
 // ================================================================================================ decode
 namespace {
 
+using Points = std::vector<std::pair<int, int>>;
+
 struct DecodeBufs {
   int S = 0, Tmax = 0, Ncap = 0;
   float* x = nullptr;
@@ -672,60 +672,95 @@ struct DecodeBufs {
   int* loc_counters = nullptr;
 };
 
+// The rows of nd decoders d0 .. d0 + nd - 1 stepped together, and each decoder's rows as single-decoder buffers (its
+// head selection, its cross-attention, the steps its loop runs alone).  nd 2 is the joint polygon + recognition pass:
+// rows [0, S) are the polygon sequences, rows [S, 2S) the recognition sequences.  With nd 1 the view is the rows.
+struct StepBufs {
+  int nd = 1;
+  DecodeBufs all, half[2];
+  DecodeBufs& v(int i) { return nd == 1 ? all : half[i]; }
+};
+
+// nd decoders x B images x Ncap sequences each, caches of Tmax positions (nd 2: the longer loop's, for both halves).
 // pt_loop: the point loop may take the skinny path with up to 16 prompts per image (the fused cross-attention serves
 // them as the rows of its 16-query variant); the poly / rec loops and teacher forcing take it with one sequence per image.
 // img0: first image of the B the buffers serve (its live-key counts size the cross-attention schedule)
-DecodeBufs alloc_decode(Ctx* c, OmniModel* m, int B, int Ncap, int Tmax, bool pt_loop = false, int img0 = 0) {
-  DecodeBufs d;
-  d.S = B * Ncap; d.Tmax = Tmax; d.Ncap = Ncap;
-  const size_t S = d.S;
-  d.x = c->ws.get<float>(S * 512);
-  d.qpos = c->ws.get<float>(512);
+StepBufs alloc_decode(Ctx* c, OmniModel* m, int nd, int B, int Ncap, int Tmax, bool pt_loop, int img0) {
+  StepBufs sb;
+  sb.nd = nd;
+  DecodeBufs& d = sb.all;
+  const size_t S = static_cast<size_t>(B) * Ncap, R = nd * S;  // rows per decoder, rows in all
+  d.S = static_cast<int>(R); d.Tmax = Tmax; d.Ncap = Ncap;
+  d.x = c->ws.get<float>(R * 512);
+  d.qpos = c->ws.get<float>(nd * 512);
   d.tpos = c->ws.get<int>(1);
-  d.ln = alloc_split(c, S * 512);
-  d.lnp = alloc_split(c, S * 512);
-  d.att = alloc_split(c, S * 512);
-  d.q = alloc_split(c, S * 512);
-  d.o = alloc_split(c, S * 512);
-  d.hid = alloc_split(c, S * 2048);
-  d.h0 = alloc_split(c, S * 512);
-  d.h1 = alloc_split(c, S * 512);
-  d.qk = c->ws.get<float>(S * 1024);
-  d.v = c->ws.get<float>(S * 512);
-  d.qf = c->ws.get<float>(S * 512);
-  // xattn_impl 1 has a one-query skinny kernel only (cross_attn_q1)
-  d.skinny = d.S <= 32 && (Ncap == 1 || (pt_loop && Ncap <= 16 && c->xattn_impl != 1));
+  d.ln = alloc_split(c, R * 512);
+  d.lnp = alloc_split(c, R * 512);
+  d.att = alloc_split(c, R * 512);
+  d.q = alloc_split(c, R * 512);
+  d.o = alloc_split(c, R * 512);
+  d.hid = alloc_split(c, R * 2048);
+  d.h0 = alloc_split(c, R * 512);
+  d.h1 = alloc_split(c, R * 512);
+  d.qk = c->ws.get<float>(R * 1024);
+  d.v = c->ws.get<float>(R * 512);
+  d.qf = c->ws.get<float>(R * 512);
+  d.logits = c->ws.get<float>(R * m->V);
+  for (int l = 0; l < 4; ++l) {
+    d.kc[l] = c->ws.get<float>(R * Tmax * 512);
+    d.vc[l] = c->ws.get<float>(R * Tmax * 512);
+  }
+  // xattn_impl 1 has a one-query skinny kernel only (cross_attn_q1); the joint pass has no skinny step
+  d.skinny = nd == 1 && S <= 32 && (Ncap == 1 || (pt_loop && Ncap <= 16 && c->xattn_impl != 1));
   if (d.skinny) {
     d.lnf = c->ws.get<float>(S * 512); d.lnpf = c->ws.get<float>(S * 512); d.attf = c->ws.get<float>(S * 512);
     d.of = c->ws.get<float>(S * 512); d.hidf = c->ws.get<float>(S * 2048); d.h0f = c->ws.get<float>(S * 512);
     d.h1f = c->ws.get<float>(S * 512);
     d.qkv = c->ws.get<float>(S * 1536);
   }
-  if (c->xattn_impl == 0 || c->xattn_impl == 2) {
-    int pairs = 0;
-    d.fused_xattn = true;
-    d.tma_xattn = c->xattn_impl == 2;
-    const int* key_len = m->mixed ? m->page_keys.data() + img0 : nullptr;
-    if (d.tma_xattn) cross_attn_tma_plan(c, B, Ncap, m->M, &d.mq_grid, &d.mq_parts, &pairs, key_len);
-    else cross_attn_mq_plan(c, B, Ncap, m->M, &d.mq_grid, &d.mq_parts, &pairs, key_len);
-    d.xq_partial = c->ws.get<float>(cross_attn_mq_partial_floats(pairs, d.mq_parts));
-    d.xq_counters = c->ws.get<int>(pairs);
-    fill_i32(c, d.xq_counters, pairs, 0);
-  } else if (Ncap == 1) {
-    d.xq_splits = cross_attn_q1_splits(c, B, m->M);
-    d.xq_partial = c->ws.get<float>(static_cast<size_t>(B) * 8 * d.xq_splits * 66);
-    d.xq_counters = c->ws.get<int>(static_cast<size_t>(B) * 8);
-    fill_i32(c, d.xq_counters, static_cast<long>(B) * 8, 0);
-  } else {
-    d.scores = c->ws.get<float>(S * 8 * m->Mpad);
-    d.prob = alloc_split(c, S * 8 * m->Mpad);
+  for (int i = 0; i < nd; ++i) {
+    DecodeBufs& u = sb.v(i);
+    if (nd > 1) {  // decoder i's rows [i S, (i + 1) S) of every buffer
+      const size_t r = i * S;
+      auto rows = [&](const SplitBuf& b, size_t w) { return SplitBuf{b.hi + r * w, b.lo + r * w}; };
+      u = d;
+      u.S = static_cast<int>(S);
+      u.x = d.x + r * 512;
+      u.qpos = d.qpos + i * 512;
+      u.ln = rows(d.ln, 512); u.lnp = rows(d.lnp, 512); u.att = rows(d.att, 512); u.q = rows(d.q, 512);
+      u.o = rows(d.o, 512); u.hid = rows(d.hid, 2048); u.h0 = rows(d.h0, 512); u.h1 = rows(d.h1, 512);
+      u.qk = d.qk + r * 1024;
+      u.v = d.v + r * 512;
+      u.qf = d.qf + r * 512;
+      u.logits = d.logits + r * m->V;
+      for (int l = 0; l < 4; ++l) {
+        u.kc[l] = d.kc[l] + r * Tmax * 512;
+        u.vc[l] = d.vc[l] + r * Tmax * 512;
+      }
+    }
+    // the decoder's own cross-attention schedule: the fused kernels' plan, partials and counters, the one-query
+    // kernel's key splits, or the unfused path's score and probability planes
+    if (c->xattn_impl == 0 || c->xattn_impl == 2) {
+      int pairs = 0;
+      u.fused_xattn = true;
+      u.tma_xattn = c->xattn_impl == 2;
+      const int* key_len = m->mixed ? m->page_keys.data() + img0 : nullptr;
+      if (u.tma_xattn) cross_attn_tma_plan(c, B, Ncap, m->M, &u.mq_grid, &u.mq_parts, &pairs, key_len);
+      else cross_attn_mq_plan(c, B, Ncap, m->M, &u.mq_grid, &u.mq_parts, &pairs, key_len);
+      u.xq_partial = c->ws.get<float>(cross_attn_mq_partial_floats(pairs, u.mq_parts));
+      u.xq_counters = c->ws.get<int>(pairs);
+      fill_i32(c, u.xq_counters, pairs, 0);
+    } else if (Ncap == 1) {
+      u.xq_splits = cross_attn_q1_splits(c, B, m->M);
+      u.xq_partial = c->ws.get<float>(static_cast<size_t>(B) * 8 * u.xq_splits * 66);
+      u.xq_counters = c->ws.get<int>(static_cast<size_t>(B) * 8);
+      fill_i32(c, u.xq_counters, static_cast<long>(B) * 8, 0);
+    } else {
+      u.scores = c->ws.get<float>(S * 8 * m->Mpad);
+      u.prob = alloc_split(c, S * 8 * m->Mpad);
+    }
   }
-  d.logits = c->ws.get<float>(S * m->V);
-  for (int l = 0; l < 4; ++l) {
-    d.kc[l] = c->ws.get<float>(S * Tmax * 512);
-    d.vc[l] = c->ws.get<float>(S * Tmax * 512);
-  }
-  return d;
+  return sb;
 }
 
 // Fused cross-attention of `nimg` images x Ncap queries against decoder-layer dl of the cached K_c / V_c
@@ -757,19 +792,71 @@ void rec_locate_step(Ctx* c, OmniModel* m, DecodeBufs& u, const bf16* q_hi, cons
              u.tpos, 2, u.loc_L, u.loc);
 }
 
-// One decoder pass over the token at position *u.tpos of every sequence (pre-norm layer, transformer.py:430-454,
-// with self-attention K/V cached and the cross-attention K/V precomputed per image).
-// img0: first image of the batch slice the S sequences belong to; nimg images x Ncap sequences each.
-void decoder_step(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens, int tstride, int img0, int nimg,
-                  bool want_logits) {
-  const int S = u.S, Ncap = u.Ncap, M = m->M, Mpad = m->Mpad;
-  // generated rec steps with locations on: the last layer's queries also feed the locate kernel
-  const bool locate = u.loc && d == 2 && want_logits;
-  embed_ln(c, tokens, tstride, u.tpos, S, m->word_emb, m->pos_emb[d], m->emb_norm.g, m->emb_norm.b, u.x, u.qpos);
+// The cross-attention of one decoder's rows `u` against decoder layer dl (d * 4 + l) of the cached K_c / V_c^T of
+// images img0 .. img0 + nimg - 1.  Queries in qf (fp32) on the skinny step or with one query per image, else in the
+// split planes q; the output to of (fp32) on the skinny step, else to the split planes o.  A generated rec step with
+// locations on also hands the last layer's queries to the locate kernel.
+void cross_attn(Ctx* c, OmniModel* m, DecodeBufs& u, long dl, int img0, int nimg, bool want_logits) {
+  const int M = m->M, Mpad = m->Mpad, Ncap = u.Ncap;
+  const bool q32 = u.skinny || Ncap == 1;
+  const bf16 *q_hi = q32 ? nullptr : u.q.hi, *q_lo = q32 ? nullptr : u.q.lo;
+  const float* q_f32 = q32 ? u.qf : nullptr;
+  bf16 *o_hi = u.skinny ? nullptr : u.o.hi, *o_lo = u.skinny ? nullptr : u.o.lo;
+  float* o_f32 = u.skinny ? u.of : nullptr;
+  if (u.loc && want_logits && dl == 11) rec_locate_step(c, m, u, q_hi, q_lo, q_f32, img0, nimg);
+  if (u.fused_xattn) {
+    // scores, mask, online softmax and P.V fused; K_c / V_c streamed once per layer-step (HBM-bound)
+    fused_xattn(c, m, u, q_hi, q_lo, q_f32, img0, nimg, Ncap, dl, o_hi, o_lo, o_f32);
+    return;
+  }
+  const long koff = (static_cast<long>(img0) * 96 + dl * 8) * M * 64;
+  const long voff = (static_cast<long>(img0) * 6144 + dl * 512) * Mpad;
+  if (Ncap == 1) {
+    cross_attn_q1(c, u.qf, m->kc_hi + koff, m->kc_lo + koff, m->vt_hi + voff, m->vt_lo + voff,
+                  m->kpm + static_cast<long>(img0) * M, nimg, M, Mpad, u.xq_partial, u.xq_counters, u.xq_splits, o_hi,
+                  o_lo, o_f32);
+    return;
+  }
+  {
+    Operand a = act_op(u.q.hi, u.q.lo, Ncap, 64, 512);
+    a.nb0 = 8; a.bs0 = 64; a.nb1 = nimg; a.bs1 = static_cast<long>(Ncap) * 512;
+    Operand k = act_op(m->kc_hi + koff, m->kc_lo + koff, M, 64, 64);
+    k.nb0 = 8; k.bs0 = static_cast<long>(M) * 64; k.nb1 = nimg; k.bs1 = static_cast<long>(96) * M * 64;
+    Epilogue e;
+    e.out_f32 = u.scores; e.ldo = Mpad; e.obs0 = static_cast<long>(Ncap) * Mpad; e.obs1 = static_cast<long>(8) * Ncap * Mpad;
+    e.alpha = 0.125f;  // == scaling q by 64^-0.5 before q k^T (exact: power of two)
+    gemm(c, a, k, e);
+  }
+  softmax_rows(c, u.scores, Mpad, static_cast<long>(u.S) * 8, M, m->kpm + static_cast<long>(img0) * M, 8 * Ncap, M,
+               nullptr, u.prob.hi, u.prob.lo, Mpad);
+  {
+    Operand a = act_op(u.prob.hi, u.prob.lo, Ncap, M, Mpad);
+    a.nb0 = 8; a.bs0 = static_cast<long>(Ncap) * Mpad; a.nb1 = nimg; a.bs1 = static_cast<long>(8) * Ncap * Mpad;
+    Operand v = act_op(m->vt_hi + voff, m->vt_lo + voff, 64, M, Mpad);
+    v.nb0 = 8; v.bs0 = static_cast<long>(64) * Mpad; v.nb1 = nimg; v.bs1 = static_cast<long>(6144) * Mpad;
+    Epilogue e;
+    e.out_hi = u.o.hi; e.out_lo = u.o.lo; e.ldo = 512; e.obs0 = 64; e.obs1 = static_cast<long>(Ncap) * 512;
+    gemm(c, a, v, e);
+  }
+}
+
+// One decoder pass over the token at position *tpos of every sequence of decoders d0 .. d0 + b.nd - 1 (pre-norm layer,
+// transformer.py:430-454, with self-attention K/V cached and the cross-attention K/V precomputed per image); decoder
+// d0 + i reads its tokens at tokens[i] (row stride tstride[i]).  img0: first image of the batch slice the sequences
+// belong to; nimg images x Ncap sequences each, per decoder.
+void decoder_step(Ctx* c, OmniModel* m, int d0, StepBufs& b, const int* const tokens[], const int tstride[], int img0,
+                  int nimg, bool want_logits) {
+  DecodeBufs& u = b.all;
+  const int nd = b.nd, d1 = d0 + nd - 1, S = u.S / nd;
+  const bool two = nd == 2;
+  embed_ln(c, tokens[0], tstride[0], u.tpos, u.S, m->word_emb, m->pos_emb[d0], m->emb_norm.g, m->emb_norm.b, u.x, u.qpos,
+           two ? S : 0, two ? tokens[1] : nullptr, two ? tstride[1] : 0, two ? m->pos_emb[d1] : nullptr,
+           two ? u.qpos + 512 : nullptr);
   const float* qpos = u.qpos;
   if (u.skinny) {
     // At most 32 live sequences (one per image, or up to 16 prompts per image in the pt loop): every linear is a skinny
     // fp32 GEMV (exact fp32 weights, one warp per output column), no operand splitting, no tensor-core tile padding.
+    const int d = d0;
     auto lin = [&](const float* x, int K, const Lin& w, int act, float* out, const float* resid) {
       gemv_rows(c, x, nullptr, 1 << 30, K, w.wf, w.b, resid, w.w.N, out, w.w.N, S, w.w.N, K, act);
     };
@@ -783,14 +870,12 @@ void decoder_step(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens,
       };
       for (int l = 0; l < 4; ++l) {
         const DecLayerW& w = m->dec[d][l];
-        const long dl = static_cast<long>(d) * 4 + l;
         lnlin(w.n1, qpos, 1024, w.sa_qkv_f, w.sa_qkv_b, 1536, ACT_NONE, u.qkv, 1536);   // q | k from LN(x)+pos, v from LN(x)
         self_attn_step(c, u.qkv, u.qkv + 1024, u.kc[l], u.vc[l], S, u.tpos, u.Tmax, nullptr, nullptr, u.attf, 1536, 1536,
                        u.anc);
         lin(u.attf, 512, w.sa_out, ACT_NONE, u.x, u.x);
         lnlin(w.n2, qpos, 1 << 30, w.ca_q.wf, w.ca_q.b, 512, ACT_NONE, u.qf, 512);
-        if (locate && l == 3) rec_locate_step(c, m, u, nullptr, nullptr, u.qf, img0, nimg);
-        fused_xattn(c, m, u, nullptr, nullptr, u.qf, img0, nimg, Ncap, dl, nullptr, nullptr, u.of);
+        cross_attn(c, m, u, d * 4 + l, img0, nimg, want_logits);
         lin(u.of, 512, w.ca_out, ACT_NONE, u.x, u.x);
         lnlin(w.n3, nullptr, 0, w.l1.wf, w.l1.b, 2048, ACT_RELU, u.hidf, 2048);
         lin(u.hidf, 2048, w.l2, ACT_NONE, u.x, u.x);
@@ -804,7 +889,6 @@ void decoder_step(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens,
     }
     for (int l = 0; l < 4; ++l) {
       const DecLayerW& w = m->dec[d][l];
-      const long dl = static_cast<long>(d) * 4 + l;
       gather_ln(c, u.x, 512, nullptr, 1, 512, S, w.n1.g, w.n1.b, 1e-5f, false, qpos, 0, u.lnf, 512, nullptr, nullptr, 512,
                 nullptr, nullptr, u.lnpf);
       // q|k from LN(x)+pos and v from LN(x) in ONE launch: the fp32 in_proj rows are contiguous (q, k, v)
@@ -815,15 +899,7 @@ void decoder_step(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens,
       gather_ln(c, u.x, 512, nullptr, 1, 512, S, w.n2.g, w.n2.b, 1e-5f, false, qpos, 0, nullptr, 512, nullptr, nullptr, 512,
                 nullptr, nullptr, u.lnpf);
       lin(u.lnpf, 512, w.ca_q, ACT_NONE, u.qf, nullptr);
-      if (locate && l == 3) rec_locate_step(c, m, u, nullptr, nullptr, u.qf, img0, nimg);
-      const long koff = (static_cast<long>(img0) * 96 + dl * 8) * M * 64;
-      const long voff = (static_cast<long>(img0) * 6144 + dl * 512) * Mpad;
-      if (u.fused_xattn)
-        fused_xattn(c, m, u, nullptr, nullptr, u.qf, img0, nimg, Ncap, dl, nullptr, nullptr, u.of);
-      else
-        cross_attn_q1(c, u.qf, m->kc_hi + koff, m->kc_lo + koff, m->vt_hi + voff, m->vt_lo + voff,
-                      m->kpm + static_cast<long>(img0) * M, nimg, M, Mpad, u.xq_partial, u.xq_counters, u.xq_splits, nullptr,
-                      nullptr, u.of);
+      cross_attn(c, m, u, d * 4 + l, img0, nimg, want_logits);
       lin(u.of, 512, w.ca_out, ACT_NONE, u.x, u.x);
       gather_ln(c, u.x, 512, nullptr, 1, 512, S, w.n3.g, w.n3.b, 1e-5f, false, nullptr, 0, u.lnf, 512, nullptr, nullptr, 512,
                 nullptr, nullptr);
@@ -839,78 +915,52 @@ void decoder_step(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens,
     lin(u.h1f, 512, m->head[d][2], ACT_NONE, u.logits, nullptr);
     return;
   }
+  // Tensor-core step.  Every LayerNorm is one launch over all rows and every linear one GEMM; with nd 2 rows [S, 2S)
+  // take decoder d1's affine, query position and weights (linear2: a batch of two over the load_lin_pair slab), so each
+  // row's arithmetic is the single-decoder step's.
+  auto ln = [&](const LNW& n0, const LNW& n1, bool pos, const SplitBuf& out, const SplitBuf& out_pos) {
+    gather_ln(c, u.x, 512, nullptr, 1, 512, u.S, n0.g, n0.b, 1e-5f, false, pos ? qpos : nullptr, 0, nullptr, 0, out.hi,
+              out.lo, 512, out_pos.hi, out_pos.lo, nullptr, two ? S : 0, two ? n1.g : nullptr, two ? n1.b : nullptr,
+              two && pos ? qpos + 512 : nullptr);
+  };
+  auto lin = [&](const SplitBuf& a, const Lin& l0, const Lin& l1, int act, float* out_f32, SplitBuf* out_split,
+                 bool resid) {
+    if (two) linear2(c, a, S, l0, l1, act, out_f32, out_split, resid ? u.x : nullptr);
+    else linear(c, a, S, l0, act, out_f32, out_split, resid ? u.x : nullptr);
+  };
+  // the self-attention step runs over all rows at once when each decoder's rows alone would take the same kernel
+  auto wide = [&](long rows) { return c->sattn_wide && rows * 8 <= 4L * c->num_sms; };
+  const bool one_sattn = wide(S) == wide(u.S);
   c->skip_scope = true;
   for (int l = 0; l < 4; ++l) {
-    const DecLayerW& w = m->dec[d][l];
-    const long dl = static_cast<long>(d) * 4 + l;
+    const DecLayerW& w = m->dec[d0][l];
+    const DecLayerW& w1 = m->dec[d1][l];
     // --- self attention
-    gather_ln(c, u.x, 512, nullptr, 1, 512, S, w.n1.g, w.n1.b, 1e-5f, false, qpos, 0, nullptr, 0, u.ln.hi, u.ln.lo, 512,
-              u.lnp.hi, u.lnp.lo);
-    linear(c, u.lnp, S, w.sa_qk, ACT_NONE, u.qk, nullptr);
-    linear(c, u.ln, S, w.sa_v, ACT_NONE, u.v, nullptr);
-    self_attn_step(c, u.qk, u.v, u.kc[l], u.vc[l], S, u.tpos, u.Tmax, u.att.hi, u.att.lo, nullptr, 1024, 512, u.anc);
-    linear(c, u.att, S, w.sa_out, ACT_NONE, u.x, nullptr, u.x, nullptr, nullptr, 512);
-    // --- cross attention against the per-image cached K / V^T
-    gather_ln(c, u.x, 512, nullptr, 1, 512, S, w.n2.g, w.n2.b, 1e-5f, false, qpos, 0, nullptr, 0, nullptr, nullptr, 512,
-              u.lnp.hi, u.lnp.lo);
-    if (Ncap == 1) {
-      // one query per image: fused scores + mask + softmax + P.V, K/V streamed once (HBM-bound)
-      linear(c, u.lnp, S, w.ca_q, ACT_NONE, u.qf, nullptr);
-      if (locate && l == 3) rec_locate_step(c, m, u, nullptr, nullptr, u.qf, img0, nimg);
-      const long koff = (static_cast<long>(img0) * 96 + dl * 8) * M * 64;
-      const long voff = (static_cast<long>(img0) * 6144 + dl * 512) * Mpad;
-      if (u.fused_xattn)
-        fused_xattn(c, m, u, nullptr, nullptr, u.qf, img0, nimg, 1, dl, u.o.hi, u.o.lo, nullptr);
-      else
-        cross_attn_q1(c, u.qf, m->kc_hi + koff, m->kc_lo + koff, m->vt_hi + voff, m->vt_lo + voff,
-                      m->kpm + static_cast<long>(img0) * M, nimg, M, Mpad, u.xq_partial, u.xq_counters, u.xq_splits, u.o.hi,
-                      u.o.lo);
-    } else if (u.fused_xattn) {
-      // Ncap queries per image: scores, mask, online softmax and P.V fused; K_c / V_c^T streamed once per layer-step
-      linear(c, u.lnp, S, w.ca_q, ACT_NONE, nullptr, &u.q);
-      if (locate && l == 3) rec_locate_step(c, m, u, u.q.hi, u.q.lo, nullptr, img0, nimg);
-      fused_xattn(c, m, u, u.q.hi, u.q.lo, nullptr, img0, nimg, Ncap, dl, u.o.hi, u.o.lo, nullptr);
-    } else {
-      linear(c, u.lnp, S, w.ca_q, ACT_NONE, nullptr, &u.q);
-      if (locate && l == 3) rec_locate_step(c, m, u, u.q.hi, u.q.lo, nullptr, img0, nimg);
-      {
-        Operand a = act_op(u.q.hi, u.q.lo, Ncap, 64, 512);
-        a.nb0 = 8; a.bs0 = 64; a.nb1 = nimg; a.bs1 = static_cast<long>(Ncap) * 512;
-        const long koff = (static_cast<long>(img0) * 96 + dl * 8) * M * 64;
-        Operand k = act_op(m->kc_hi + koff, m->kc_lo + koff, M, 64, 64);
-        k.nb0 = 8; k.bs0 = static_cast<long>(M) * 64; k.nb1 = nimg; k.bs1 = static_cast<long>(96) * M * 64;
-        Epilogue e;
-        e.out_f32 = u.scores; e.ldo = Mpad; e.obs0 = static_cast<long>(Ncap) * Mpad; e.obs1 = static_cast<long>(8) * Ncap * Mpad;
-        e.alpha = 0.125f;  // == scaling q by 64^-0.5 before q k^T (exact: power of two)
-        gemm(c, a, k, e);
-      }
-      softmax_rows(c, u.scores, Mpad, static_cast<long>(S) * 8, M, m->kpm + static_cast<long>(img0) * M, 8 * Ncap, M,
-                   nullptr, u.prob.hi, u.prob.lo, Mpad);
-      {
-        Operand a = act_op(u.prob.hi, u.prob.lo, Ncap, M, Mpad);
-        a.nb0 = 8; a.bs0 = static_cast<long>(Ncap) * Mpad; a.nb1 = nimg; a.bs1 = static_cast<long>(8) * Ncap * Mpad;
-        const long voff = (static_cast<long>(img0) * 6144 + dl * 512) * Mpad;
-        Operand v = act_op(m->vt_hi + voff, m->vt_lo + voff, 64, M, Mpad);
-        v.nb0 = 8; v.bs0 = static_cast<long>(64) * Mpad; v.nb1 = nimg; v.bs1 = static_cast<long>(6144) * Mpad;
-        Epilogue e;
-        e.out_hi = u.o.hi; e.out_lo = u.o.lo; e.ldo = 512; e.obs0 = 64; e.obs1 = static_cast<long>(Ncap) * 512;
-        gemm(c, a, v, e);
-      }
+    ln(w.n1, w1.n1, true, u.ln, u.lnp);
+    lin(u.lnp, w.sa_qk, w1.sa_qk, ACT_NONE, u.qk, nullptr, false);
+    lin(u.ln, w.sa_v, w1.sa_v, ACT_NONE, u.v, nullptr, false);
+    for (int i = 0; i < (one_sattn ? 1 : nd); ++i) {
+      DecodeBufs& v = one_sattn ? u : b.v(i);
+      self_attn_step(c, v.qk, v.v, v.kc[l], v.vc[l], v.S, v.tpos, v.Tmax, v.att.hi, v.att.lo, nullptr, 1024, 512, v.anc);
     }
-    linear(c, u.o, S, w.ca_out, ACT_NONE, u.x, nullptr, u.x, nullptr, nullptr, 512);
+    lin(u.att, w.sa_out, w1.sa_out, ACT_NONE, u.x, nullptr, true);
+    // --- cross attention, each decoder against its own layer of the per-image cached K / V^T
+    ln(w.n2, w1.n2, true, SplitBuf{}, u.lnp);
+    if (u.Ncap == 1) lin(u.lnp, w.ca_q, w1.ca_q, ACT_NONE, u.qf, nullptr, false);
+    else lin(u.lnp, w.ca_q, w1.ca_q, ACT_NONE, nullptr, &u.q, false);
+    for (int i = 0; i < nd; ++i) cross_attn(c, m, b.v(i), (d0 + i) * 4 + l, img0, nimg, want_logits);
+    lin(u.o, w.ca_out, w1.ca_out, ACT_NONE, u.x, nullptr, true);
     // --- FFN
-    gather_ln(c, u.x, 512, nullptr, 1, 512, S, w.n3.g, w.n3.b, 1e-5f, false, nullptr, 0, nullptr, 0, u.ln.hi, u.ln.lo,
-              512, nullptr, nullptr);
-    linear(c, u.ln, S, w.l1, ACT_RELU, nullptr, &u.hid);
-    linear(c, u.hid, S, w.l2, ACT_NONE, u.x, nullptr, u.x, nullptr, nullptr, 512);
+    ln(w.n3, w1.n3, false, u.ln, SplitBuf{});
+    lin(u.ln, w.l1, w1.l1, ACT_RELU, nullptr, &u.hid, false);
+    lin(u.hid, w.l2, w1.l2, ACT_NONE, u.x, nullptr, true);
   }
   c->skip_scope = false;
   if (!want_logits) return;
-  gather_ln(c, u.x, 512, nullptr, 1, 512, S, m->dec_norm[d].g, m->dec_norm[d].b, 1e-5f, false, nullptr, 0, nullptr, 0,
-            u.ln.hi, u.ln.lo, 512, nullptr, nullptr);
-  linear(c, u.ln, S, m->head[d][0], ACT_RELU, nullptr, &u.h0);
-  linear(c, u.h0, S, m->head[d][1], ACT_RELU, nullptr, &u.h1);
-  linear(c, u.h1, S, m->head[d][2], ACT_NONE, u.logits, nullptr);
+  ln(m->dec_norm[d0], m->dec_norm[d1], false, u.ln, SplitBuf{});
+  lin(u.ln, m->head[d0][0], m->head[d1][0], ACT_RELU, nullptr, &u.h0, false);
+  lin(u.h0, m->head[d0][1], m->head[d1][1], ACT_RELU, nullptr, &u.h1, false);
+  lin(u.h1, m->head[d0][2], m->head[d1][2], ACT_NONE, u.logits, nullptr, false);
 }
 
 // Sleep (do not spin) until everything enqueued on `s` has finished.  The decode loops wait for the GPU several
@@ -1007,29 +1057,24 @@ void run_graph(Ctx* c, OmniModel* m, const std::vector<long>& key, int n, const 
   c->launches += it->second.launches * n;
 }
 
-// `n` consecutive token steps of decoder d.
-void run_steps(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int* tokens, int tstride, int img0, int nimg, int n,
-               const HeadArgs& h) {
+// `n` consecutive token steps of decoders d0 .. d0 + b.nd - 1: their layers, then each decoder's head selection, then
+// the shared position counter.  One graph key per decoder, joined by -1 (no single-decoder key has that length).
+void run_steps(Ctx* c, OmniModel* m, int d0, StepBufs& b, const int* const tokens[], const int tstride[], int img0,
+               int nimg, int n, const HeadArgs h[]) {
   if (n <= 0) return;
-  run_graph(c, m, step_key(c, m, d, u, tokens, tstride, img0, nimg, h), n, [&] {
-    decoder_step(c, m, d, u, tokens, tstride, img0, nimg, h.on);
-    select_heads(c, m, d, u, h);
-    add_i32(c, u.tpos, 1);
+  ALM_REQUIRE(h[0].on == h[b.nd - 1].on, ALM_ERR_STATE, "joint decoder step: both halves select or neither");
+  std::vector<long> key;
+  for (int i = 0; i < b.nd; ++i) {
+    const std::vector<long> k = step_key(c, m, d0 + i, b.v(i), tokens[i], tstride[i], img0, nimg, h[i]);
+    if (i > 0) key.push_back(-1);
+    key.insert(key.end(), k.begin(), k.end());
+  }
+  run_graph(c, m, key, n, [&] {
+    decoder_step(c, m, d0, b, tokens, tstride, img0, nimg, h[0].on);
+    for (int i = 0; i < b.nd; ++i) select_heads(c, m, d0 + i, b.v(i), h[i]);
+    add_i32(c, b.all.tpos, 1);
   });
 }
-
-// ------------------------------------------------------------------ joint polygon + recognition pass
-// The polygon and the recognition loop decode the same instances from the same prompt shape, so while both have steps
-// left they run as ONE pass: rows [0, S) are the polygon sequences, rows [S, 2S) the recognition sequences, and every
-// linear and LayerNorm of a layer is one launch over both (each row with its own decoder's weights).  The
-// cross-attention runs once per decoder, each with its own key-split plan, so every kernel computes what the
-// single-decoder step computes, bit for bit.
-struct JointBufs {
-  DecodeBufs j;     // both decoders' rows
-  DecodeBufs h[2];  // the halves as single-decoder buffers: head selection, cross-attention, steps one loop runs alone
-};
-
-SplitBuf half_of(const SplitBuf& b, size_t off) { return SplitBuf{b.hi + off, b.lo + off}; }
 
 // The joint pass serves the tensor-core step of the fused cross-attention over one row per instance; the fp32 GEMV
 // step (<= 32 single-instance sequences), the unfused cross-attention and beam search keep the single-decoder steps,
@@ -1039,145 +1084,6 @@ bool joint_pass_ok(Ctx* c, int B, int Ncap, bool beams) {
   return c->joint_decode && !skinny && !beams && (c->xattn_impl == 0 || c->xattn_impl == 2);
 }
 
-// B images x Ncap sequences per decoder, caches of Tmax positions (the longer loop's) for both halves
-JointBufs alloc_joint(Ctx* c, OmniModel* m, int B, int Ncap, int Tmax, int img0) {
-  JointBufs jb;
-  DecodeBufs& d = jb.j;
-  const size_t S = static_cast<size_t>(B) * Ncap, S2 = 2 * S;
-  d.S = static_cast<int>(S2); d.Tmax = Tmax; d.Ncap = Ncap;
-  d.x = c->ws.get<float>(S2 * 512);
-  d.qpos = c->ws.get<float>(2 * 512);
-  d.tpos = c->ws.get<int>(1);
-  d.ln = alloc_split(c, S2 * 512);
-  d.lnp = alloc_split(c, S2 * 512);
-  d.att = alloc_split(c, S2 * 512);
-  d.q = alloc_split(c, S2 * 512);
-  d.o = alloc_split(c, S2 * 512);
-  d.hid = alloc_split(c, S2 * 2048);
-  d.h0 = alloc_split(c, S2 * 512);
-  d.h1 = alloc_split(c, S2 * 512);
-  d.qk = c->ws.get<float>(S2 * 1024);
-  d.v = c->ws.get<float>(S2 * 512);
-  d.qf = c->ws.get<float>(S2 * 512);
-  d.logits = c->ws.get<float>(S2 * m->V);
-  for (int l = 0; l < 4; ++l) {
-    d.kc[l] = c->ws.get<float>(S2 * Tmax * 512);
-    d.vc[l] = c->ws.get<float>(S2 * Tmax * 512);
-  }
-  d.fused_xattn = true;
-  d.tma_xattn = c->xattn_impl == 2;
-  const int* key_len = m->mixed ? m->page_keys.data() + img0 : nullptr;
-  for (int h = 0; h < 2; ++h) {
-    DecodeBufs& u = jb.h[h];
-    u = d;
-    u.S = static_cast<int>(S);
-    u.x = d.x + h * S * 512;
-    u.qpos = d.qpos + h * 512;
-    u.ln = half_of(d.ln, h * S * 512);
-    u.lnp = half_of(d.lnp, h * S * 512);
-    u.att = half_of(d.att, h * S * 512);
-    u.q = half_of(d.q, h * S * 512);
-    u.o = half_of(d.o, h * S * 512);
-    u.hid = half_of(d.hid, h * S * 2048);
-    u.h0 = half_of(d.h0, h * S * 512);
-    u.h1 = half_of(d.h1, h * S * 512);
-    u.qk = d.qk + h * S * 1024;
-    u.v = d.v + h * S * 512;
-    u.qf = d.qf + h * S * 512;
-    u.logits = d.logits + h * S * m->V;
-    for (int l = 0; l < 4; ++l) {
-      u.kc[l] = d.kc[l] + h * S * Tmax * 512;
-      u.vc[l] = d.vc[l] + h * S * Tmax * 512;
-    }
-    // each decoder's own cross-attention plan, partials and counters (alloc_decode's)
-    int pairs = 0;
-    if (u.tma_xattn) cross_attn_tma_plan(c, B, Ncap, m->M, &u.mq_grid, &u.mq_parts, &pairs, key_len);
-    else cross_attn_mq_plan(c, B, Ncap, m->M, &u.mq_grid, &u.mq_parts, &pairs, key_len);
-    u.xq_partial = c->ws.get<float>(cross_attn_mq_partial_floats(pairs, u.mq_parts));
-    u.xq_counters = c->ws.get<int>(pairs);
-    fill_i32(c, u.xq_counters, pairs, 0);
-  }
-  return jb;
-}
-
-// One token of both decoders (decoder_step's tensor-core branch, layer by layer, over the joint rows).
-void joint_step(Ctx* c, OmniModel* m, JointBufs& jb, const int* const tokens[2], const int tstride[2], int img0, int nimg,
-                bool want_logits) {
-  DecodeBufs& u = jb.j;
-  const long S = jb.h[0].S;
-  const int Ncap = u.Ncap;
-  const bool locate = jb.h[1].loc && want_logits;
-  embed_ln(c, tokens[0], tstride[0], u.tpos, u.S, m->word_emb, m->pos_emb[1], m->emb_norm.g, m->emb_norm.b, u.x, u.qpos,
-           static_cast<int>(S), tokens[1], tstride[1], m->pos_emb[2], u.qpos + 512);
-  const float *qpos = u.qpos, *qpos2 = u.qpos + 512;
-  // the self-attention step runs over both halves at once when each half alone would take the same kernel
-  auto wide = [&](long rows) { return c->sattn_wide && rows * 8 <= 4L * c->num_sms; };
-  const bool one_sattn = wide(S) == wide(2 * S);
-  c->skip_scope = true;
-  for (int l = 0; l < 4; ++l) {
-    const DecLayerW& w = m->dec[1][l];
-    const DecLayerW& w2 = m->dec[2][l];
-    // --- self attention
-    gather_ln(c, u.x, 512, nullptr, 1, 512, u.S, w.n1.g, w.n1.b, 1e-5f, false, qpos, 0, nullptr, 0, u.ln.hi, u.ln.lo, 512,
-              u.lnp.hi, u.lnp.lo, nullptr, S, w2.n1.g, w2.n1.b, qpos2);
-    linear2(c, u.lnp, S, w.sa_qk, w2.sa_qk, ACT_NONE, u.qk, nullptr);
-    linear2(c, u.ln, S, w.sa_v, w2.sa_v, ACT_NONE, u.v, nullptr);
-    if (one_sattn) {
-      self_attn_step(c, u.qk, u.v, u.kc[l], u.vc[l], u.S, u.tpos, u.Tmax, u.att.hi, u.att.lo, nullptr, 1024, 512, nullptr);
-    } else {
-      for (DecodeBufs& v : jb.h)
-        self_attn_step(c, v.qk, v.v, v.kc[l], v.vc[l], v.S, v.tpos, v.Tmax, v.att.hi, v.att.lo, nullptr, 1024, 512, nullptr);
-    }
-    linear2(c, u.att, S, w.sa_out, w2.sa_out, ACT_NONE, u.x, nullptr, u.x);
-    // --- cross attention, each decoder against its own layer of the cached K / V
-    gather_ln(c, u.x, 512, nullptr, 1, 512, u.S, w.n2.g, w.n2.b, 1e-5f, false, qpos, 0, nullptr, 0, nullptr, nullptr, 512,
-              u.lnp.hi, u.lnp.lo, nullptr, S, w2.n2.g, w2.n2.b, qpos2);
-    if (Ncap == 1) linear2(c, u.lnp, S, w.ca_q, w2.ca_q, ACT_NONE, u.qf, nullptr);
-    else linear2(c, u.lnp, S, w.ca_q, w2.ca_q, ACT_NONE, nullptr, &u.q);
-    for (int h = 0; h < 2; ++h) {
-      DecodeBufs& v = jb.h[h];
-      const long dl = static_cast<long>(1 + h) * 4 + l;
-      if (Ncap == 1) {
-        if (h == 1 && locate && l == 3) rec_locate_step(c, m, v, nullptr, nullptr, v.qf, img0, nimg);
-        fused_xattn(c, m, v, nullptr, nullptr, v.qf, img0, nimg, 1, dl, v.o.hi, v.o.lo, nullptr);
-      } else {
-        if (h == 1 && locate && l == 3) rec_locate_step(c, m, v, v.q.hi, v.q.lo, nullptr, img0, nimg);
-        fused_xattn(c, m, v, v.q.hi, v.q.lo, nullptr, img0, nimg, Ncap, dl, v.o.hi, v.o.lo, nullptr);
-      }
-    }
-    linear2(c, u.o, S, w.ca_out, w2.ca_out, ACT_NONE, u.x, nullptr, u.x);
-    // --- FFN
-    gather_ln(c, u.x, 512, nullptr, 1, 512, u.S, w.n3.g, w.n3.b, 1e-5f, false, nullptr, 0, nullptr, 0, u.ln.hi, u.ln.lo,
-              512, nullptr, nullptr, nullptr, S, w2.n3.g, w2.n3.b, nullptr);
-    linear2(c, u.ln, S, w.l1, w2.l1, ACT_RELU, nullptr, &u.hid);
-    linear2(c, u.hid, S, w.l2, w2.l2, ACT_NONE, u.x, nullptr, u.x);
-  }
-  c->skip_scope = false;
-  if (!want_logits) return;
-  gather_ln(c, u.x, 512, nullptr, 1, 512, u.S, m->dec_norm[1].g, m->dec_norm[1].b, 1e-5f, false, nullptr, 0, nullptr, 0,
-            u.ln.hi, u.ln.lo, 512, nullptr, nullptr, nullptr, S, m->dec_norm[2].g, m->dec_norm[2].b, nullptr);
-  linear2(c, u.ln, S, m->head[1][0], m->head[2][0], ACT_RELU, nullptr, &u.h0);
-  linear2(c, u.h0, S, m->head[1][1], m->head[2][1], ACT_RELU, nullptr, &u.h1);
-  linear2(c, u.h1, S, m->head[1][2], m->head[2][2], ACT_NONE, u.logits, nullptr);
-}
-
-// n joint steps: both decoders' layers, then each decoder's head selection, then the shared position counter.
-void run_joint(Ctx* c, OmniModel* m, JointBufs& jb, const int* const tokens[2], const int tstride[2], int img0, int nimg,
-               int n, const HeadArgs h[2]) {
-  if (n <= 0) return;
-  ALM_REQUIRE(h[0].on == h[1].on, ALM_ERR_STATE, "joint decoder step: both halves select or neither");
-  std::vector<long> key = step_key(c, m, 1, jb.h[0], tokens[0], tstride[0], img0, nimg, h[0]);
-  const std::vector<long> k2 = step_key(c, m, 2, jb.h[1], tokens[1], tstride[1], img0, nimg, h[1]);
-  key.push_back(-1);  // joint: no single-decoder key has this length
-  key.insert(key.end(), k2.begin(), k2.end());
-  run_graph(c, m, key, n, [&] {
-    joint_step(c, m, jb, tokens, tstride, img0, nimg, h[0].on);
-    select_heads(c, m, 1, jb.h[0], h[0]);
-    select_heads(c, m, 2, jb.h[1], h[1]);
-    add_i32(c, jb.j.tpos, 1);
-  });
-}
-
 // The point loop (transformer.py:102-141) of images img0 .. img0 + nimg - 1 with P prompts each: sequence
 // (b - img0) P + p of pt_tok [S][n_prompt + pt_steps], prompt tokens first, EOS per sequence in finished / ntok
 // (zeroed by the caller).  Runs in chunks of 16 steps with one small sync after each to stop once every sequence chose
@@ -1185,10 +1091,11 @@ void run_joint(Ctx* c, OmniModel* m, JointBufs& jb, const int* const tokens[2], 
 bool pt_loop(Ctx* c, OmniModel* m, const HeadCfg& hc, int img0, int nimg, int P, int n_prompt, int pt_steps,
              bool check_last, int* pt_tok, float* pt_prob, int* finished, int* ntok) {
   const int S = nimg * P, Tpt = n_prompt + pt_steps;
-  DecodeBufs u = alloc_decode(c, m, nimg, P, Tpt - 1, true, img0);
-  fill_i32(c, u.tpos, 1, 0);
+  StepBufs u = alloc_decode(c, m, 1, nimg, P, Tpt - 1, true, img0);
+  fill_i32(c, u.all.tpos, 1, 0);
+  const int* const tok[1] = {pt_tok};
   HeadArgs off;
-  run_steps(c, m, 0, u, pt_tok, Tpt, img0, nimg, n_prompt - 1, off);  // prompt tokens only fill the caches
+  run_steps(c, m, 0, u, tok, &Tpt, img0, nimg, n_prompt - 1, &off);  // prompt tokens only fill the caches
   HeadArgs h;
   h.on = true; h.cfg = hc; h.tokens = pt_tok; h.tstride = Tpt; h.n_prompt_m1 = n_prompt - 1;
   h.probs = pt_prob; h.pstride = pt_steps;
@@ -1197,7 +1104,7 @@ bool pt_loop(Ctx* c, OmniModel* m, const HeadCfg& hc, int img0, int nimg, int P,
   bool all_done = false;
   for (int done = 0; done < pt_steps && !all_done;) {
     const int chunk = std::min(16, pt_steps - done);
-    run_steps(c, m, 0, u, pt_tok, Tpt, img0, nimg, chunk, h);
+    run_steps(c, m, 0, u, tok, &Tpt, img0, nimg, chunk, &h);
     done += chunk;
     if (done < pt_steps || check_last) {  // every sequence hit EOS?  (one small sync per 16 tokens)
       wait_stream(c, c->stream);
@@ -1248,71 +1155,50 @@ struct Level0 {
   std::vector<int> ntok, tok;
 };
 
-// Polygon and recognition loops (transformer.py:249-284 ; :153-185 for KIE) of the encoded batch at given points.
-// uniq[b] lists the (x, y) bins of image b, one row per entry (Ncap = the longest list; a shorter image pads with dead
-// rows 0, 0, sos); instance n of slot q (image q / P) takes the result of entry slot_inst[q][n] of its image.  Writes
-// poly / rec / rec_prob in alm_omni_decode's layout with maxI rows per slot, and keeps the candidate / beam / location
-// lists of the context's settings in the model.  alm_omni_decode, _prompts, _kie and _at run them here.
-void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P, int maxI,
-                    const std::vector<std::vector<std::pair<int, int>>>& uniq, const std::vector<std::vector<int>>& slot_inst,
-                    int64_t* poly, int64_t* rec, float* rec_prob) {
+// What poly_rec returns on the host, per row r (page-major, Ncap rows per page): tok[d] [r][3 + length] ([x, y, sos] +
+// generated) and prob[d] [r][length] of the polygon (d 1) and the recognition loop (d 2; with beams none, their
+// hypothesis 0 is the reading), candidates [r][rec_length][K], n-best lists ids / probs [r][W][rec_length] and scores
+// [r][W], locations [r][rec_length][5]; each list empty unless its option is on.
+struct PolyRec {
+  std::vector<int> tok[3], cand_ids, beam_ids;
+  std::vector<float> prob[3], cand_probs, beam_probs, beam_scores, loc;
+};
+
+// Polygon and recognition loops (transformer.py:249-284 ; :153-185 for KIE) of pages img0 .. img0 + pts.size() - 1,
+// Ncap rows per page: row n of page img0 + i is [x, y, sos] of pts[i][n], a dead row 0, 0, sos past pts[i]'s end.  The
+// context's rec_topk / rec_beams / rec_locations add candidates, beam search or locations to the recognition loop.
+// The two loops only depend on the points, not on each other.  With one row per instance they run as one joint pass
+// while both have steps left, then the longer loop finishes alone; otherwise (beams, the fp32 GEMV step, the unfused
+// cross-attention) they run concurrently on two streams.  `done` (if any) is recorded on the caller's stream once every
+// loop is enqueued.
+PolyRec poly_rec(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int img0, const std::vector<Points>& pts, int Ncap,
+                 cudaEvent_t done) {
   OmniModel* m = c->omni;
   Arena& ws = c->ws;
-  const int B = m->B, S = static_cast<int>(slot_inst.size());
+  const int nimg = static_cast<int>(pts.size()), Si = nimg * Ncap;  // poly / rec instances
   const int K = c->rec_topk, Wb = c->rec_beams;
   const bool Lc = c->rec_locations;
-  int Ncap = 0;
-  for (const auto& u : uniq) Ncap = std::max(Ncap, static_cast<int>(u.size()));
-  std::vector<int64_t> cand_ids, beam_ids;
-  std::vector<float> cand_probs, beam_probs, beam_scores, rec_loc;
-  if (K > 0) {  // [slot][max_inst][rec_length][K]; instances past n_inst stay 0
-    cand_ids.assign(static_cast<size_t>(S) * maxI * cfg.rec_length * K, 0);
-    cand_probs.assign(cand_ids.size(), 0.f);
-  }
-  if (Wb > 0) {  // ids / probs [slot][max_inst][W][rec_length], scores [slot][max_inst][W]; instances past n_inst stay 0
-    beam_ids.assign(static_cast<size_t>(S) * maxI * Wb * cfg.rec_length, 0);
-    beam_probs.assign(beam_ids.size(), 0.f);
-    beam_scores.assign(static_cast<size_t>(S) * maxI * Wb, 0.f);
-  }
-  if (Lc) rec_loc.assign(static_cast<size_t>(S) * maxI * cfg.rec_length * 5, 0.f);  // [slot][max_inst][rec_length][5]
-  auto keep_lists = [&] {
-    m->cand_ids.swap(cand_ids);
-    m->cand_probs.swap(cand_probs);
-    m->beam_ids.swap(beam_ids);
-    m->beam_probs.swap(beam_probs);
-    m->beam_scores.swap(beam_scores);
-    m->rec_loc.swap(rec_loc);
-  };
-  if (Ncap == 0) {
-    keep_lists();
-    return;
-  }
-
-  // ------------------------------------------------------------------ poly / rec loops (:249-284 ; :153-185 for KIE)
-  // The two loops only depend on the decoded points, not on each other.  With one row per instance they run as one
-  // joint pass (joint_step) while both have steps left, then the longer loop finishes alone; otherwise (beams, the
-  // fp32 GEMV step, the unfused cross-attention) they run concurrently on two streams.
+  const int lens[3] = {0, cfg.poly_length, cfg.rec_length};
   if (!c->stream2) ALM_CHECK_CUDA(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
   if (!c->ev_fork) {
     ALM_CHECK_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
     ALM_CHECK_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
   }
   cudaStream_t s0 = c->stream, s1 = c->decode_streams == 2 ? c->stream2 : c->stream;
-  const int Si = B * Ncap;  // poly / rec instances
   // sequences per instance: the rec loop with beams runs the W hypotheses of an instance as adjacent rows of its image
   const int rows_per[3] = {1, 1, Wb > 0 ? Wb : 1};
   int* toks[3] = {nullptr, nullptr, nullptr};
   float* prbs[3] = {nullptr, nullptr, nullptr};
   std::vector<int> h_prompt[3];
-  for (int phase = 1; phase <= 2; ++phase) {  // [x, y, sos] per instance (transformer.py:252,268 ; :153,172); dead slots 0,0,sos
-    const int T = 3 + (phase == 1 ? cfg.poly_length : cfg.rec_length), R = rows_per[phase];
+  for (int phase = 1; phase <= 2; ++phase) {  // [x, y, sos] per instance (transformer.py:252,268 ; :153,172); dead rows 0,0,sos
+    const int T = 3 + lens[phase], R = rows_per[phase];
     h_prompt[phase].assign(static_cast<size_t>(Si) * R * T, 0);
-    for (int b = 0; b < B; ++b)
+    for (int b = 0; b < nimg; ++b)
       for (int n = 0; n < Ncap; ++n)
         for (int w = 0; w < R; ++w) {
           int* row = &h_prompt[phase][((static_cast<size_t>(b) * Ncap + n) * R + w) * T];
-          if (n < static_cast<int>(uniq[b].size())) {
-            row[0] = uniq[b][n].first; row[1] = uniq[b][n].second;
+          if (n < static_cast<int>(pts[b].size())) {
+            row[0] = pts[b][n].first; row[1] = pts[b][n].second;
           }
           row[2] = phase == 1 ? cfg.poly_sos : cfg.rec_sos;
         }
@@ -1321,7 +1207,7 @@ void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P,
     ALM_CHECK_CUDA(cudaMemcpyAsync(toks[phase], h_prompt[phase].data(), h_prompt[phase].size() * sizeof(int),
                                    cudaMemcpyHostToDevice, s0));
   }
-  // rec candidates on the device: [B * Ncap sequences][rec_length][K], every entry written by the rec loop
+  // rec candidates on the device: [Si sequences][rec_length][K], every entry written by the rec loop
   const size_t cand_n = static_cast<size_t>(Si) * cfg.rec_length * K;
   int* d_cand_ids = K > 0 ? ws.get<int>(cand_n) : nullptr;
   float* d_cand_probs = K > 0 ? ws.get<float>(cand_n) : nullptr;
@@ -1333,10 +1219,9 @@ void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P,
   int* d_bids = Wb > 0 ? ws.get<int>(bl_n) : nullptr;
   float* d_bprobs = Wb > 0 ? ws.get<float>(bl_n) : nullptr;
   float* d_bscores = Wb > 0 ? ws.get<float>(nb) : nullptr;
-  // character locations on the device: [B * Ncap sequences][rec_length][5], every entry written by the rec loop
+  // character locations on the device: [Si sequences][rec_length][5], every entry written by the rec loop
   const size_t loc_n = Lc ? static_cast<size_t>(Si) * cfg.rec_length * 5 : 0;
   float* d_loc = Lc ? ws.get<float>(loc_n) : nullptr;
-  const int lens[3] = {0, cfg.poly_length, cfg.rec_length};
   auto heads = [&](int phase) {  // head selection of the polygon (1) or recognition (2) loop
     HeadArgs h;
     h.on = true; h.cfg = hc; h.tokens = toks[phase]; h.tstride = 3 + lens[phase]; h.n_prompt_m1 = 2;
@@ -1349,7 +1234,7 @@ void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P,
   auto locations = [&](DecodeBufs& u) {  // the rec loop's character locations
     size_t pf = 0;
     int groups = 0;
-    rec_locate_plan(c, B, Ncap, m->M, m->mixed ? m->page_keys.data() : nullptr, &u.loc_ks, &pf, &groups);
+    rec_locate_plan(c, nimg, Ncap, m->M, m->mixed ? m->page_keys.data() + img0 : nullptr, &u.loc_ks, &pf, &groups);
     u.loc = d_loc;
     u.loc_L = lens[2];
     u.loc_partial = ws.get<float>(pf);
@@ -1357,37 +1242,38 @@ void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P,
     // a memset, not a kernel: locations add exactly one launch per generated rec step
     ALM_CHECK_CUDA(cudaMemsetAsync(u.loc_counters, 0, groups * sizeof(int), c->stream));
   };
-  if (joint_pass_ok(c, B, Ncap, Wb > 0)) {
-    JointBufs jb = alloc_joint(c, m, B, Ncap, 2 + std::max(lens[1], lens[2]), 0);
-    fill_i32(c, jb.j.tpos, 1, 0);
-    if (Lc) locations(jb.h[1]);
-    const int* jt[2] = {toks[1], toks[2]};
+  if (joint_pass_ok(c, nimg, Ncap, Wb > 0)) {
+    StepBufs jb = alloc_decode(c, m, 2, nimg, Ncap, 2 + std::max(lens[1], lens[2]), false, img0);
+    fill_i32(c, jb.all.tpos, 1, 0);
+    if (Lc) locations(jb.half[1]);
+    const int* const jt[2] = {toks[1], toks[2]};
     const int js[2] = {3 + lens[1], 3 + lens[2]};
     const HeadArgs off[2], hs[2] = {heads(1), heads(2)};
-    run_joint(c, m, jb, jt, js, 0, B, 2, off);  // the prompts [x, y, sos] only fill the caches
+    run_steps(c, m, 1, jb, jt, js, img0, nimg, 2, off);  // the prompts [x, y, sos] only fill the caches
     const int both = std::min(lens[1], lens[2]);
-    run_joint(c, m, jb, jt, js, 0, B, both, hs);
-    for (int phase = 1; phase <= 2; ++phase)  // the longer loop alone
-      run_steps(c, m, phase, jb.h[phase - 1], toks[phase], js[phase - 1], 0, B, lens[phase] - both, hs[phase - 1]);
+    run_steps(c, m, 1, jb, jt, js, img0, nimg, both, hs);
+    for (int i = 0; i < 2; ++i) {  // the longer loop alone
+      StepBufs alone{1, jb.half[i]};
+      run_steps(c, m, 1 + i, alone, &jt[i], &js[i], img0, nimg, lens[1 + i] - both, &hs[i]);
+    }
   } else {
     ALM_CHECK_CUDA(cudaEventRecord(c->ev_fork, s0));
     ALM_CHECK_CUDA(cudaStreamWaitEvent(s1, c->ev_fork, 0));
     try {
       for (int phase = 1; phase <= 2; ++phase) {
         c->stream = (phase == 1) ? s0 : s1;
-        const int len = lens[phase];
-        const int T = 3 + len;
+        const int len = lens[phase], T = 3 + len;
         const bool beams = phase == 2 && Wb > 0;
-        DecodeBufs u = alloc_decode(c, m, B, Ncap * rows_per[phase], T - 1);
-        fill_i32(c, u.tpos, 1, 0);
+        StepBufs u = alloc_decode(c, m, 1, nimg, Ncap * rows_per[phase], T - 1, false, img0);
+        fill_i32(c, u.all.tpos, 1, 0);
         if (beams) {  // the prompt [x, y, sos] is cached in every beam's own row
           anc_identity(c, d_anc, static_cast<int>(nb), T - 1);
-          u.anc = d_anc;
+          u.all.anc = d_anc;
         }
-        if (phase == 2 && Lc) locations(u);
-        HeadArgs off;
-        run_steps(c, m, phase, u, toks[phase], T, 0, B, 2, off);
-        run_steps(c, m, phase, u, toks[phase], T, 0, B, len, heads(phase));
+        if (phase == 2 && Lc) locations(u.all);
+        const HeadArgs off, h = heads(phase);
+        run_steps(c, m, phase, u, &toks[phase], &T, img0, nimg, 2, &off);
+        run_steps(c, m, phase, u, &toks[phase], &T, img0, nimg, len, &h);
         if (beams)
           beam_backtrace(c, toks[phase], T, prbs[phase], len, d_bscore, d_blen, d_anc, T - 1, Si, Wb, len, 3, c->beam_alpha,
                          d_bids, d_bprobs, d_bscores);
@@ -1401,65 +1287,86 @@ void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P,
     ALM_CHECK_CUDA(cudaEventRecord(c->ev_join, s1));
     ALM_CHECK_CUDA(cudaStreamWaitEvent(s0, c->ev_join, 0));
   }
-  ALM_CHECK_CUDA(cudaEventRecord(c->ev_t[4], s0));
-  c->timing_valid[1] = true;
-  wait_stream(c, c->stream);
-  for (int phase = 1; phase <= 2; ++phase) {
-    const int len = phase == 1 ? cfg.poly_length : cfg.rec_length;
-    const int T = 3 + len;
-    const bool beams = phase == 2 && Wb > 0;
-    std::vector<int> hh(beams ? 0 : static_cast<size_t>(Si) * T);
-    std::vector<float> hp(beams ? 0 : static_cast<size_t>(Si) * len);
-    if (!beams) {
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hh.data(), toks[phase], hh.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hp.data(), prbs[phase], hp.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  if (done) ALM_CHECK_CUDA(cudaEventRecord(done, s0));
+  wait_stream(c, s0);
+  PolyRec r;
+  auto fetch = [&](auto& host, const auto* dev, size_t n) {
+    host.resize(n);
+    ALM_CHECK_CUDA(cudaMemcpyAsync(host.data(), dev, n * sizeof(*dev), cudaMemcpyDeviceToHost, s0));
+  };
+  for (int phase = 1; phase <= 2; ++phase)
+    if (phase == 1 || Wb == 0) {  // beams: only the n-best lists leave the device
+      fetch(r.tok[phase], toks[phase], static_cast<size_t>(Si) * (3 + lens[phase]));
+      fetch(r.prob[phase], prbs[phase], static_cast<size_t>(Si) * lens[phase]);
     }
-    std::vector<int> hci(phase == 2 ? cand_n : 0);
-    std::vector<float> hcp(hci.size());
-    if (!hci.empty()) {
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hci.data(), d_cand_ids, cand_n * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hcp.data(), d_cand_probs, cand_n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    }
-    std::vector<float> hloc(phase == 2 ? loc_n : 0);
-    if (!hloc.empty())
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hloc.data(), d_loc, loc_n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    // beams: only the n-best lists leave the device; hypothesis 0 is rec / rec_prob
-    std::vector<int> hbi(beams ? bl_n : 0);
-    std::vector<float> hbp(hbi.size()), hbs(beams ? nb : 0);
-    if (beams) {
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hbi.data(), d_bids, bl_n * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hbp.data(), d_bprobs, bl_n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-      ALM_CHECK_CUDA(cudaMemcpyAsync(hbs.data(), d_bscores, nb * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    }
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+  if (K > 0) {
+    fetch(r.cand_ids, d_cand_ids, cand_n);
+    fetch(r.cand_probs, d_cand_probs, cand_n);
+  }
+  if (Wb > 0) {
+    fetch(r.beam_ids, d_bids, bl_n);
+    fetch(r.beam_probs, d_bprobs, bl_n);
+    fetch(r.beam_scores, d_bscores, nb);
+  }
+  if (Lc) fetch(r.loc, d_loc, loc_n);
+  ALM_CHECK_CUDA(cudaStreamSynchronize(s0));
+  return r;
+}
+
+// The polygon and recognition stage of alm_omni_decode, _prompts, _kie and _at at given points.  uniq[b] lists the
+// (x, y) bins of image b, one row per entry (Ncap = the longest list); instance n of slot q (image q / P) takes the
+// result of entry slot_inst[q][n] of its image.  Writes poly / rec / rec_prob in alm_omni_decode's layout with maxI
+// rows per slot, and keeps the candidate / beam / location lists of the context's settings in the model.
+void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P, int maxI, const std::vector<Points>& uniq,
+                    const std::vector<std::vector<int>>& slot_inst, int64_t* poly, int64_t* rec, float* rec_prob) {
+  OmniModel* m = c->omni;
+  const int S = static_cast<int>(slot_inst.size()), K = c->rec_topk, Wb = c->rec_beams;
+  const size_t L = cfg.rec_length, rows = static_cast<size_t>(S) * maxI;
+  int Ncap = 0;
+  for (const auto& u : uniq) Ncap = std::max(Ncap, static_cast<int>(u.size()));
+  OmniModel::RecLists lists;  // [slot][max_inst][...]; instances past n_inst stay 0
+  if (K > 0) {
+    lists.cand_ids.assign(rows * L * K, 0);
+    lists.cand_probs.assign(rows * L * K, 0.f);
+  }
+  if (Wb > 0) {
+    lists.beam_ids.assign(rows * Wb * L, 0);
+    lists.beam_probs.assign(rows * Wb * L, 0.f);
+    lists.beam_scores.assign(rows * Wb, 0.f);
+  }
+  if (c->rec_locations) lists.rec_loc.assign(rows * L * 5, 0.f);
+  if (Ncap > 0) {
+    const PolyRec r = poly_rec(c, cfg, hc, 0, uniq, Ncap, c->ev_t[4]);
+    c->timing_valid[1] = true;
+    const size_t T1 = 3 + cfg.poly_length, T2 = 3 + L;
     for (int q = 0; q < S; ++q)
       for (int n = 0; n < static_cast<int>(slot_inst[q].size()); ++n) {
-        const size_t sq = static_cast<size_t>(q / P) * Ncap + slot_inst[q][n];
-        for (int k = 0; k < len; ++k) {
-          const size_t o = (static_cast<size_t>(q) * maxI + n) * len + k;
-          if (phase == 1) poly[o] = hh[sq * T + 3 + k];
-          else if (beams) { rec[o] = hbi[sq * Wb * len + k]; rec_prob[o] = hbp[sq * Wb * len + k]; }
-          else { rec[o] = hh[sq * T + 3 + k]; rec_prob[o] = hp[sq * len + k]; }
+        // a deduplicated (x, y) carries its results to every slot holding it: entries [from, from + len) of row sq of
+        // `src` to row o = (q, n) of `dst`
+        const size_t sq = static_cast<size_t>(q / P) * Ncap + slot_inst[q][n], o = static_cast<size_t>(q) * maxI + n;
+        auto carry = [&](const auto& src, size_t from, size_t len, auto* dst) {
+          std::copy(src.begin() + from, src.begin() + from + len, dst + o * len);
+        };
+        carry(r.tok[1], sq * T1 + 3, cfg.poly_length, poly);
+        if (Wb > 0) {  // hypothesis 0 is rec / rec_prob
+          carry(r.beam_ids, sq * Wb * L, L, rec);
+          carry(r.beam_probs, sq * Wb * L, L, rec_prob);
+          carry(r.beam_ids, sq * Wb * L, Wb * L, lists.beam_ids.data());
+          carry(r.beam_probs, sq * Wb * L, Wb * L, lists.beam_probs.data());
+          carry(r.beam_scores, sq * Wb, Wb, lists.beam_scores.data());
+        } else {
+          carry(r.tok[2], sq * T2 + 3, L, rec);
+          carry(r.prob[2], sq * L, L, rec_prob);
         }
-        if (beams) {  // like rec: a deduplicated (x, y) carries its n-best list to every slot holding it
-          const size_t src = sq * Wb, dst = (static_cast<size_t>(q) * maxI + n) * Wb;
-          std::copy(hbi.begin() + src * len, hbi.begin() + (src + Wb) * len, beam_ids.begin() + dst * len);
-          std::copy(hbp.begin() + src * len, hbp.begin() + (src + Wb) * len, beam_probs.begin() + dst * len);
-          std::copy(hbs.begin() + src, hbs.begin() + src + Wb, beam_scores.begin() + dst);
+        if (K > 0) {
+          carry(r.cand_ids, sq * L * K, L * K, lists.cand_ids.data());
+          carry(r.cand_probs, sq * L * K, L * K, lists.cand_probs.data());
         }
-        if (!hci.empty()) {  // like rec: a deduplicated (x, y) carries its candidates to every slot holding it
-          const size_t src = sq * len * K, dst = (static_cast<size_t>(q) * maxI + n) * len * K;
-          std::copy(hci.begin() + src, hci.begin() + src + static_cast<size_t>(len) * K, cand_ids.begin() + dst);
-          std::copy(hcp.begin() + src, hcp.begin() + src + static_cast<size_t>(len) * K, cand_probs.begin() + dst);
-        }
-        if (!hloc.empty()) {  // like rec: a deduplicated (x, y) carries its locations to every slot holding it
-          const size_t src = sq * len * 5, dst = (static_cast<size_t>(q) * maxI + n) * len * 5;
-          std::copy(hloc.begin() + src, hloc.begin() + src + static_cast<size_t>(len) * 5, rec_loc.begin() + dst);
-        }
+        if (!r.loc.empty()) carry(r.loc, sq * L * 5, L * 5, lists.rec_loc.data());
       }
+    c->ws.release(m->ws_mark);
   }
-  keep_lists();
-  ws.release(m->ws_mark);
+  m->rec_lists = std::move(lists);
 }
 
 }  // namespace
@@ -1505,14 +1412,7 @@ void omni_decode_impl(Ctx* c, const int64_t* prompts, long page_stride, int P, i
   // character locations of the greedy rec loop (alm_omni_set_rec_locations); they describe this decode or none
   const bool Lc = !points_only && c->rec_locations;
   ALM_REQUIRE(!Lc || Wb == 0, ALM_ERR_INVALID, "character locations and beams cannot be combined");
-  if (!points_only) {
-    m->cand_ids.clear();
-    m->cand_probs.clear();
-    m->beam_ids.clear();
-    m->beam_probs.clear();
-    m->beam_scores.clear();
-    m->rec_loc.clear();
-  }
+  if (!points_only) m->rec_lists = {};
   c->timing_valid[1] = false;
   DecodeScope scope(c);
   ALM_CHECK_CUDA(cudaEventRecord(c->ev_t[2], c->stream));
@@ -1644,34 +1544,34 @@ size_t omni_dense_loops(Ctx* c, int32_t* out, size_t elems) {
 
 size_t omni_rec_beams(Ctx* c, int64_t* ids, float* probs, float* scores, size_t elems) {
   OmniModel* m = c->omni;
-  ALM_REQUIRE(m && !m->beam_ids.empty(), ALM_ERR_STATE,
+  ALM_REQUIRE(m && !m->rec_lists.beam_ids.empty(), ALM_ERR_STATE,
               "no n-best lists: the last decode ran with alm_omni_set_rec_beams W = 0");
-  const size_t n = m->beam_ids.size();
+  const size_t n = m->rec_lists.beam_ids.size();
   ALM_REQUIRE(elems >= n, ALM_ERR_INVALID, "n-best buffers too small: need " + std::to_string(n) + " elements");
-  std::copy(m->beam_ids.begin(), m->beam_ids.end(), ids);
-  std::copy(m->beam_probs.begin(), m->beam_probs.end(), probs);
-  std::copy(m->beam_scores.begin(), m->beam_scores.end(), scores);
+  std::copy(m->rec_lists.beam_ids.begin(), m->rec_lists.beam_ids.end(), ids);
+  std::copy(m->rec_lists.beam_probs.begin(), m->rec_lists.beam_probs.end(), probs);
+  std::copy(m->rec_lists.beam_scores.begin(), m->rec_lists.beam_scores.end(), scores);
   return n;
 }
 
 size_t omni_rec_locations(Ctx* c, float* out, size_t elems) {
   OmniModel* m = c->omni;
-  ALM_REQUIRE(m && !m->rec_loc.empty(), ALM_ERR_STATE,
+  ALM_REQUIRE(m && !m->rec_lists.rec_loc.empty(), ALM_ERR_STATE,
               "no character locations: the last decode ran with alm_omni_set_rec_locations off");
-  const size_t n = m->rec_loc.size();
+  const size_t n = m->rec_lists.rec_loc.size();
   ALM_REQUIRE(elems >= n, ALM_ERR_INVALID, "location buffer too small: need " + std::to_string(n) + " elements");
-  std::copy(m->rec_loc.begin(), m->rec_loc.end(), out);
+  std::copy(m->rec_lists.rec_loc.begin(), m->rec_lists.rec_loc.end(), out);
   return n;
 }
 
 size_t omni_rec_candidates(Ctx* c, int64_t* ids, float* probs, size_t elems) {
   OmniModel* m = c->omni;
-  ALM_REQUIRE(m && !m->cand_ids.empty(), ALM_ERR_STATE,
+  ALM_REQUIRE(m && !m->rec_lists.cand_ids.empty(), ALM_ERR_STATE,
               "no recognition candidates: the last decode ran with alm_omni_set_rec_candidates k = 0");
-  const size_t n = m->cand_ids.size();
+  const size_t n = m->rec_lists.cand_ids.size();
   ALM_REQUIRE(elems >= n, ALM_ERR_INVALID, "candidate buffers too small: need " + std::to_string(n) + " elements");
-  std::copy(m->cand_ids.begin(), m->cand_ids.end(), ids);
-  std::copy(m->cand_probs.begin(), m->cand_probs.end(), probs);
+  std::copy(m->rec_lists.cand_ids.begin(), m->rec_lists.cand_ids.end(), ids);
+  std::copy(m->rec_lists.cand_probs.begin(), m->rec_lists.cand_probs.end(), probs);
   return n;
 }
 
@@ -1745,12 +1645,7 @@ void omni_decode_at(Ctx* c, const int32_t* xy, const int32_t* count, int cap, co
   std::fill(poly, poly + rows * 32, 0);
   std::fill(rec, rec + rows * cfg.rec_length, 0);
   std::fill(rec_prob, rec_prob + rows * cfg.rec_length, 0.f);
-  m->cand_ids.clear();
-  m->cand_probs.clear();
-  m->beam_ids.clear();
-  m->beam_probs.clear();
-  m->beam_scores.clear();
-  m->rec_loc.clear();
+  m->rec_lists = {};
   c->ws.release(m->ws_mark);
   c->timing_valid[1] = false;
   DecodeScope scope(c);
@@ -1778,14 +1673,14 @@ void omni_decode_logits(Ctx* c, int image, int kind, const int64_t* seq, int n_s
   }
   int* tok = ws.get<int>(h.size());
   ALM_CHECK_CUDA(cudaMemcpyAsync(tok, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  DecodeBufs u = alloc_decode(c, m, 1, n_seq, len, false, image);
-  fill_i32(c, u.tpos, 1, 0);
+  StepBufs u = alloc_decode(c, m, 1, 1, n_seq, len, false, image);
+  fill_i32(c, u.all.tpos, 1, 0);
   for (int t = 0; t < len; ++t) {
-    decoder_step(c, m, kind, u, tok, len, image, 1, true);
-    add_i32(c, u.tpos, 1);
+    decoder_step(c, m, kind, u, &tok, &len, image, 1, true);
+    add_i32(c, u.all.tpos, 1);
     // logits [n_seq, len, V] <- step t rows
     ALM_CHECK_CUDA(cudaMemcpy2DAsync(logits + static_cast<size_t>(t) * m->V, static_cast<size_t>(len) * m->V * sizeof(float),
-                                     u.logits, static_cast<size_t>(m->V) * sizeof(float), static_cast<size_t>(m->V) * sizeof(float),
+                                     u.all.logits, static_cast<size_t>(m->V) * sizeof(float), static_cast<size_t>(m->V) * sizeof(float),
                                      n_seq, cudaMemcpyDeviceToHost, c->stream));
   }
   ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
@@ -1796,8 +1691,6 @@ void omni_decode_logits(Ctx* c, int image, int kind, const int64_t* seq, int n_s
 // Pages with more words than one point sequence holds, read in the training grids' spatial windows (DESIGN 4.16;
 // rule: dense_core.h).
 namespace {
-
-using Points = std::vector<std::pair<int, int>>;
 
 // maximal runs [first, first + count) of consecutive pages with want[b]
 std::vector<std::pair<int, int>> page_runs(const std::vector<uint8_t>& want) {
@@ -1862,19 +1755,13 @@ void read_windows(Ctx* c, OmniModel* m, const HeadCfg& hc, const int64_t* prompt
 void poly_rec_passes(Ctx* c, OmniModel* m, const alm_decode_cfg& cfg, const HeadCfg& hc, const std::vector<Points>& uniq,
                      long budget, std::vector<std::vector<int>>* poly, std::vector<std::vector<int>>* rec,
                      std::vector<std::vector<float>>* prob) {
-  const int B = m->B, lens[3] = {0, cfg.poly_length, cfg.rec_length};
+  const int B = m->B, L1 = cfg.poly_length, L2 = cfg.rec_length;
   Arena& ws = c->ws;
   for (int b = 0; b < B; ++b) {
-    (*poly)[b].assign(uniq[b].size() * cfg.poly_length, 0);
-    (*rec)[b].assign(uniq[b].size() * cfg.rec_length, 0);
-    (*prob)[b].assign(uniq[b].size() * cfg.rec_length, 0.f);
+    (*poly)[b].assign(uniq[b].size() * L1, 0);
+    (*rec)[b].assign(uniq[b].size() * L2, 0);
+    (*prob)[b].assign(uniq[b].size() * L2, 0.f);
   }
-  if (!c->stream2) ALM_CHECK_CUDA(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
-  if (!c->ev_fork) {
-    ALM_CHECK_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-    ALM_CHECK_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
-  }
-  cudaStream_t s0 = c->stream, s1 = c->decode_streams == 2 ? c->stream2 : c->stream;
   std::vector<int> next(B, 0);
   for (;;) {
     std::vector<uint8_t> left(B);
@@ -1886,87 +1773,21 @@ void poly_rec_passes(Ctx* c, OmniModel* m, const alm_decode_cfg& cfg, const Head
       long most = 0;
       for (int b = i0; b < i0 + n; ++b) most = std::max<long>(most, static_cast<long>(uniq[b].size()) - next[b]);
       const int Ncap = static_cast<int>(std::min<long>(most, std::max<long>(1, budget / n)));
-      const int Si = n * Ncap;
       m->dense_loops.insert(m->dense_loops.end(), {1, i0, n, Ncap});
-      const size_t mark = ws.mark();
-      int* toks[3] = {nullptr, nullptr, nullptr};
-      float* prbs[3] = {nullptr, nullptr, nullptr};
-      std::vector<int> h_prompt[3];
-      for (int phase = 1; phase <= 2; ++phase) {  // [x, y, sos] per row; dead rows 0, 0, sos
-        const int T = 3 + lens[phase];
-        h_prompt[phase].assign(static_cast<size_t>(Si) * T, 0);
-        for (int b = i0; b < i0 + n; ++b)
-          for (int j = 0; j < Ncap; ++j) {
-            int* row = &h_prompt[phase][(static_cast<size_t>(b - i0) * Ncap + j) * T];
-            if (next[b] + j < static_cast<int>(uniq[b].size())) {
-              row[0] = uniq[b][next[b] + j].first;
-              row[1] = uniq[b][next[b] + j].second;
-            }
-            row[2] = phase == 1 ? cfg.poly_sos : cfg.rec_sos;
-          }
-        toks[phase] = ws.get<int>(h_prompt[phase].size());
-        prbs[phase] = ws.get<float>(static_cast<size_t>(Si) * lens[phase]);
-        ALM_CHECK_CUDA(cudaMemcpyAsync(toks[phase], h_prompt[phase].data(), h_prompt[phase].size() * sizeof(int),
-                                       cudaMemcpyHostToDevice, s0));
-      }
-      auto heads = [&](int phase) {
-        HeadArgs h;
-        h.on = true; h.cfg = hc; h.tokens = toks[phase]; h.tstride = 3 + lens[phase]; h.n_prompt_m1 = 2;
-        h.probs = prbs[phase]; h.pstride = lens[phase]; h.seqs_per_image = Ncap; h.nsoft = m->V - m->vie;
-        return h;
-      };
-      if (joint_pass_ok(c, n, Ncap, false)) {  // as omni_decode_impl: one joint pass, then the longer loop alone
-        JointBufs jb = alloc_joint(c, m, n, Ncap, 2 + std::max(lens[1], lens[2]), i0);
-        fill_i32(c, jb.j.tpos, 1, 0);
-        const int* jt[2] = {toks[1], toks[2]};
-        const int js[2] = {3 + lens[1], 3 + lens[2]};
-        const HeadArgs off[2], hs[2] = {heads(1), heads(2)};
-        run_joint(c, m, jb, jt, js, i0, n, 2, off);
-        const int both = std::min(lens[1], lens[2]);
-        run_joint(c, m, jb, jt, js, i0, n, both, hs);
-        for (int phase = 1; phase <= 2; ++phase)
-          run_steps(c, m, phase, jb.h[phase - 1], toks[phase], js[phase - 1], i0, n, lens[phase] - both, hs[phase - 1]);
-      } else {
-        ALM_CHECK_CUDA(cudaEventRecord(c->ev_fork, s0));
-        ALM_CHECK_CUDA(cudaStreamWaitEvent(s1, c->ev_fork, 0));
-        try {
-          for (int phase = 1; phase <= 2; ++phase) {
-            c->stream = phase == 1 ? s0 : s1;
-            const int len = lens[phase], T = 3 + len;
-            DecodeBufs u = alloc_decode(c, m, n, Ncap, T - 1, false, i0);
-            fill_i32(c, u.tpos, 1, 0);
-            HeadArgs off;
-            run_steps(c, m, phase, u, toks[phase], T, i0, n, 2, off);
-            run_steps(c, m, phase, u, toks[phase], T, i0, n, len, heads(phase));
-          }
-        } catch (...) {
-          c->stream = s0;
-          cudaStreamSynchronize(s1);
-          throw;
-        }
-        c->stream = s0;
-        ALM_CHECK_CUDA(cudaEventRecord(c->ev_join, s1));
-        ALM_CHECK_CUDA(cudaStreamWaitEvent(s0, c->ev_join, 0));
-      }
-      wait_stream(c, s0);
-      for (int phase = 1; phase <= 2; ++phase) {
-        const int len = lens[phase], T = 3 + len;
-        std::vector<int> hh(static_cast<size_t>(Si) * T);
-        std::vector<float> hp(static_cast<size_t>(Si) * len);
-        ALM_CHECK_CUDA(cudaMemcpyAsync(hh.data(), toks[phase], hh.size() * sizeof(int), cudaMemcpyDeviceToHost, s0));
-        ALM_CHECK_CUDA(cudaMemcpyAsync(hp.data(), prbs[phase], hp.size() * sizeof(float), cudaMemcpyDeviceToHost, s0));
-        ALM_CHECK_CUDA(cudaStreamSynchronize(s0));
-        for (int b = i0; b < i0 + n; ++b)
-          for (int j = 0; j < Ncap && next[b] + j < static_cast<int>(uniq[b].size()); ++j) {
-            const size_t r = static_cast<size_t>(b - i0) * Ncap + j, e = static_cast<size_t>(next[b]) + j;
-            for (int k = 0; k < len; ++k) {
-              if (phase == 1) (*poly)[b][e * len + k] = hh[r * T + 3 + k];
-              else { (*rec)[b][e * len + k] = hh[r * T + 3 + k]; (*prob)[b][e * len + k] = hp[r * len + k]; }
-            }
-          }
-      }
+      std::vector<Points> pts(n);  // the pass's rows of each page: its next Ncap points
       for (int b = i0; b < i0 + n; ++b)
-        next[b] = std::min(static_cast<int>(uniq[b].size()), next[b] + Ncap);
+        pts[b - i0].assign(uniq[b].begin() + next[b], uniq[b].begin() + std::min<size_t>(uniq[b].size(), next[b] + Ncap));
+      const size_t mark = ws.mark();
+      const PolyRec r = poly_rec(c, cfg, hc, i0, pts, Ncap, nullptr);
+      for (int b = i0; b < i0 + n; ++b) {
+        for (size_t j = 0; j < pts[b - i0].size(); ++j) {
+          const size_t row = static_cast<size_t>(b - i0) * Ncap + j, e = next[b] + j;
+          std::copy_n(r.tok[1].begin() + row * (3 + L1) + 3, L1, (*poly)[b].begin() + e * L1);
+          std::copy_n(r.tok[2].begin() + row * (3 + L2) + 3, L2, (*rec)[b].begin() + e * L2);
+          std::copy_n(r.prob[2].begin() + row * L2, L2, (*prob)[b].begin() + e * L2);
+        }
+        next[b] += static_cast<int>(pts[b - i0].size());
+      }
       ws.release(mark);
     }
   }
@@ -2007,9 +1828,7 @@ void omni_decode_dense(Ctx* c, const int64_t* prompt, int n_prompt, const alm_de
   // the preamble of every decode entry: a fresh workspace after the encoded state, and no candidate / n-best / location
   // lists (they describe the last decode or none; dense decoding makes none)
   c->ws.release(m->ws_mark);
-  m->cand_ids.clear(); m->cand_probs.clear();
-  m->beam_ids.clear(); m->beam_probs.clear(); m->beam_scores.clear();
-  m->rec_loc.clear();
+  m->rec_lists = {};
   m->dense_loops.clear();
   const int B = m->B, L = cfg.rec_length;
   const size_t W = kMaxWindows;

@@ -79,17 +79,18 @@ struct OmniModel {
   bf16 *vc_hi = nullptr, *vc_lo = nullptr;                // [B, 12 (dec,layer), 8 heads, M, 64]
   bf16 *vt_hi = nullptr, *vt_lo = nullptr;                // [B, 6144, Mpad] (only for the unfused debug path, xattn_impl 1)
   size_t ws_mark = 0;                                     // arena offset after the encode-persistent buffers
-  // recognition candidates of the last decode that ran the rec loop with Ctx::rec_topk > 0 (empty otherwise):
-  // [slot][max_inst][rec_length][k]
-  std::vector<int64_t> cand_ids;
-  std::vector<float> cand_probs;
-  // n-best lists of the last decode that ran the rec loop with Ctx::rec_beams > 0 (empty otherwise):
-  // ids / probs [slot][max_inst][W][rec_length], scores [slot][max_inst][W]
-  std::vector<int64_t> beam_ids;
-  std::vector<float> beam_probs, beam_scores;
-  // character locations of the last decode that ran the rec loop with Ctx::rec_locations (empty otherwise):
-  // [slot][max_inst][rec_length][5] = cx, cy, sxx, sxy, syy in encoder-input pixels
-  std::vector<float> rec_loc;
+  // side lists of the last decode that ran the rec loop, each empty unless its option was on
+  struct RecLists {
+    // candidates (Ctx::rec_topk > 0): [slot][max_inst][rec_length][k]
+    std::vector<int64_t> cand_ids;
+    std::vector<float> cand_probs;
+    // n-best lists (Ctx::rec_beams > 0): ids / probs [slot][max_inst][W][rec_length], scores [slot][max_inst][W]
+    std::vector<int64_t> beam_ids;
+    std::vector<float> beam_probs, beam_scores;
+    // character locations (Ctx::rec_locations): [slot][max_inst][rec_length][5] = cx, cy, sxx, sxy, syy in
+    // encoder-input pixels
+    std::vector<float> rec_loc;
+  } rec_lists;
   // the loops of the last alm_omni_decode_dense beyond level 0, [n][4] = (kind, img0, nimg, per page): kind 0 a window
   // point loop with `per page` = P window prompts, kind 1 a polygon / recognition pass of `per page` = Ncap rows
   std::vector<int> dense_loops;

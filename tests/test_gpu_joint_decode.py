@@ -387,7 +387,7 @@ def test_recognition_loop_as_long_as_or_longer_than_the_polygon_loop(rec_length,
 
 def _regimes():
     """batches of the 'full' page (4 instances each) whose S = 4 B rows per decoder put the self-attention step in each
-    regime of joint_step: both halves and the joint rows on the wide kernel (S <= SMs / 4), one launch per half
+    regime of the joint pass's decoder step: both halves and the joint rows on the wide kernel (S <= SMs / 4), one launch per half
     (SMs / 4 < S <= SMs / 2), none on the wide kernel (S > SMs / 2)"""
     sms = _sms()
     return {'one_wide_launch': (sms // 4) // 4, 'per_half_launches': (sms // 2) // 4, 'one_launch': (sms // 2) // 4 + 1}
