@@ -857,6 +857,46 @@ int alm_pre_omni_tiles_turned(alm_ctx* h, const uint8_t* const* rgb, const int* 
 
 namespace {
 
+// The tiles of a tile merge's plan (alm_omni_merge_tiles, _turned, alm_omni_merge_kie_tiles), once the page sizes, the
+// layout, margin / band / iou, the turns (null: upright pages), n_tiles and every tile's page and origin are checked
+std::vector<tile_core::Tile> merge_plan(const char* fn, const int* heights, const int* widths, int n_pages,
+                                        const int32_t* turns, int tile, int overlap, double margin, double band,
+                                        double iou, int n_tiles, const int* tile_page, const int* tile_origin) {
+  ALM_REQUIRE(pages_ok(heights, widths, n_pages) && tile_core::valid_layout(tile, overlap), ALM_ERR_INVALID,
+              std::string(fn) + ": page sizes, or tile size / overlap (need tile >= 64, 0 <= 2 overlap <= tile)");
+  ALM_REQUIRE(std::isfinite(margin) && margin >= 0.0 && std::isfinite(band) && band >= 0.0 && std::isfinite(iou) &&
+                  iou > 0.0 && iou <= 1.0,
+              ALM_ERR_INVALID, std::string(fn) + ": margin and band must be finite and >= 0, iou in (0, 1]");
+  ALM_REQUIRE(tile_page && tile_origin, ALM_ERR_INVALID, std::string(fn) + ": null argument");
+  if (turns) require_turns(turns, n_pages, fn);
+  std::vector<tile_core::Tile> tiles = page_tiles(heights, widths, n_pages, tile, overlap, band, turns);
+  ALM_REQUIRE(n_tiles == static_cast<int>(tiles.size()), ALM_ERR_INVALID,
+              std::string(fn) + ": " + std::to_string(n_tiles) + " tiles, the plan has " + std::to_string(tiles.size()));
+  for (int k = 0; k < n_tiles; ++k) {
+    const tile_core::Tile& t = tiles[static_cast<size_t>(k)];
+    ALM_REQUIRE(tile_page[k] >= 0 && tile_page[k] < n_pages, ALM_ERR_INVALID,
+                std::string(fn) + ": tile " + std::to_string(k) + ": page index out of range");
+    ALM_REQUIRE(tile_page[k] == t.page && tile_origin[2 * k] == t.y0 && tile_origin[2 * k + 1] == t.x0,
+                ALM_ERR_INVALID, std::string(fn) + ": tile " + std::to_string(k) + " is not the plan's tile " +
+                                     std::to_string(k) + " (pages in order, tiles row-major)");
+  }
+  return tiles;
+}
+
+// The total of n counts, once every count is checked >= 0 and every offset the sum of the earlier counts; the
+// refusals name each count `what` and its index
+long prefix_total(const char* fn, const char* what, const int32_t* count, const int32_t* offset, long n) {
+  long total = 0;
+  for (long r = 0; r < n; ++r) {
+    ALM_REQUIRE(count[r] >= 0, ALM_ERR_INVALID,
+                std::string(fn) + ": " + what + " " + std::to_string(r) + ": negative count");
+    ALM_REQUIRE(offset[r] == total, ALM_ERR_INVALID,
+                std::string(fn) + ": " + what + " " + std::to_string(r) + ": offset is not the sum of the earlier counts");
+    total += count[r];
+  }
+  return total;
+}
+
 // alm_omni_merge_tiles (turned false) / alm_omni_merge_tiles_turned
 int merge_tiles(alm_ctx* h, const char* fn, const int* heights, const int* widths, int n_pages, bool turned,
                 const int32_t* turns, int tile, int overlap, int n_tiles, const int* tile_page, const int* tile_origin,
@@ -865,29 +905,14 @@ int merge_tiles(alm_ctx* h, const char* fn, const int* heights, const int* width
                 double iou, int* page_count, int* page_offset, double* pts, double* polys, int64_t* rec_out,
                 float* prob_out, int32_t* source, long cap) {
   return guarded(h, [&] {
-    ALM_REQUIRE(pages_ok(heights, widths, n_pages) && tile_core::valid_layout(tile, overlap), ALM_ERR_INVALID,
-                std::string(fn) + ": page sizes, or tile size / overlap (need tile >= 64, 0 <= 2 overlap <= tile)");
-    ALM_REQUIRE(std::isfinite(margin) && margin >= 0.0 && std::isfinite(band) && band >= 0.0 && std::isfinite(iou) &&
-                    iou > 0.0 && iou <= 1.0,
-                ALM_ERR_INVALID, std::string(fn) + ": margin and band must be finite and >= 0, iou in (0, 1]");
     ALM_REQUIRE(max_inst >= 1 && rec_length >= 1 && num_bins >= 1, ALM_ERR_INVALID,
                 std::string(fn) + ": max_inst, rec_length and num_bins must be >= 1");
-    ALM_REQUIRE(tile_page && tile_origin && n_inst && pt && poly && rec && rec_prob && page_count && page_offset &&
-                    (turns || !turned),
+    ALM_REQUIRE(n_inst && pt && poly && rec && rec_prob && page_count && page_offset && (turns || !turned),
                 ALM_ERR_INVALID, std::string(fn) + ": null argument");
-    if (turns) require_turns(turns, n_pages, fn);
-    const std::vector<tile_core::Tile> tiles = page_tiles(heights, widths, n_pages, tile, overlap, band, turns);
-    ALM_REQUIRE(n_tiles == static_cast<int>(tiles.size()), ALM_ERR_INVALID,
-                std::string(fn) + ": " + std::to_string(n_tiles) + " tiles, the plan has " +
-                    std::to_string(tiles.size()));
+    const std::vector<tile_core::Tile> tiles = merge_plan(fn, heights, widths, n_pages, turns, tile, overlap, margin,
+                                                          band, iou, n_tiles, tile_page, tile_origin);
     long total = 0;
     for (int k = 0; k < n_tiles; ++k) {
-      const tile_core::Tile& t = tiles[static_cast<size_t>(k)];
-      ALM_REQUIRE(tile_page[k] >= 0 && tile_page[k] < n_pages, ALM_ERR_INVALID,
-                  std::string(fn) + ": tile " + std::to_string(k) + ": page index out of range");
-      ALM_REQUIRE(tile_page[k] == t.page && tile_origin[2 * k] == t.y0 && tile_origin[2 * k + 1] == t.x0,
-                  ALM_ERR_INVALID, std::string(fn) + ": tile " + std::to_string(k) + " is not the plan's tile " +
-                                       std::to_string(k) + " (pages in order, tiles row-major)");
       ALM_REQUIRE(n_inst[k] >= 0 && n_inst[k] <= max_inst, ALM_ERR_INVALID,
                   std::string(fn) + ": tile " + std::to_string(k) + ": n_inst outside [0, max_inst]");
       total += n_inst[k];
@@ -896,7 +921,7 @@ int merge_tiles(alm_ctx* h, const char* fn, const int* heights, const int* width
     ALM_REQUIRE(total == 0 || (pts && polys && rec_out && prob_out && source), ALM_ERR_INVALID,
                 std::string(fn) + ": null output buffer");
     tile_merge(&h->c, tiles, n_pages, max_inst, rec_length, num_bins, margin, iou, n_inst, pt, poly, rec, rec_prob,
-               page_count, page_offset, pts, polys, rec_out, prob_out, source);
+               MergeRows{page_count, page_offset, pts, polys, rec_out, prob_out, source});
   });
 }
 
@@ -957,17 +982,11 @@ int merge_readings(alm_ctx* h, const char* fn, int n_pages, int nr, const int32_
     ALM_REQUIRE(std::isfinite(iou) && iou > 0.0 && iou <= 1.0, ALM_ERR_INVALID,
                 std::string(fn) + ": iou must be in (0, 1]");
     ALM_REQUIRE(static_cast<long>(nr) * n_pages <= INT_MAX / 2, ALM_ERR_INVALID, std::string(fn) + ": too many readings");
-    long total = 0;
-    for (long r = 0; r < static_cast<long>(nr) * n_pages; ++r) {
-      ALM_REQUIRE(count[r] >= 0, ALM_ERR_INVALID, std::string(fn) + ": reading " + std::to_string(r) + ": negative count");
-      ALM_REQUIRE(offset[r] == total, ALM_ERR_INVALID,
-                  std::string(fn) + ": reading " + std::to_string(r) + ": offset is not the sum of the earlier counts");
-      total += count[r];
-      ALM_REQUIRE(total <= INT_MAX / 32, ALM_ERR_INVALID, std::string(fn) + ": too many rows");
-    }
+    const long total = prefix_total(fn, "reading", count, offset, static_cast<long>(nr) * n_pages);
+    ALM_REQUIRE(total <= INT_MAX / 32, ALM_ERR_INVALID, std::string(fn) + ": too many rows");
     ALM_REQUIRE(cap >= total, ALM_ERR_INVALID, std::string(fn) + ": output capacity below the sum of the counts");
     reading_merge(&h->c, n_pages, nr, count, offset, rec_length, recog_pad_index, rec_eos_index, iou, pts, polys, rec,
-                  rec_prob, page_count, page_offset, pts_out, polys_out, rec_out, prob_out, source);
+                  rec_prob, MergeRows{page_count, page_offset, pts_out, polys_out, rec_out, prob_out, source});
   });
 }
 
@@ -1012,15 +1031,12 @@ int alm_omni_merge_whole_page(alm_ctx* h, const int* heights, const int* widths,
                     whole_prob && page_count && page_offset && pts_out && polys_out && rec_out && prob_out && source,
                 ALM_ERR_INVALID, std::string(fn) + ": null argument");
     if (turns) require_turns(turns, n_pages, fn);
-    long total = 0, whole = 0;
+    const long total = prefix_total(fn, "page", count, offset, n_pages);
+    long whole = 0;
     std::vector<whole_core::Page> pages(static_cast<size_t>(n_pages));
     for (int p = 0; p < n_pages; ++p) {
-      ALM_REQUIRE(count[p] >= 0, ALM_ERR_INVALID, std::string(fn) + ": page " + std::to_string(p) + ": negative count");
-      ALM_REQUIRE(offset[p] == total, ALM_ERR_INVALID,
-                  std::string(fn) + ": page " + std::to_string(p) + ": offset is not the sum of the earlier counts");
       ALM_REQUIRE(n_inst[p] >= 0 && n_inst[p] <= cap_in, ALM_ERR_INVALID,
                   std::string(fn) + ": page " + std::to_string(p) + ": n_inst outside [0, cap_in]");
-      total += count[p];
       whole += n_inst[p];
       pages[static_cast<size_t>(p)] = whole_core::Page{heights[p], widths[p], turns ? turns[p] : 0};
     }
@@ -1029,8 +1045,8 @@ int alm_omni_merge_whole_page(alm_ctx* h, const int* heights, const int* widths,
     ALM_REQUIRE(cap >= total + whole, ALM_ERR_INVALID,
                 std::string(fn) + ": output capacity below the tile rows plus the whole-page instances");
     whole_merge(&h->c, pages, tile, overlap, num_bins, margin, rec_length, count, offset, pts, polys, rec, rec_prob,
-                source_in, cap_in, n_inst, pt, poly, whole_rec, whole_prob, page_count, page_offset, pts_out,
-                polys_out, rec_out, prob_out, source);
+                source_in, cap_in, n_inst, pt, poly, whole_rec, whole_prob,
+                MergeRows{page_count, page_offset, pts_out, polys_out, rec_out, prob_out, source});
   });
 }
 
@@ -1073,31 +1089,19 @@ int alm_omni_merge_kie_tiles(alm_ctx* h, const int* heights, const int* widths, 
                              double* word_rect, double* word_poly, int32_t* word_source, long cap_words) {
   return guarded(h, [&] {
     const char* fn = "alm_omni_merge_kie_tiles";
-    ALM_REQUIRE(pages_ok(heights, widths, n_pages) && tile_core::valid_layout(tile, overlap), ALM_ERR_INVALID,
-                std::string(fn) + ": page sizes, or tile size / overlap (need tile >= 64, 0 <= 2 overlap <= tile)");
-    ALM_REQUIRE(std::isfinite(margin) && margin >= 0.0 && std::isfinite(band) && band >= 0.0 && std::isfinite(iou) &&
-                    iou > 0.0 && iou <= 1.0,
-                ALM_ERR_INVALID, std::string(fn) + ": margin and band must be finite and >= 0, iou in (0, 1]");
     ALM_REQUIRE(max_tok >= 1 && max_inst >= 1 && num_bins >= 1 && n_classes >= 1, ALM_ERR_INVALID,
                 std::string(fn) + ": max_tok, max_inst, num_bins and n_classes must be >= 1");
-    ALM_REQUIRE(tile_page && tile_origin && n_tok && tokens && tok_prob && n_inst && inst_pos && poly && page_count &&
-                    page_offset,
-                ALM_ERR_INVALID, std::string(fn) + ": null argument");
-    if (turns) require_turns(turns, n_pages, fn);
-    const std::vector<tile_core::Tile> tiles = page_tiles(heights, widths, n_pages, tile, overlap, band, turns);
-    ALM_REQUIRE(n_tiles == static_cast<int>(tiles.size()), ALM_ERR_INVALID,
-                std::string(fn) + ": " + std::to_string(n_tiles) + " tiles, the plan has " +
-                    std::to_string(tiles.size()));
+    ALM_REQUIRE(n_tok && tokens && tok_prob && n_inst && inst_pos && poly && page_count && page_offset, ALM_ERR_INVALID,
+                std::string(fn) + ": null argument");
+    const std::vector<tile_core::Tile> tiles = merge_plan(fn, heights, widths, n_pages, turns, tile, overlap, margin,
+                                                          band, iou, n_tiles, tile_page, tile_origin);
     // the walk of every tile's token stream: the checks, and the entity table of the merge
     std::vector<std::vector<kie_tile_core::Entity>> per(static_cast<size_t>(n_tiles));
     std::vector<int> n_ent(static_cast<size_t>(n_tiles));
     long ents = 0, words = 0;
     int max_ent = 1;
     for (int k = 0; k < n_tiles; ++k) {
-      const tile_core::Tile& t = tiles[static_cast<size_t>(k)];
       const std::string at = std::string(fn) + ": tile " + std::to_string(k);
-      ALM_REQUIRE(tile_page[k] == t.page && tile_origin[2 * k] == t.y0 && tile_origin[2 * k + 1] == t.x0,
-                  ALM_ERR_INVALID, at + " is not the plan's tile " + std::to_string(k) + " (pages in order, tiles row-major)");
       ALM_REQUIRE(n_tok[k] >= 0 && n_tok[k] <= max_tok, ALM_ERR_INVALID, at + ": n_tok outside [0, max_tok]");
       ALM_REQUIRE(n_inst[k] >= 0 && n_inst[k] <= max_inst, ALM_ERR_INVALID, at + ": n_inst outside [0, max_inst]");
       const long o = static_cast<long>(k) * max_tok;

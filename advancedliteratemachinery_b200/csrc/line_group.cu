@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "alm_internal.h"
+#include "block_scan.cuh"
 #include "group_core.h"
 #include "pre.h"
 
@@ -32,19 +33,6 @@ struct Pages {
   const int* offset;  // [n] first row
   const long* block;  // [n + 1] first block of each page in the pair / order grids: max(1, ceil(count / 128)) each
 };
-
-// sum of v over the block (every thread gets it); red: kThreads / 32 ints of shared memory
-template <int kThreads>
-__device__ int block_sum(int v, int* red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  int s = 0;
-#pragma unroll
-  for (int k = 0; k < kThreads / 32; ++k) s += red[k];
-  return s;
-}
 
 __global__ void __launch_bounds__(kBlock)
 group_frame_kernel(int N, const double* __restrict__ polys, double* __restrict__ F) {
@@ -143,7 +131,7 @@ group_chain_kernel(Pages pg, const int* __restrict__ succ, const int* __restrict
     if (nxt[i] < 0) len[k.a[i]] = k.r[i] + 1;  // the line's last word: one writer per head
     heads += prv[i] < 0;
   }
-  const int total = block_sum<kChainBlock>(heads, red);
+  const int total = block_scan::block_sum<kChainBlock>(heads, red);
   if (tid == 0) n_lines[p] = total;
 }
 
@@ -162,9 +150,7 @@ group_order_kernel(int N, Pages pg, const double* __restrict__ F, const int* __r
   const int li = chunk * kBlock + tid;
   const bool live = li < cnt;
   const int w = off + li;
-  int s = 0;
-  for (int q = tid; q < p; q += kBlock) s += n_lines[q];
-  const int before = block_sum<kBlock>(s, red);  // lines of the pages before this one
+  const int before = block_scan::range_sum<kBlock>(n_lines, 0, p, red);  // lines of the pages before this one
   if (chunk == 0 && tid == 0) line_offset[p] = before;
   const int h = live ? head[w] : 0;
   const double hy = live ? F[static_cast<long>(N) + h] : 0.0, hx = live ? F[h] : 0.0;
@@ -224,32 +210,21 @@ void group_lines(Ctx* c, int n_pages, const int* page_count, const int* page_off
   for (int p = 0; p < n_pages; ++p)
     block[p + 1] = block[p] + std::max(1, (page_count[p] + kBlock - 1) / kBlock);
   const unsigned nblk = static_cast<unsigned>(block[n_pages]);
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* src, size_t bytes) {
-    void* d = ws.alloc(bytes);
-    ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
-  Pages pg;
-  pg.n = n_pages;
-  pg.count = static_cast<const int*>(up(page_count, n_pages * sizeof(int)));
-  pg.offset = static_cast<const int*>(up(page_offset, n_pages * sizeof(int)));
-  pg.block = static_cast<const long*>(up(block.data(), block.size() * sizeof(long)));
-  const auto* d_polys = static_cast<const double*>(up(polys, N * 32 * sizeof(double)));
-  double* F = ws.get<double>(N * kFrame);
-  int* succ = ws.get<int>(N);
-  int* pred = ws.get<int>(N);
-  int* nxt = ws.get<int>(N);
-  int* prv = ws.get<int>(N);
-  Rank k{ws.get<int>(N), ws.get<int>(N), ws.get<int>(N), ws.get<int>(N), ws.get<int>(N), ws.get<int>(N)};
-  uint8_t* cyc = ws.get<uint8_t>(N);
-  int* len = ws.get<int>(N);
-  int* o_page = ws.get<int>(2 * static_cast<size_t>(n_pages));  // n_lines [n_pages], line_offset [n_pages]
-  int* o_line = ws.get<int>(2 * N);                             // line_first [N], line_words [N]
-  int* o_word = ws.get<int>(3 * N);                             // order [N], line_of [N], rank_of [N]
-  double* o_polys = ws.get<double>(N * 32);
+  Staging st(c);
+  const Pages pg{n_pages, st.up(page_count, n_pages), st.up(page_offset, n_pages), st.up(block.data(), block.size())};
+  const double* d_polys = st.up(polys, N * 32);
+  double* F = st.out<double>(N * kFrame);
+  int* succ = st.out<int>(N);
+  int* pred = st.out<int>(N);
+  int* nxt = st.out<int>(N);
+  int* prv = st.out<int>(N);
+  Rank k{st.out<int>(N), st.out<int>(N), st.out<int>(N), st.out<int>(N), st.out<int>(N), st.out<int>(N)};
+  uint8_t* cyc = st.out<uint8_t>(N);
+  int* len = st.out<int>(N);
+  int* o_page = st.out<int>(2 * static_cast<size_t>(n_pages));  // n_lines [n_pages], line_offset [n_pages]
+  int* o_line = st.out<int>(2 * N);                             // line_first [N], line_words [N]
+  int* o_word = st.out<int>(3 * N);                             // order [N], line_of [N], rank_of [N]
+  double* o_polys = st.out<double>(N * 32);
   const int n = static_cast<int>(N);
   const unsigned wblk = static_cast<unsigned>((N + kBlock - 1) / kBlock);
 
@@ -266,20 +241,17 @@ void group_lines(Ctx* c, int n_pages, const int* page_count, const int* page_off
                                                        o_line + N, o_word, o_polys);
   count_launch(c); check_launch("group_polygon");
 
-  auto down = [&](void* dst, const void* src, size_t bytes) {
-    ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
-  };
-  down(n_lines, o_page, n_pages * sizeof(int));
-  down(line_offset, o_page + n_pages, n_pages * sizeof(int));
-  down(order, o_word, N * sizeof(int));
-  down(line_of, o_word + N, N * sizeof(int));
-  down(rank_of, o_word + 2 * N, N * sizeof(int));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));  // also: the pageable uploads above are done
+  st.down(n_lines, o_page, n_pages);
+  st.down(line_offset, o_page + n_pages, n_pages);
+  st.down(order, o_word, N);
+  st.down(line_of, o_word + N, N);
+  st.down(rank_of, o_word + 2 * N, N);
+  st.sync();  // also: the pageable uploads above are done
   const long total = static_cast<long>(line_offset[n_pages - 1]) + n_lines[n_pages - 1];
-  down(line_first, o_line, total * sizeof(int));
-  down(line_words, o_line + N, total * sizeof(int));
-  down(line_polys, o_polys, total * 32 * sizeof(double));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+  st.down(line_first, o_line, total);
+  st.down(line_words, o_line + N, total);
+  st.down(line_polys, o_polys, total * 32);
+  st.sync();
 }
 
 }  // namespace alm

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 
+#include "block_scan.cuh"
 #include "box_core.h"
 #include "fuse_core.h"
 #include "line_core.h"
@@ -203,25 +204,15 @@ line_stitch_kernel(const int* __restrict__ ids, const float* __restrict__ probs,
                    const int* __restrict__ cnt, const float* __restrict__ boxes, const float* __restrict__ centres,
                    const double* __restrict__ X, int* __restrict__ ids_out, float* __restrict__ probs_out,
                    int* __restrict__ n_out, float* __restrict__ box_out, float* __restrict__ cen_out) {
-  constexpr int kWarps = line_core::kStitchThreads / 32;
-  __shared__ int warp_kept[kWarps];
-  const int r = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  __shared__ int warp_kept[line_core::kStitchThreads / 32];
+  const int r = blockIdx.x, t = threadIdx.x;
   const int w0 = wstart[r], nw = wstart[r + 1] - w0;
   const bool keep = line_core::stitch_keeps(t, w0, nw, win, cnt, X);
-  const unsigned m = __ballot_sync(0xffffffffu, keep);
-  if (lane == 0) warp_kept[warp] = __popc(m);
-  __syncthreads();
-  int before = 0, total = 0;
-#pragma unroll
-  for (int k = 0; k < kWarps; ++k) {
-    before += k < warp ? warp_kept[k] : 0;
-    total += warp_kept[k];
-  }
+  const block_scan::Rank k = block_scan::ballot_rank<line_core::kStitchThreads>(keep, warp_kept);
   if (keep)
-    line_core::stitch_put(r, t, before + __popc(m & ((1u << lane) - 1u)), w0, ids, probs, boxes, centres, ids_out,
-                          probs_out, box_out, cen_out);
-  line_core::stitch_fill(r, t, total, w0, nw, head, ids, probs, cnt, ids_out, probs_out, box_out, cen_out);
-  if (t == 0) n_out[r] = total;
+    line_core::stitch_put(r, t, k.pos, w0, ids, probs, boxes, centres, ids_out, probs_out, box_out, cen_out);
+  line_core::stitch_fill(r, t, k.total, w0, nw, head, ids, probs, cnt, ids_out, probs_out, box_out, cen_out);
+  if (t == 0) n_out[r] = k.total;
 }
 
 // Orientation selection (MgpSelect): one output of every head, [n_a3][N][row] 4-byte words on the device, gathered to

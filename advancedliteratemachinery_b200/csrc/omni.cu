@@ -1959,8 +1959,8 @@ void omni_decode_dense(Ctx* c, const int64_t* prompt, int n_prompt, const alm_de
         row_of(merged[j], w, i, &d_pts[n * 2], &d_polys[n * 32], &d_rec[n * L], &d_prob[n * L]);
       }
   reading_merge(c, np, nr, count.data(), offset.data(), L, cfg.recog_pad, cfg.rec_eos, iou, d_pts.data(),
-                d_polys.data(), d_rec.data(), d_prob.data(), pc.data(), po.data(), o_pts.data(), o_polys.data(),
-                o_rec.data(), o_prob.data(), src.data());
+                d_polys.data(), d_rec.data(), d_prob.data(),
+                MergeRows{pc.data(), po.data(), o_pts.data(), o_polys.data(), o_rec.data(), o_prob.data(), src.data()});
   for (int j = 0; j < np; ++j) {
     const int b = merged[j];
     n_inst[b] = pc[j];

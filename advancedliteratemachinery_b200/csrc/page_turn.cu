@@ -90,24 +90,17 @@ void tile_gather(Ctx* c, const std::vector<PreImage>& pages, const std::vector<t
 void orient_select(Ctx* c, int n_pages, int max_inst, int L, int64_t pad, int64_t eos, const int* n_inst,
                    const int64_t* rec, const float* prob, int* turns_out, double* scores) {
   const long R = 4L * n_pages, S = R * max_inst * L;
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* src, size_t bytes) {
-    void* d = ws.alloc(bytes);
-    ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
-  const auto* d_n = static_cast<const int*>(up(n_inst, R * sizeof(int)));
-  const auto* d_rec = static_cast<const int64_t*>(up(rec, S * sizeof(int64_t)));
-  const auto* d_prob = static_cast<const float*>(up(prob, S * sizeof(float)));
-  int* d_turns = ws.get<int>(n_pages);
-  double* d_scores = ws.get<double>(R);
+  Staging st(c);
+  const int* d_n = st.up(n_inst, R);
+  const int64_t* d_rec = st.up(rec, S);
+  const float* d_prob = st.up(prob, S);
+  int* d_turns = st.out<int>(n_pages);
+  double* d_scores = st.out<double>(R);
   orient_select_kernel<<<n_pages, 128, 0, c->stream>>>(max_inst, L, d_n, d_rec, d_prob, pad, eos, d_turns, d_scores);
   count_launch(c); check_launch("orient_select");
-  ALM_CHECK_CUDA(cudaMemcpyAsync(turns_out, d_turns, n_pages * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaMemcpyAsync(scores, d_scores, R * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+  st.down(turns_out, d_turns, n_pages);
+  st.down(scores, d_scores, R);
+  st.sync();
 }
 
 }  // namespace alm

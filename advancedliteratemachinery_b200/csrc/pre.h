@@ -1,5 +1,6 @@
 // Test-time image pipeline (preproc.cu): shared declarations.
 #pragma once
+#include <algorithm>
 #include <vector>
 
 #include "alm_internal.h"
@@ -10,6 +11,52 @@
 #include "whole_core.h"
 
 namespace alm {
+
+// Host <-> device staging of one call on the context's stream, in workspace buffers released when the call ends.
+// Every buffer gets at least one element, so an empty one is still a valid pointer, and empty copies are skipped.
+class Staging {
+ public:
+  explicit Staging(Ctx* c) : c_(c), scope_(ready(c)) {}
+  // a device buffer of n elements
+  template <class T>
+  T* out(size_t n) {
+    return c_->ws.get<T>(std::max<size_t>(n, 1));
+  }
+  // a device copy of host src [n]; src must stay valid until the next sync()
+  template <class T>
+  const T* up(const T* src, size_t n) {
+    T* d = out<T>(n);
+    if (n) ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, c_->stream));
+    return d;
+  }
+  // host dst [n] from device src, complete after the next sync()
+  template <class T>
+  void down(T* dst, const T* src, size_t n) {
+    if (n) ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, c_->stream));
+  }
+  void sync() { ALM_CHECK_CUDA(cudaStreamSynchronize(c_->stream)); }
+
+ private:
+  static Arena& ready(Ctx* c) {
+    c->ensure_ws();
+    return c->ws;
+  }
+  Ctx* c_;
+  ArenaScope scope_;
+};
+
+// Host outputs of the row merges (tile_merge, reading_merge, whole_merge): per page its kept row count and its first
+// kept row [n_pages], then the kept rows in page order, each pts [2], polys [32], rec [L], prob [L] and source [2].
+// The row buffers hold at least the merge's input rows.
+struct MergeRows {
+  int* page_count;
+  int* page_offset;
+  double* pts;
+  double* polys;
+  int64_t* rec;
+  float* prob;
+  int* source;
+};
 
 enum { PRE_BILINEAR = 0, PRE_BICUBIC = 1 };
 
@@ -73,12 +120,11 @@ void pre_line_crops(Ctx* c, const std::vector<PreImage>& pages, const std::vecto
 
 // Pages spotted in tiles (tile_core.h, tile_merge.cu): merge the decoded instances of `tiles` (the plan's tiles of every
 // page in plan order; max_inst slots each, the layout of alm_omni_decode, host buffers) into page coordinates.  Writes
-// page_count / page_offset [n_pages] and the kept rows (page then tile then instance order) to the host outputs, which
-// hold at least sum(n_inst) rows.  Three launches whatever the page and tile counts.
+// the page counts and offsets and the kept rows (page then tile then instance order) to out, whose rows hold at least
+// sum(n_inst).  Three launches whatever the page and tile counts.
 void tile_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, int max_inst, int L, int num_bins,
                 double margin, double iou, const int* n_inst, const int64_t* pt, const int64_t* poly, const int64_t* rec,
-                const float* prob, int* page_count, int* page_offset, double* pts_out, double* polys_out,
-                int64_t* rec_out, float* prob_out, int* source);
+                const float* prob, const MergeRows& out);
 
 // Turned pages (page_turn.cu, DESIGN 4.14).  tile_gather: tiles idx[0], idx[1], ... of `tiles` (make_tile /
 // make_turned_tile of the staged `pages`) cut into one workspace buffer, [h][w][3] each, in one launch; imgs gets one
@@ -90,31 +136,24 @@ void tile_gather(Ctx* c, const std::vector<PreImage>& pages, const std::vector<t
 void orient_select(Ctx* c, int n_pages, int max_inst, int L, int64_t pad, int64_t eos, const int* n_inst,
                    const int64_t* rec, const float* prob, int* turns_out, double* scores);
 
-// A page's four turned readings merged into one set of words (tile_merge.cu; rule: turn_core.h, DESIGN 4.15).  Host
-// inputs in the layout alm_omni_merge_tiles_turned writes for 4 n_pages readings (reading 4 p + k = page p at turn k;
-// count / offset [4 n_pages], offsets the exclusive prefix of the counts, checked by the caller); host outputs as
-// there, source = (turn, index within the reading).  Three launches.
-void turn_merge(Ctx* c, int n_pages, const int* count, const int* offset, int L, int64_t pad, int64_t eos, double iou,
-                const double* pts, const double* polys, const int64_t* rec, const float* prob, int* page_count,
-                int* page_offset, double* pts_out, double* polys_out, int64_t* rec_out, float* prob_out,
-                int* source);
-// The same merge over nr readings per page (reading nr p + k = page p's reading k; DESIGN 4.16 for the window readings
-// of a dense page): source = (k, index within the reading).  turn_merge is nr = 4.  Three launches.
+// A page's nr readings merged into one set of words (tile_merge.cu; rule: turn_core.h): its four turned readings
+// (nr = 4, DESIGN 4.15) or a dense page's window readings (DESIGN 4.16).  Host inputs in the layout
+// alm_omni_merge_tiles_turned writes for nr n_pages readings (reading nr p + k = page p's reading k; count / offset
+// [nr n_pages], offsets the exclusive prefix of the counts, checked by the caller); out as tile_merge's, source = (k,
+// index within the reading).  Three launches.
 void reading_merge(Ctx* c, int n_pages, int nr, const int* count, const int* offset, int L, int64_t pad, int64_t eos,
                    double iou, const double* pts, const double* polys, const int64_t* rec, const float* prob,
-                   int* page_count, int* page_offset, double* pts_out, double* polys_out, int64_t* rec_out,
-                   float* prob_out, int* source);
+                   const MergeRows& out);
 
 // Words that cross tile seams, recovered from a whole-page reading of each page (tile_merge.cu; rule: whole_core.h,
 // DESIGN 4.17).  Host inputs: the tile merge's rows of the pages (count / offset [n_pages], offsets the exclusive
 // prefix of the counts, checked by the caller; pts, polys, rec, prob, src in the layout alm_omni_merge_tiles writes) and
 // the whole-page readings in the layout of alm_omni_decode with cap slots per page (n_inst [n_pages] in [0, cap]).
-// Host outputs hold at least sum(count) + sum(n_inst) rows.  Three launches.
+// The rows of out hold at least sum(count) + sum(n_inst).  Three launches.
 void whole_merge(Ctx* c, const std::vector<whole_core::Page>& pages, int T, int ov, int num_bins, double margin,
                  int L, const int* count, const int* offset, const double* pts, const double* polys,
                  const int64_t* rec, const float* prob, const int* src, int cap, const int* n_inst, const int64_t* pt,
-                 const int64_t* poly, const int64_t* wrec, const float* wprob, int* page_count, int* page_offset,
-                 double* pts_out, double* polys_out, int64_t* rec_out, float* prob_out, int* source);
+                 const int64_t* poly, const int64_t* wrec, const float* wprob, const MergeRows& out);
 
 // KIE entities of pages read in tiles, turned or not (tile_merge.cu; rule: kie_tile_core.h, DESIGN 4.18).  Host
 // inputs: the entity table of every tile (max_ent slots per tile, n_ent [tiles] used; kie_tile_core::walk's rows, checked

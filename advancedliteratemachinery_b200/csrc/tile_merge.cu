@@ -7,7 +7,8 @@
 //                        slots of the block in instance order by a warp ballot (no atomics: bit-reproducible); the
 //                        first block of a page also writes the page's count and offset; rows of a turned page
 //                        (DESIGN 4.14) are mapped back to the upright page as they are written
-// Only the kept rows, the per-page counts and offsets cross PCIe back.
+// Only the kept rows, the per-page counts and offsets cross PCIe back.  The block sums and ballot ranks of every
+// compaction are block_scan.cuh's.
 //
 // The merge of a page's nr readings (rule: turn_core.h; four turned readings, DESIGN 4.15, or a dense page's window
 // readings, DESIGN 4.16), three launches whatever the counts:
@@ -51,6 +52,7 @@
 #include <vector>
 
 #include "alm_internal.h"
+#include "block_scan.cuh"
 #include "pre.h"
 #include "kie_tile_core.h"
 #include "rec_box_core.h"
@@ -73,16 +75,26 @@ tile_map_kernel(long S, int max_inst, const tile_core::Tile* __restrict__ tiles,
   if (g < S) tile_core::map_slot(g, max_inst, tiles, n_inst, pt, poly, num_bins, margin, pts, polys, box, dist, cand);
 }
 
-// sum of v over the block (every thread gets it); red: kWarps ints of shared memory
-__device__ int block_sum(int v, int* red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  int s = 0;
-#pragma unroll
-  for (int k = 0; k < kWarps; ++k) s += red[k];
-  return s;
+// Where a compaction block puts its kept slots: before = the kept count of every earlier block (blk_count), pos = a
+// kept slot's output row, the block's kept slots following in thread order.  red, warp_kept: kWarps ints of shared
+// memory each
+struct Place {
+  int before, pos;
+};
+__device__ __forceinline__ Place place(const int* blk_count, bool kept, int* red, int* warp_kept) {
+  const int before = block_scan::range_sum<kBlock>(blk_count, 0, blockIdx.x, red);
+  return Place{before, before + block_scan::ballot_rank<kBlock>(kept, warp_kept).pos};
+}
+
+// Called by the first block of a page only (uniform over the block): the page's count, the kept count of its blocks
+// [b0, b1), and its offset, the kept count of the blocks before it
+__device__ __forceinline__ void put_page(const int* blk_count, int b0, int b1, int before, int* count, int* offset,
+                                         int* red) {
+  const int total = block_scan::range_sum<kBlock>(blk_count, b0, b1, red);
+  if (threadIdx.x == 0) {
+    *offset = before;
+    *count = total;
+  }
 }
 
 __global__ void __launch_bounds__(kBlock)
@@ -130,7 +142,7 @@ tile_pair_kernel(int max_inst, int nchunk, const tile_core::Tile* __restrict__ t
   }
   const bool kp = live && !dropped;
   if (i < max_inst) keep[g] = kp;
-  const int total = block_sum(kp ? 1 : 0, red);
+  const int total = block_scan::block_sum<kBlock>(kp ? 1 : 0, red);
   if (tid == 0) blk_count[blk] = total;
 }
 
@@ -141,37 +153,19 @@ tile_compact_kernel(int max_inst, int nchunk, int L, const tile_core::Tile* __re
                     double* __restrict__ pts_out, double* __restrict__ polys_out, int64_t* __restrict__ rec_out,
                     float* __restrict__ prob_out, int* __restrict__ source, int* __restrict__ page_count,
                     int* __restrict__ page_offset) {
-  __shared__ int red[kWarps];
-  __shared__ int warp_kept[kWarps];
-  const int blk = blockIdx.x, t = blk / nchunk, chunk = blk - t * nchunk, tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int i = chunk * kBlock + tid;
+  __shared__ int red[kWarps], warp_kept[kWarps];
+  const int t = blockIdx.x / nchunk, chunk = blockIdx.x - t * nchunk, i = chunk * kBlock + threadIdx.x;
   const long g = static_cast<long>(t) * max_inst + i;
-  int s = 0;
-  for (int b = tid; b < blk; b += kBlock) s += blk_count[b];
-  const int before = block_sum(s, red);
   const bool kp = i < max_inst && keep[g];
-  const unsigned m = __ballot_sync(0xffffffffu, kp);
-  if (lane == 0) warp_kept[warp] = __popc(m);
-  __syncthreads();
-  int pos = before + __popc(m & ((1u << lane) - 1u));
-#pragma unroll
-  for (int k = 0; k < kWarps; ++k) pos += k < warp ? warp_kept[k] : 0;
+  const Place at = place(blk_count, kp, red, warp_kept);
   const tile_core::Tile tl = tiles[t];
   if (kp) {
-    tile_core::put(g, pos, max_inst, L, pts, polys, rec, prob, pts_out, polys_out, rec_out, prob_out, source);
-    tile_core::unturn_row(pos, tl, pts_out, polys_out);  // turned pages only (DESIGN 4.14)
+    tile_core::put(g, at.pos, max_inst, L, pts, polys, rec, prob, pts_out, polys_out, rec_out, prob_out, source);
+    tile_core::unturn_row(at.pos, tl, pts_out, polys_out);  // turned pages only (DESIGN 4.14)
   }
-  if (chunk == 0 && t == tl.first) {  // uniform over the block
-    const int b0 = tl.first * nchunk, b1 = (tl.first + tl.nx * tl.ny) * nchunk;
-    int c = 0;
-    for (int b = b0 + tid; b < b1; b += kBlock) c += blk_count[b];
-    const int count = block_sum(c, red);
-    if (tid == 0) {
-      page_offset[tl.page] = before;
-      page_count[tl.page] = count;
-    }
-  }
+  if (chunk == 0 && t == tl.first)  // uniform over the block
+    put_page(blk_count, tl.first * nchunk, (tl.first + tl.nx * tl.ny) * nchunk, at.before, &page_count[tl.page],
+             &page_offset[tl.page], red);
 }
 
 __global__ void __launch_bounds__(kBlock)
@@ -227,7 +221,7 @@ turn_pair_kernel(int nr_arg, const turn_core::Blk* __restrict__ blks, const int*
   }
   const bool kp = live && !dropped;
   if (live) keep[n] = kp;
-  const int total = block_sum(kp ? 1 : 0, red);
+  const int total = block_scan::block_sum<kBlock>(kp ? 1 : 0, red);
   if (tid == 0) blk_count[blk] = total;
 }
 
@@ -239,34 +233,18 @@ turn_compact_kernel(int nr_arg, int L, const turn_core::Blk* __restrict__ blks, 
                     const float* __restrict__ prob, double* __restrict__ pts_out, double* __restrict__ polys_out,
                     int64_t* __restrict__ rec_out, float* __restrict__ prob_out, int* __restrict__ source,
                     int* __restrict__ page_count, int* __restrict__ page_offset) {
-  __shared__ int red[kWarps];
-  __shared__ int warp_kept[kWarps];
+  __shared__ int red[kWarps], warp_kept[kWarps];
   const int nr = kNr ? kNr : nr_arg;
-  const int blk = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const turn_core::Blk b = blks[blk];
-  const int i = b.row0 + tid;
+  const turn_core::Blk b = blks[blockIdx.x];
+  const int i = b.row0 + threadIdx.x;
   const long n = static_cast<long>(offset[b.reading]) + i;
-  int s = 0;
-  for (int q = tid; q < blk; q += kBlock) s += blk_count[q];
-  const int before = block_sum(s, red);
   const bool kp = i < count[b.reading] && keep[n];
-  const unsigned m = __ballot_sync(0xffffffffu, kp);
-  if (lane == 0) warp_kept[warp] = __popc(m);
-  __syncthreads();
-  int pos = before + __popc(m & ((1u << lane) - 1u));
-#pragma unroll
-  for (int q = 0; q < kWarps; ++q) pos += q < warp ? warp_kept[q] : 0;
+  const Place at = place(blk_count, kp, red, warp_kept);
   if (kp)
-    turn_core::put(n, pos, b.reading % nr, i, L, pts, polys, rec, prob, pts_out, polys_out, rec_out, prob_out, source);
-  if (blk == b.blk_first) {  // uniform over the block
-    int c = 0;
-    for (int q = b.blk_first + tid; q < b.blk_end; q += kBlock) c += blk_count[q];
-    const int total = block_sum(c, red);
-    if (tid == 0) {
-      page_offset[b.page] = before;
-      page_count[b.page] = total;
-    }
-  }
+    turn_core::put(n, at.pos, b.reading % nr, i, L, pts, polys, rec, prob, pts_out, polys_out, rec_out, prob_out,
+                   source);
+  if (static_cast<int>(blockIdx.x) == b.blk_first)  // uniform over the block
+    put_page(blk_count, b.blk_first, b.blk_end, at.before, &page_count[b.page], &page_offset[b.page], red);
 }
 
 __global__ void __launch_bounds__(kBlock)
@@ -317,7 +295,7 @@ whole_pair_kernel(const turn_core::Blk* __restrict__ blks, const int* __restrict
     kp = live && !dropped;
     if (live) keep[n] = kp;
   }
-  const int total = block_sum(kp ? 1 : 0, red);
+  const int total = block_scan::block_sum<kBlock>(kp ? 1 : 0, red);
   if (tid == 0) blk_count[blk] = total;
 }
 
@@ -330,37 +308,21 @@ whole_compact_kernel(int L, const turn_core::Blk* __restrict__ blks, const int* 
                      const int64_t* __restrict__ wrec, const float* __restrict__ wprob, double* __restrict__ pts_out,
                      double* __restrict__ polys_out, int64_t* __restrict__ rec_out, float* __restrict__ prob_out,
                      int* __restrict__ source, int* __restrict__ page_count, int* __restrict__ page_offset) {
-  __shared__ int red[kWarps];
-  __shared__ int warp_kept[kWarps];
-  const int blk = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const turn_core::Blk b = blks[blk];
-  const int i = b.row0 + tid;
+  __shared__ int red[kWarps], warp_kept[kWarps];
+  const turn_core::Blk b = blks[blockIdx.x];
+  const int i = b.row0 + threadIdx.x;
   const long n = static_cast<long>(offset[b.reading]) + i;
-  int s = 0;
-  for (int q = tid; q < blk; q += kBlock) s += blk_count[q];
-  const int before = block_sum(s, red);
   const bool kp = i < count[b.reading] && keep[n];
-  const unsigned m = __ballot_sync(0xffffffffu, kp);
-  if (lane == 0) warp_kept[warp] = __popc(m);
-  __syncthreads();
-  int pos = before + __popc(m & ((1u << lane) - 1u));
-#pragma unroll
-  for (int q = 0; q < kWarps; ++q) pos += q < warp ? warp_kept[q] : 0;
+  const Place at = place(blk_count, kp, red, warp_kept);
   if (kp) {
     if (b.reading & 1)
-      whole_core::put_whole(n - N, pos, i, L, wpts, wpolys, wrec, wprob, pts_out, polys_out, rec_out, prob_out, source);
+      whole_core::put_whole(n - N, at.pos, i, L, wpts, wpolys, wrec, wprob, pts_out, polys_out, rec_out, prob_out,
+                            source);
     else
-      whole_core::put_tile(n, pos, L, pts, polys, rec, prob, src, pts_out, polys_out, rec_out, prob_out, source);
+      whole_core::put_tile(n, at.pos, L, pts, polys, rec, prob, src, pts_out, polys_out, rec_out, prob_out, source);
   }
-  if (blk == b.blk_first) {  // uniform over the block
-    int c = 0;
-    for (int q = b.blk_first + tid; q < b.blk_end; q += kBlock) c += blk_count[q];
-    const int total = block_sum(c, red);
-    if (tid == 0) {
-      page_offset[b.page] = before;
-      page_count[b.page] = total;
-    }
-  }
+  if (static_cast<int>(blockIdx.x) == b.blk_first)  // uniform over the block
+    put_page(blk_count, b.blk_first, b.blk_end, at.before, &page_count[b.page], &page_offset[b.page], red);
 }
 
 __global__ void __launch_bounds__(kBlock)
@@ -373,23 +335,6 @@ kie_map_kernel(long S, int max_ent, int max_inst, const tile_core::Tile* __restr
     kie_tile_core::map_entity(g, max_ent, max_inst, tiles, n_ent, ents, poly, num_bins, margin, box, dist, cand);
 }
 
-// exclusive prefix of v over the block in thread order (every thread gets its own); red: kWarps ints of shared memory
-__device__ int block_exclusive(int v, int* red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int x = v;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  __syncthreads();
-  if (lane == 31) red[warp] = x;
-  __syncthreads();
-  int before = x - v;
-#pragma unroll
-  for (int k = 0; k < kWarps; ++k) before += k < warp ? red[k] : 0;
-  return before;
-}
-
 __global__ void __launch_bounds__(kBlock)
 kie_count_kernel(int max_ent, int nchunk, const kie_tile_core::Entity* __restrict__ ents,
                  const uint8_t* __restrict__ keep, int* __restrict__ blk_words) {
@@ -397,7 +342,7 @@ kie_count_kernel(int max_ent, int nchunk, const kie_tile_core::Entity* __restric
   const int blk = blockIdx.x, t = blk / nchunk, e = (blk - t * nchunk) * kBlock + threadIdx.x;
   const long g = static_cast<long>(t) * max_ent + e;
   const int words = e < max_ent && keep[g] ? ents[g].words : 0;
-  const int total = block_sum(words, red);
+  const int total = block_scan::block_sum<kBlock>(words, red);
   if (threadIdx.x == 0) blk_words[blk] = total;
 }
 
@@ -410,45 +355,24 @@ kie_compact_kernel(int max_ent, int max_inst, int nchunk, int num_bins, int n_pa
                    float* __restrict__ prob_out, int* __restrict__ word_offset, int* __restrict__ word_count,
                    int* __restrict__ ent_src, double* __restrict__ rects, double* __restrict__ polys,
                    int* __restrict__ word_src, int* __restrict__ o_page) {
-  __shared__ int red[kWarps];
-  __shared__ int warp_kept[kWarps];
-  const int blk = blockIdx.x, t = blk / nchunk, chunk = blk - t * nchunk, tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int e = chunk * kBlock + tid;
+  __shared__ int red[kWarps], warp_kept[kWarps];
+  const int t = blockIdx.x / nchunk, chunk = blockIdx.x - t * nchunk, e = chunk * kBlock + threadIdx.x;
   const long g = static_cast<long>(t) * max_ent + e;
-  int s = 0, sw = 0;
-  for (int b = tid; b < blk; b += kBlock) {
-    s += blk_count[b];
-    sw += blk_words[b];
-  }
-  const int before = block_sum(s, red);
-  const int wbefore = block_sum(sw, red);
   const bool kp = e < max_ent && keep[g];
+  const Place at = place(blk_count, kp, red, warp_kept);
+  const int wbefore = block_scan::range_sum<kBlock>(blk_words, 0, blockIdx.x, red);
   const int words = kp ? ents[g].words : 0;
-  const int wpos = wbefore + block_exclusive(words, red);
-  const unsigned m = __ballot_sync(0xffffffffu, kp);
-  if (lane == 0) warp_kept[warp] = __popc(m);
-  __syncthreads();
-  int pos = before + __popc(m & ((1u << lane) - 1u));
-#pragma unroll
-  for (int k = 0; k < kWarps; ++k) pos += k < warp ? warp_kept[k] : 0;
+  const int wpos = wbefore + block_scan::block_exclusive<kBlock>(words, red);
   if (kp)
-    kie_tile_core::put_entity(g, pos, wpos, max_ent, max_inst, tiles, ents, poly, num_bins, cls_out, prob_out,
+    kie_tile_core::put_entity(g, at.pos, wpos, max_ent, max_inst, tiles, ents, poly, num_bins, cls_out, prob_out,
                               word_offset, word_count, ent_src, rects, polys, word_src);
   const tile_core::Tile tl = tiles[t];
-  if (chunk == 0 && t == tl.first) {  // uniform over the block
-    const int b0 = tl.first * nchunk, b1 = (tl.first + tl.nx * tl.ny) * nchunk;
-    int c = 0;
-    for (int b = b0 + tid; b < b1; b += kBlock) c += blk_count[b];
-    const int count = block_sum(c, red);
-    if (tid == 0) {
-      o_page[n_pages + tl.page] = before;
-      o_page[tl.page] = count;
-    }
-  }
-  if (blk == static_cast<int>(gridDim.x) - 1) {  // uniform over the block
-    const int last = block_sum(words, red);
-    if (tid == 0) o_page[2 * n_pages] = wbefore + last;
+  if (chunk == 0 && t == tl.first)  // uniform over the block
+    put_page(blk_count, tl.first * nchunk, (tl.first + tl.nx * tl.ny) * nchunk, at.before, &o_page[tl.page],
+             &o_page[n_pages + tl.page], red);
+  if (blockIdx.x == gridDim.x - 1) {  // uniform over the block
+    const int last = block_scan::block_sum<kBlock>(words, red);
+    if (threadIdx.x == 0) o_page[2 * n_pages] = wbefore + last;
   }
 }
 
@@ -494,43 +418,57 @@ rec_box_kernel(long N, int L, const rec_box_core::Frame* __restrict__ frames, co
   if (lane == 0) n_chars[n] = kept;
 }
 
+// A row merge's outputs on the device (MergeRows): room for `rows` rows, and the page counts then offsets [2 n_pages]
+struct DevRows {
+  int n_pages, L;
+  double* pts;
+  double* polys;
+  int64_t* rec;
+  float* prob;
+  int* source;
+  int* page;
+  DevRows(Staging& st, size_t rows, int L, int n_pages)
+      : n_pages(n_pages), L(L), pts(st.out<double>(rows * 2)), polys(st.out<double>(rows * 32)),
+        rec(st.out<int64_t>(rows * L)), prob(st.out<float>(rows * L)), source(st.out<int>(rows * 2)),
+        page(st.out<int>(2 * static_cast<size_t>(n_pages))) {}
+  // the page counts and offsets, then the kept rows, to the host
+  void download(Staging& st, const MergeRows& h) const {
+    st.down(h.page_count, page, n_pages);
+    st.down(h.page_offset, page + n_pages, n_pages);
+    st.sync();  // also: the pageable uploads are done
+    const long total = static_cast<long>(h.page_offset[n_pages - 1]) + h.page_count[n_pages - 1];
+    st.down(h.pts, pts, total * 2);
+    st.down(h.polys, polys, total * 32);
+    st.down(h.rec, rec, total * L);
+    st.down(h.prob, prob, total * L);
+    st.down(h.source, source, total * 2);
+    st.sync();
+  }
+};
+
 }  // namespace
 
 void tile_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, int max_inst, int L, int num_bins,
                 double margin, double iou, const int* n_inst, const int64_t* pt, const int64_t* poly, const int64_t* rec,
-                const float* prob, int* page_count, int* page_offset, double* pts_out, double* polys_out,
-                int64_t* rec_out, float* prob_out, int* source) {
+                const float* prob, const MergeRows& out) {
   const int nt = static_cast<int>(tiles.size());
   const long S = static_cast<long>(nt) * max_inst;
-  const int nchunk = (max_inst + kBlock - 1) / kBlock;
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* src, size_t bytes) {
-    void* d = ws.alloc(bytes);
-    ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
-  const auto* d_tiles = static_cast<const tile_core::Tile*>(up(tiles.data(), tiles.size() * sizeof(tile_core::Tile)));
-  const auto* d_n = static_cast<const int*>(up(n_inst, nt * sizeof(int)));
-  const auto* d_pt = static_cast<const int64_t*>(up(pt, S * 2 * sizeof(int64_t)));
-  const auto* d_poly = static_cast<const int64_t*>(up(poly, S * 32 * sizeof(int64_t)));
-  const auto* d_rec = static_cast<const int64_t*>(up(rec, S * L * sizeof(int64_t)));
-  const auto* d_prob = static_cast<const float*>(up(prob, S * L * sizeof(float)));
-  double* pts = ws.get<double>(S * 2);
-  double* polys = ws.get<double>(S * 32);
-  double* box = ws.get<double>(S * 4);
-  double* dist = ws.get<double>(S);
-  uint8_t* cand = ws.get<uint8_t>(S);
-  uint8_t* keep = ws.get<uint8_t>(S);
-  const int nblk = nt * nchunk;
-  int* blk_count = ws.get<int>(nblk);
-  double* o_pts = ws.get<double>(S * 2);
-  double* o_polys = ws.get<double>(S * 32);
-  int64_t* o_rec = ws.get<int64_t>(S * L);
-  float* o_prob = ws.get<float>(S * L);
-  int* o_src = ws.get<int>(S * 2);
-  int* o_page = ws.get<int>(2 * static_cast<size_t>(n_pages));  // count [n_pages], offset [n_pages]
+  const int nchunk = (max_inst + kBlock - 1) / kBlock, nblk = nt * nchunk;
+  Staging st(c);
+  const tile_core::Tile* d_tiles = st.up(tiles.data(), tiles.size());
+  const int* d_n = st.up(n_inst, nt);
+  const int64_t* d_pt = st.up(pt, S * 2);
+  const int64_t* d_poly = st.up(poly, S * 32);
+  const int64_t* d_rec = st.up(rec, S * L);
+  const float* d_prob = st.up(prob, S * L);
+  double* pts = st.out<double>(S * 2);
+  double* polys = st.out<double>(S * 32);
+  double* box = st.out<double>(S * 4);
+  double* dist = st.out<double>(S);
+  uint8_t* cand = st.out<uint8_t>(S);
+  uint8_t* keep = st.out<uint8_t>(S);
+  int* blk_count = st.out<int>(nblk);
+  const DevRows o(st, S, L, n_pages);
 
   tile_map_kernel<<<static_cast<unsigned>((S + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(
       S, max_inst, d_tiles, d_n, d_pt, d_poly, num_bins, margin, pts, polys, box, dist, cand);
@@ -538,63 +476,34 @@ void tile_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, 
   tile_pair_kernel<<<nblk, kBlock, 0, c->stream>>>(max_inst, nchunk, d_tiles, d_n, box, dist, cand, iou, keep, blk_count);
   count_launch(c); check_launch("tile_pair");
   tile_compact_kernel<<<nblk, kBlock, 0, c->stream>>>(max_inst, nchunk, L, d_tiles, blk_count, keep, pts, polys, d_rec,
-                                                      d_prob, o_pts, o_polys, o_rec, o_prob, o_src, o_page,
-                                                      o_page + n_pages);
+                                                      d_prob, o.pts, o.polys, o.rec, o.prob, o.source, o.page,
+                                                      o.page + n_pages);
   count_launch(c); check_launch("tile_compact");
-
-  ALM_CHECK_CUDA(cudaMemcpyAsync(page_count, o_page, n_pages * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaMemcpyAsync(page_offset, o_page + n_pages, n_pages * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));  // also: the pageable uploads above are done
-  const long total = static_cast<long>(page_offset[n_pages - 1]) + page_count[n_pages - 1];
-  if (total > 0) {
-    auto down = [&](void* dst, const void* src, size_t bytes) {
-      ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
-    };
-    down(pts_out, o_pts, total * 2 * sizeof(double));
-    down(polys_out, o_polys, total * 32 * sizeof(double));
-    down(rec_out, o_rec, total * L * sizeof(int64_t));
-    down(prob_out, o_prob, total * L * sizeof(float));
-    down(source, o_src, total * 2 * sizeof(int));
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-  }
+  o.download(st, out);
 }
 
 void reading_merge(Ctx* c, int n_pages, int nr, const int* count, const int* offset, int L, int64_t pad, int64_t eos,
                    double iou, const double* pts, const double* polys, const int64_t* rec, const float* prob,
-                   int* page_count, int* page_offset, double* pts_out, double* polys_out, int64_t* rec_out,
-                   float* prob_out, int* source) {
+                   const MergeRows& out) {
   const int R = nr * n_pages;
   const long N = static_cast<long>(offset[R - 1]) + count[R - 1];
   const std::vector<turn_core::Blk> blks = turn_core::blocks(n_pages, nr, count);
   const int nblk = static_cast<int>(blks.size());
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* src, size_t bytes) {
-    void* d = ws.alloc(std::max<size_t>(bytes, 1));
-    if (bytes) ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
-  const auto* d_blks = static_cast<const turn_core::Blk*>(up(blks.data(), blks.size() * sizeof(turn_core::Blk)));
-  const auto* d_count = static_cast<const int*>(up(count, R * sizeof(int)));
-  const auto* d_offset = static_cast<const int*>(up(offset, R * sizeof(int)));
-  const auto* d_pts = static_cast<const double*>(up(pts, N * 2 * sizeof(double)));
-  const auto* d_polys = static_cast<const double*>(up(polys, N * 32 * sizeof(double)));
-  const auto* d_rec = static_cast<const int64_t*>(up(rec, N * L * sizeof(int64_t)));
-  const auto* d_prob = static_cast<const float*>(up(prob, N * L * sizeof(float)));
-  const size_t rows = static_cast<size_t>(std::max<long>(N, 1));
-  double* box = ws.get<double>(rows * 4);
-  double* score = ws.get<double>(rows);
-  uint8_t* keep = ws.get<uint8_t>(rows);
-  int* blk_count = ws.get<int>(nblk);
-  double* o_pts = ws.get<double>(rows * 2);
-  double* o_polys = ws.get<double>(rows * 32);
-  int64_t* o_rec = ws.get<int64_t>(rows * L);
-  float* o_prob = ws.get<float>(rows * L);
-  int* o_src = ws.get<int>(rows * 2);
-  int* o_page = ws.get<int>(2 * static_cast<size_t>(n_pages));  // count [n_pages], offset [n_pages]
+  Staging st(c);
+  const turn_core::Blk* d_blks = st.up(blks.data(), blks.size());
+  const int* d_count = st.up(count, R);
+  const int* d_offset = st.up(offset, R);
+  const double* d_pts = st.up(pts, N * 2);
+  const double* d_polys = st.up(polys, N * 32);
+  const int64_t* d_rec = st.up(rec, N * L);
+  const float* d_prob = st.up(prob, N * L);
+  double* box = st.out<double>(N * 4);
+  double* score = st.out<double>(N);
+  uint8_t* keep = st.out<uint8_t>(N);
+  int* blk_count = st.out<int>(nblk);
+  const DevRows o(st, N, L, n_pages);
 
-  turn_map_kernel<<<static_cast<unsigned>((rows + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(
+  turn_map_kernel<<<static_cast<unsigned>((std::max<long>(N, 1) + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(
       N, L, d_polys, d_rec, d_prob, pad, eos, box, score);
   count_launch(c); check_launch("turn_map");
   auto pair = nr == 4 ? turn_pair_kernel<4> : turn_pair_kernel<0>;
@@ -602,39 +511,15 @@ void reading_merge(Ctx* c, int n_pages, int nr, const int* count, const int* off
   pair<<<nblk, kBlock, 0, c->stream>>>(nr, d_blks, d_count, d_offset, box, score, iou, keep, blk_count);
   count_launch(c); check_launch("turn_pair");
   compact<<<nblk, kBlock, 0, c->stream>>>(nr, L, d_blks, d_count, d_offset, blk_count, keep, d_pts, d_polys, d_rec,
-                                          d_prob, o_pts, o_polys, o_rec, o_prob, o_src, o_page, o_page + n_pages);
+                                          d_prob, o.pts, o.polys, o.rec, o.prob, o.source, o.page, o.page + n_pages);
   count_launch(c); check_launch("turn_compact");
-
-  ALM_CHECK_CUDA(cudaMemcpyAsync(page_count, o_page, n_pages * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaMemcpyAsync(page_offset, o_page + n_pages, n_pages * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));  // also: the pageable uploads above are done
-  const long total = static_cast<long>(page_offset[n_pages - 1]) + page_count[n_pages - 1];
-  if (total > 0) {
-    auto down = [&](void* dst, const void* src, size_t bytes) {
-      ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
-    };
-    down(pts_out, o_pts, total * 2 * sizeof(double));
-    down(polys_out, o_polys, total * 32 * sizeof(double));
-    down(rec_out, o_rec, total * L * sizeof(int64_t));
-    down(prob_out, o_prob, total * L * sizeof(float));
-    down(source, o_src, total * 2 * sizeof(int));
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-  }
-}
-
-void turn_merge(Ctx* c, int n_pages, const int* count, const int* offset, int L, int64_t pad, int64_t eos, double iou,
-                const double* pts, const double* polys, const int64_t* rec, const float* prob, int* page_count,
-                int* page_offset, double* pts_out, double* polys_out, int64_t* rec_out, float* prob_out,
-                int* source) {
-  reading_merge(c, n_pages, 4, count, offset, L, pad, eos, iou, pts, polys, rec, prob, page_count, page_offset,
-                pts_out, polys_out, rec_out, prob_out, source);
+  o.download(st, out);
 }
 
 void whole_merge(Ctx* c, const std::vector<whole_core::Page>& pages, int T, int ov, int num_bins, double margin,
                  int L, const int* count, const int* offset, const double* pts, const double* polys,
                  const int64_t* rec, const float* prob, const int* src, int cap, const int* n_inst, const int64_t* pt,
-                 const int64_t* poly, const int64_t* wrec, const float* wprob, int* page_count, int* page_offset,
-                 double* pts_out, double* polys_out, int64_t* rec_out, float* prob_out, int* source) {
+                 const int64_t* poly, const int64_t* wrec, const float* wprob, const MergeRows& out) {
   const int P = static_cast<int>(pages.size());
   const long N = static_cast<long>(offset[P - 1]) + count[P - 1];
   const long S = static_cast<long>(P) * cap;
@@ -647,39 +532,26 @@ void whole_merge(Ctx* c, const std::vector<whole_core::Page>& pages, int T, int 
   }
   const std::vector<turn_core::Blk> blks = turn_core::blocks(P, 2, count2.data());
   const int nblk = static_cast<int>(blks.size());
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* p, size_t bytes) {
-    void* d = ws.alloc(std::max<size_t>(bytes, 1));
-    if (bytes) ALM_CHECK_CUDA(cudaMemcpyAsync(d, p, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
-  const auto* d_pages = static_cast<const whole_core::Page*>(up(pages.data(), P * sizeof(whole_core::Page)));
-  const auto* d_blks = static_cast<const turn_core::Blk*>(up(blks.data(), blks.size() * sizeof(turn_core::Blk)));
-  const auto* d_count = static_cast<const int*>(up(count2.data(), count2.size() * sizeof(int)));
-  const auto* d_offset = static_cast<const int*>(up(offset2.data(), offset2.size() * sizeof(int)));
-  const auto* d_pts = static_cast<const double*>(up(pts, N * 2 * sizeof(double)));
-  const auto* d_polys = static_cast<const double*>(up(polys, N * 32 * sizeof(double)));
-  const auto* d_rec = static_cast<const int64_t*>(up(rec, N * L * sizeof(int64_t)));
-  const auto* d_prob = static_cast<const float*>(up(prob, N * L * sizeof(float)));
-  const auto* d_src = static_cast<const int*>(up(src, N * 2 * sizeof(int)));
-  const auto* d_n = static_cast<const int*>(up(n_inst, P * sizeof(int)));
-  const auto* d_pt = static_cast<const int64_t*>(up(pt, S * 2 * sizeof(int64_t)));
-  const auto* d_poly = static_cast<const int64_t*>(up(poly, S * 32 * sizeof(int64_t)));
-  const auto* d_wrec = static_cast<const int64_t*>(up(wrec, S * L * sizeof(int64_t)));
-  const auto* d_wprob = static_cast<const float*>(up(wprob, S * L * sizeof(float)));
-  const size_t rows = static_cast<size_t>(N + S);
-  double* wpts = ws.get<double>(S * 2);
-  double* wpolys = ws.get<double>(S * 32);
-  uint8_t* keep = ws.get<uint8_t>(rows);
-  int* blk_count = ws.get<int>(nblk);
-  double* o_pts = ws.get<double>(rows * 2);
-  double* o_polys = ws.get<double>(rows * 32);
-  int64_t* o_rec = ws.get<int64_t>(rows * L);
-  float* o_prob = ws.get<float>(rows * L);
-  int* o_src = ws.get<int>(rows * 2);
-  int* o_page = ws.get<int>(2 * static_cast<size_t>(P));  // count [P], offset [P]
+  Staging st(c);
+  const whole_core::Page* d_pages = st.up(pages.data(), pages.size());
+  const turn_core::Blk* d_blks = st.up(blks.data(), blks.size());
+  const int* d_count = st.up(count2.data(), count2.size());
+  const int* d_offset = st.up(offset2.data(), offset2.size());
+  const double* d_pts = st.up(pts, N * 2);
+  const double* d_polys = st.up(polys, N * 32);
+  const int64_t* d_rec = st.up(rec, N * L);
+  const float* d_prob = st.up(prob, N * L);
+  const int* d_src = st.up(src, N * 2);
+  const int* d_n = st.up(n_inst, P);
+  const int64_t* d_pt = st.up(pt, S * 2);
+  const int64_t* d_poly = st.up(poly, S * 32);
+  const int64_t* d_wrec = st.up(wrec, S * L);
+  const float* d_wprob = st.up(wprob, S * L);
+  double* wpts = st.out<double>(S * 2);
+  double* wpolys = st.out<double>(S * 32);
+  uint8_t* keep = st.out<uint8_t>(N + S);
+  int* blk_count = st.out<int>(nblk);
+  const DevRows o(st, N + S, L, P);
 
   whole_map_kernel<<<static_cast<unsigned>((S + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(
       S, cap, d_pages, d_n, d_pt, d_poly, T, ov, num_bins, margin, wpts, wpolys, keep + N);
@@ -688,24 +560,9 @@ void whole_merge(Ctx* c, const std::vector<whole_core::Page>& pages, int T, int 
   count_launch(c); check_launch("whole_pair");
   whole_compact_kernel<<<nblk, kBlock, 0, c->stream>>>(L, d_blks, d_count, d_offset, N, blk_count, keep, d_pts,
                                                        d_polys, d_rec, d_prob, d_src, wpts, wpolys, d_wrec, d_wprob,
-                                                       o_pts, o_polys, o_rec, o_prob, o_src, o_page, o_page + P);
+                                                       o.pts, o.polys, o.rec, o.prob, o.source, o.page, o.page + P);
   count_launch(c); check_launch("whole_compact");
-
-  ALM_CHECK_CUDA(cudaMemcpyAsync(page_count, o_page, P * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaMemcpyAsync(page_offset, o_page + P, P * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));  // also: the pageable uploads above are done
-  const long total = static_cast<long>(page_offset[P - 1]) + page_count[P - 1];
-  if (total > 0) {
-    auto down = [&](void* dst, const void* from, size_t bytes) {
-      ALM_CHECK_CUDA(cudaMemcpyAsync(dst, from, bytes, cudaMemcpyDeviceToHost, c->stream));
-    };
-    down(pts_out, o_pts, total * 2 * sizeof(double));
-    down(polys_out, o_polys, total * 32 * sizeof(double));
-    down(rec_out, o_rec, total * L * sizeof(int64_t));
-    down(prob_out, o_prob, total * L * sizeof(float));
-    down(source, o_src, total * 2 * sizeof(int));
-    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
-  }
+  o.download(st, out);
 }
 
 void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, int max_ent, const int* n_ent,
@@ -715,39 +572,30 @@ void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, i
   const int nt = static_cast<int>(tiles.size());
   const long S = static_cast<long>(nt) * max_ent;
   const long SI = static_cast<long>(nt) * max_inst;
-  const int nchunk = (max_ent + kBlock - 1) / kBlock;
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* src, size_t bytes) {
-    void* d = ws.alloc(bytes);
-    ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
-  const auto* d_tiles = static_cast<const tile_core::Tile*>(up(tiles.data(), tiles.size() * sizeof(tile_core::Tile)));
-  const auto* d_n = static_cast<const int*>(up(n_ent, nt * sizeof(int)));
-  const auto* d_ents = static_cast<const kie_tile_core::Entity*>(up(ents, S * sizeof(kie_tile_core::Entity)));
-  const auto* d_poly = static_cast<const int64_t*>(up(poly, SI * 32 * sizeof(int64_t)));
-  double* box = ws.get<double>(S * 4);
-  double* dist = ws.get<double>(S);
-  uint8_t* cand = ws.get<uint8_t>(S);
-  uint8_t* keep = ws.get<uint8_t>(S);
-  const int nblk = nt * nchunk;
-  int* blk_count = ws.get<int>(nblk);
-  int* blk_words = ws.get<int>(nblk);
+  const int nchunk = (max_ent + kBlock - 1) / kBlock, nblk = nt * nchunk;
   long words = 0;  // every entity's words: an upper bound of the kept ones
   for (long g = 0; g < S; ++g)
     if (g % max_ent < n_ent[g / max_ent]) words += ents[g].words;
-  const size_t W = static_cast<size_t>(std::max<long>(words, 1));
-  int* o_cls = ws.get<int>(S);
-  float* o_prob = ws.get<float>(S);
-  int* o_woff = ws.get<int>(S);
-  int* o_wcnt = ws.get<int>(S);
-  int* o_src = ws.get<int>(S * 2);
-  double* o_rects = ws.get<double>(W * 4);
-  double* o_polys = ws.get<double>(W * 32);
-  int* o_wsrc = ws.get<int>(W * 2);
-  int* o_page = ws.get<int>(2 * static_cast<size_t>(n_pages) + 1);  // count, offset [n_pages], word total
+  Staging st(c);
+  const tile_core::Tile* d_tiles = st.up(tiles.data(), tiles.size());
+  const int* d_n = st.up(n_ent, nt);
+  const kie_tile_core::Entity* d_ents = st.up(ents, S);
+  const int64_t* d_poly = st.up(poly, SI * 32);
+  double* box = st.out<double>(S * 4);
+  double* dist = st.out<double>(S);
+  uint8_t* cand = st.out<uint8_t>(S);
+  uint8_t* keep = st.out<uint8_t>(S);
+  int* blk_count = st.out<int>(nblk);
+  int* blk_words = st.out<int>(nblk);
+  int* o_cls = st.out<int>(S);
+  float* o_prob = st.out<float>(S);
+  int* o_woff = st.out<int>(S);
+  int* o_wcnt = st.out<int>(S);
+  int* o_src = st.out<int>(S * 2);
+  double* o_rects = st.out<double>(words * 4);
+  double* o_polys = st.out<double>(words * 32);
+  int* o_wsrc = st.out<int>(words * 2);
+  int* o_page = st.out<int>(2 * static_cast<size_t>(n_pages) + 1);  // count, offset [n_pages], word total
 
   kie_map_kernel<<<static_cast<unsigned>((S + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(
       S, max_ent, max_inst, d_tiles, d_n, d_ents, d_poly, num_bins, margin, box, dist, cand);
@@ -762,61 +610,48 @@ void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, i
   count_launch(c); check_launch("kie_compact");
 
   std::vector<int> hp(2 * static_cast<size_t>(n_pages) + 1);
-  ALM_CHECK_CUDA(cudaMemcpyAsync(hp.data(), o_page, hp.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));  // also: the pageable uploads above are done
+  st.down(hp.data(), o_page, hp.size());
+  st.sync();  // also: the pageable uploads above are done
   std::copy(hp.begin(), hp.begin() + n_pages, page_count);
   std::copy(hp.begin() + n_pages, hp.begin() + 2 * n_pages, page_offset);
   const long total = static_cast<long>(page_offset[n_pages - 1]) + page_count[n_pages - 1];
   const long kept_words = hp[2 * static_cast<size_t>(n_pages)];
-  auto down = [&](void* dst, const void* src, size_t bytes) {
-    if (bytes) ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
-  };
-  down(cls_out, o_cls, total * sizeof(int));
-  down(prob_out, o_prob, total * sizeof(float));
-  down(word_offset, o_woff, total * sizeof(int));
-  down(word_count, o_wcnt, total * sizeof(int));
-  down(ent_src, o_src, total * 2 * sizeof(int));
-  down(rects, o_rects, kept_words * 4 * sizeof(double));
-  down(polys, o_polys, kept_words * 32 * sizeof(double));
-  down(word_src, o_wsrc, kept_words * 2 * sizeof(int));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+  st.down(cls_out, o_cls, total);
+  st.down(prob_out, o_prob, total);
+  st.down(word_offset, o_woff, total);
+  st.down(word_count, o_wcnt, total);
+  st.down(ent_src, o_src, total * 2);
+  st.down(rects, o_rects, kept_words * 4);
+  st.down(polys, o_polys, kept_words * 32);
+  st.down(word_src, o_wsrc, kept_words * 2);
+  st.sync();
 }
 
 void char_boxes(Ctx* c, long N, int L, int F, const rec_box_core::Frame* frames, const int* frame_index,
                 const double* polys, const int64_t* rec, const float* loc, int64_t pad, int64_t eos, int* n_chars,
                 int* step, double* centre, double* cov, double* box) {
   if (N == 0) return;
-  c->ensure_ws();
-  ArenaScope arena_scope(c->ws);
-  Arena& ws = c->ws;
-  auto up = [&](const void* src, size_t bytes) {
-    void* d = ws.alloc(bytes);
-    ALM_CHECK_CUDA(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
-    return d;
-  };
   const size_t S = static_cast<size_t>(N) * L;
-  const auto* d_frames = static_cast<const rec_box_core::Frame*>(up(frames, F * sizeof(rec_box_core::Frame)));
-  const auto* d_fi = static_cast<const int*>(up(frame_index, N * sizeof(int)));
-  const auto* d_polys = static_cast<const double*>(up(polys, N * 32 * sizeof(double)));
-  const auto* d_rec = static_cast<const int64_t*>(up(rec, S * sizeof(int64_t)));
-  const auto* d_loc = static_cast<const float*>(up(loc, S * 5 * sizeof(float)));
-  int* o_n = ws.get<int>(N);
-  int* o_step = ws.get<int>(S);
-  double* o_centre = ws.get<double>(S * 2);
-  double* o_cov = ws.get<double>(S * 3);
-  double* o_box = ws.get<double>(S * 8);
+  Staging st(c);
+  const rec_box_core::Frame* d_frames = st.up(frames, F);
+  const int* d_fi = st.up(frame_index, N);
+  const double* d_polys = st.up(polys, N * 32);
+  const int64_t* d_rec = st.up(rec, S);
+  const float* d_loc = st.up(loc, S * 5);
+  int* o_n = st.out<int>(N);
+  int* o_step = st.out<int>(S);
+  double* o_centre = st.out<double>(S * 2);
+  double* o_cov = st.out<double>(S * 3);
+  double* o_box = st.out<double>(S * 8);
   rec_box_kernel<<<static_cast<unsigned>((N + kBoxWords - 1) / kBoxWords), kBlock, 0, c->stream>>>(
       N, L, d_frames, d_fi, d_polys, d_rec, d_loc, pad, eos, o_n, o_step, o_centre, o_cov, o_box);
   count_launch(c); check_launch("rec_box");
-  auto down = [&](void* dst, const void* src, size_t bytes) {
-    ALM_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
-  };
-  down(n_chars, o_n, N * sizeof(int));
-  down(step, o_step, S * sizeof(int));
-  down(centre, o_centre, S * 2 * sizeof(double));
-  down(cov, o_cov, S * 3 * sizeof(double));
-  down(box, o_box, S * 8 * sizeof(double));
-  ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
+  st.down(n_chars, o_n, N);
+  st.down(step, o_step, S);
+  st.down(centre, o_centre, S * 2);
+  st.down(cov, o_cov, S * 3);
+  st.down(box, o_box, S * 8);
+  st.sync();
 }
 
 }  // namespace alm

@@ -171,6 +171,31 @@ def check_merge_args(margin, band, iou):
     return margin, band, iou
 
 
+def _size_arrays(sizes):
+    """The heights and widths int32 [P] of pages given as (h, w) sizes."""
+    hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
+    ws = np.ascontiguousarray([int(s[1]) for s in sizes], dtype=np.int32)
+    return hs, ws
+
+
+_ROW_MERGE_OUT = ('count', 'offset', 'pts', 'polys', 'rec', 'prob', 'source')  # in the order of the C arguments
+
+
+def _row_merge_out(P: int, K: int, L: int) -> dict:
+    """The output buffers of a row merge (alm_omni_merge_tiles, _readings, _whole_page): count / offset int32 [P] and
+    room for K >= 1 rows of rec_length L."""
+    return dict(count=np.zeros(P, np.int32), offset=np.zeros(P, np.int32), pts=np.zeros((K, 2)),
+                polys=np.zeros((K, 32)), rec=np.zeros((K, L), np.int64), prob=np.zeros((K, L), np.float32),
+                source=np.zeros((K, 2), np.int32))
+
+
+def _trim(out: dict, keys, n: int) -> dict:
+    """out with the arrays under keys cut to their first n rows."""
+    for k in keys:
+        out[k] = out[k][:n]
+    return out
+
+
 def merge_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_inst, pt, poly, rec, prob, num_bins: int,
                 margin: float = 4.0, band: Optional[float] = None, iou: float = 0.5, turns=None) -> dict:
     """The instances decoded from every tile of ``preprocess.omni_tile_plan(sizes, tile, overlap)`` (``plan``, in plan
@@ -186,8 +211,7 @@ def merge_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_inst,
     margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
     if turns is not None:
         turns = check_turns(turns, len(sizes))
-    hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
-    ws = np.ascontiguousarray([int(s[1]) for s in sizes], dtype=np.int32)
+    hs, ws = _size_arrays(sizes)
     plan = np.asarray(plan, dtype=np.int32).reshape(-1, 5)
     tpage = np.ascontiguousarray(plan[:, 0])
     torigin = np.ascontiguousarray(plan[:, 1:3])
@@ -198,24 +222,18 @@ def merge_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_inst,
     if not (len(n_inst) == T == len(plan) and poly.shape == (T, maxi, 32) and rec.shape == (T, maxi, L) and
             prob.shape == rec.shape):
         raise ValueError('merge_tiles: per-tile outputs do not match the plan')
-    K = int(n_inst.sum())
+    K = max(int(n_inst.sum()), 1)
     P = len(hs)
-    out = dict(count=np.zeros(P, np.int32), offset=np.zeros(P, np.int32), pts=np.zeros((max(K, 1), 2)),
-               polys=np.zeros((max(K, 1), 32)), rec=np.zeros((max(K, 1), L), np.int64),
-               prob=np.zeros((max(K, 1), L), np.float32), source=np.zeros((max(K, 1), 2), np.int32))
+    out = _row_merge_out(P, K, L)
     args = (int(tile), int(overlap), T, tpage.ctypes.data, torigin.ctypes.data, n_inst.ctypes.data, pt.ctypes.data,
             poly.ctypes.data, rec.ctypes.data, prob.ctypes.data, maxi, L, int(num_bins), margin, band, iou,
-            out['count'].ctypes.data, out['offset'].ctypes.data, out['pts'].ctypes.data, out['polys'].ctypes.data,
-            out['rec'].ctypes.data, out['prob'].ctypes.data, out['source'].ctypes.data, max(K, 1))
+            *[out[k].ctypes.data for k in _ROW_MERGE_OUT], K)
     if turns is None:
         ctx.check(ctx.lib.alm_omni_merge_tiles(ctx.h, hs.ctypes.data, ws.ctypes.data, P, *args))
     else:
         ctx.check(ctx.lib.alm_omni_merge_tiles_turned(ctx.h, hs.ctypes.data, ws.ctypes.data, P, turns.ctypes.data,
                                                       *args))
-    n = int(out['count'].sum())
-    for k in ('pts', 'polys', 'rec', 'prob', 'source'):
-        out[k] = out[k][:n]
-    return out
+    return _trim(out, _ROW_MERGE_OUT[2:], int(out['count'].sum()))
 
 
 MAX_REC_LENGTH = 1021  # alm_omni_char_boxes' bound on rec_length, as alm_omni_decode's
@@ -355,8 +373,7 @@ def merge_whole_page(ctx: _lib.Context, sizes, tile: int, overlap: int, tiles: d
         raise ValueError(f'margin must be finite and >= 0, got {margin}')
     if turns is not None:
         turns = check_turns(turns, len(sizes))
-    hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
-    ws = np.ascontiguousarray([int(s[1]) for s in sizes], dtype=np.int32)
+    hs, ws = _size_arrays(sizes)
     P = len(hs)
     t = {k: np.ascontiguousarray(tiles[k], dtype=d) for k, d in
          (('count', np.int32), ('offset', np.int32), ('pts', np.float64), ('polys', np.float64), ('rec', np.int64),
@@ -373,19 +390,13 @@ def merge_whole_page(ctx: _lib.Context, sizes, tile: int, overlap: int, tiles: d
             prob.shape == rec.shape):
         raise ValueError('merge_whole_page: tile rows or whole-page readings do not match the pages')
     K = max(N + int(n_inst.sum()), 1)
-    out = dict(count=np.zeros(P, np.int32), offset=np.zeros(P, np.int32), pts=np.zeros((K, 2)),
-               polys=np.zeros((K, 32)), rec=np.zeros((K, L), np.int64), prob=np.zeros((K, L), np.float32),
-               source=np.zeros((K, 2), np.int32))
+    out = _row_merge_out(P, K, L)
     ctx.check(ctx.lib.alm_omni_merge_whole_page(
         ctx.h, hs.ctypes.data, ws.ctypes.data, P, None if turns is None else turns.ctypes.data, int(tile),
-        int(overlap), margin, int(num_bins), *[t[k].ctypes.data for k in ('count', 'offset', 'pts', 'polys', 'rec',
-                                                                          'prob', 'source')],
+        int(overlap), margin, int(num_bins), *[t[k].ctypes.data for k in _ROW_MERGE_OUT],
         n_inst.ctypes.data, pt.ctypes.data, poly.ctypes.data, rec.ctypes.data, prob.ctypes.data, cap_in, L,
-        *[out[k].ctypes.data for k in ('count', 'offset', 'pts', 'polys', 'rec', 'prob', 'source')], K))
-    n = int(out['count'].sum())
-    for k in ('pts', 'polys', 'rec', 'prob', 'source'):
-        out[k] = out[k][:n]
-    return out
+        *[out[k].ctypes.data for k in _ROW_MERGE_OUT], K))
+    return _trim(out, _ROW_MERGE_OUT[2:], int(out['count'].sum()))
 
 
 def merge_kie_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_tok, tokens, tok_prob, n_inst, inst_pos,
@@ -406,8 +417,7 @@ def merge_kie_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_t
     margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
     if turns is not None:
         turns = check_turns(turns, len(sizes))
-    hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
-    ws = np.ascontiguousarray([int(s[1]) for s in sizes], dtype=np.int32)
+    hs, ws = _size_arrays(sizes)
     plan = np.asarray(plan, dtype=np.int32).reshape(-1, 5)
     tpage = np.ascontiguousarray(plan[:, 0])
     torigin = np.ascontiguousarray(plan[:, 1:3])
@@ -433,13 +443,8 @@ def merge_kie_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_t
         inst_pos.shape[1], int(num_bins), int(class_base), int(n_classes), margin, band, iou,
         *[out[k].ctypes.data for k in ('count', 'offset', 'cls', 'prob', 'word_offset', 'word_count', 'source')], E,
         *[out[k].ctypes.data for k in ('rect', 'poly', 'word_source')], N))
-    n = int(out['count'].sum())
-    w = int(out['word_count'][:n].sum())
-    for k in ('cls', 'prob', 'word_offset', 'word_count', 'source'):
-        out[k] = out[k][:n]
-    for k in ('rect', 'poly', 'word_source'):
-        out[k] = out[k][:w]
-    return out
+    _trim(out, ('cls', 'prob', 'word_offset', 'word_count', 'source'), int(out['count'].sum()))
+    return _trim(out, ('rect', 'poly', 'word_source'), int(out['word_count'].sum()))
 
 
 def _tile_of(source_tile, first_tile):
@@ -468,20 +473,15 @@ def _merge_readings(ctx, nr, count, offset, pts, polys, rec, prob, recog_pad_ind
         raise ValueError(f'{name}: {int(count.sum())} rows counted, pts {pts.shape}, polys {polys.shape}, '
                          f'rec {rec.shape}, prob {prob.shape}')
     P, L, cap = R // nr, rec.shape[1], max(N, 1)
-    out = dict(count=np.zeros(P, np.int32), offset=np.zeros(P, np.int32), pts=np.zeros((cap, 2)),
-               polys=np.zeros((cap, 32)), rec=np.zeros((cap, L), np.int64), prob=np.zeros((cap, L), np.float32),
-               source=np.zeros((cap, 2), np.int32))
-    outs = [out[k].ctypes.data for k in ('count', 'offset', 'pts', 'polys', 'rec', 'prob', 'source')]
+    out = _row_merge_out(P, cap, L)
     args = (count.ctypes.data, offset.ctypes.data, pts.ctypes.data, polys.ctypes.data, rec.ctypes.data,
-            prob.ctypes.data, L, int(recog_pad_index), int(rec_eos_index), iou, *outs, cap)
+            prob.ctypes.data, L, int(recog_pad_index), int(rec_eos_index), iou,
+            *[out[k].ctypes.data for k in _ROW_MERGE_OUT], cap)
     if nr == 4 and name == 'merge_turns':
         ctx.check(ctx.lib.alm_omni_merge_turns(ctx.h, P, *args))
     else:
         ctx.check(ctx.lib.alm_omni_merge_readings(ctx.h, P, nr, *args))
-    n = int(out['count'].sum())
-    for k in ('pts', 'polys', 'rec', 'prob', 'source'):
-        out[k] = out[k][:n]
-    return out
+    return _trim(out, _ROW_MERGE_OUT[2:], int(out['count'].sum()))
 
 
 GROUP_DEFAULTS = dict(cos_tol=math.cos(math.radians(15.0)), height_ratio=0.5, max_offset=0.5, max_overlap=0.5,
@@ -675,8 +675,7 @@ class OmniParserB200:
         B, _, Hc, Wc = t.shape
         if len(sizes) != B:
             raise ValueError(f'{len(sizes)} sizes for {B} pages')
-        hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
-        ws = np.ascontiguousarray([int(s[1]) for s in sizes], dtype=np.int32)
+        hs, ws = _size_arrays(sizes)
         self._keep_img = t
         self.ctx.wait_torch(t)
         self.ctx.check(self.lib.alm_omni_encode_pages(self.ctx.h, t.data_ptr(), B, Hc, Wc, hs.ctypes.data,
