@@ -147,6 +147,9 @@ SIGNATURES = {
     # ctx, qkv, bias_table, out_f32, out_hi, out_lo, B, nWh, nWw, C, heads, shift
     'alm_op_window_attention_ex': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    # ctx, qkv_hi, qkv_lo, bias_table, out_f32, out_hi, out_lo, B, nWh, nWw, C, heads, shift
+    'alm_op_window_attention_planes': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     # ctx, src, lds, map, nsrc, Cs, rows, gamma, beta, eps, zero_missing, add, ld_add, out_f32, ldo_f32, out_hi, out_lo,
     # ldo_bf, out2_hi, out2_lo, out2_f32
     'alm_op_gather_ln': (C.c_int, [C.c_void_p, C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_int, C.c_long, C.c_void_p,

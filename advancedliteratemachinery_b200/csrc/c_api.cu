@@ -1740,6 +1740,21 @@ int alm_op_layernorm(alm_ctx* h, const float* x, const float* gamma, const float
 
 namespace {
 
+// the relative position bias table [169, heads] (device) as the dense [heads, 49, 49] the window kernels read, in the
+// workspace (the caller holds the arena scope and synchronizes before it closes)
+float* window_bias_dense(Ctx* c, const float* bias_table, int heads) {
+  std::vector<float> tab(static_cast<size_t>(169) * heads), dense(static_cast<size_t>(heads) * 2401);
+  ALM_CHECK_CUDA(cudaMemcpy(tab.data(), bias_table, tab.size() * 4, cudaMemcpyDeviceToHost));
+  for (int hh = 0; hh < heads; ++hh)
+    for (int i = 0; i < 49; ++i)
+      for (int j = 0; j < 49; ++j)
+        dense[static_cast<size_t>(hh) * 2401 + i * 49 + j] =
+            tab[static_cast<size_t>((i / 7 - j / 7 + 6) * 13 + (i % 7 - j % 7 + 6)) * heads + hh];
+  float* dd = c->ws.get<float>(dense.size());
+  ALM_CHECK_CUDA(cudaMemcpyAsync(dd, dense.data(), dense.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  return dd;
+}
+
 void op_window_attention(alm_ctx* h, const float* qkv, const float* bias_table, float* out_f32, void* out_hi,
                          void* out_lo, int B, int nWh, int nWw, int C, int heads, int shift) {
   ALM_REQUIRE(qkv && bias_table && (out_f32 || out_hi) && (!out_lo || out_hi) && B > 0 && nWh > 0 && nWw > 0 &&
@@ -1752,15 +1767,7 @@ void op_window_attention(alm_ctx* h, const float* qkv, const float* bias_table, 
     Ctx* c = &h->c;
     c->ensure_ws();
     ArenaScope arena_scope(c->ws);
-    std::vector<float> tab(static_cast<size_t>(169) * heads), dense(static_cast<size_t>(heads) * 2401);
-    ALM_CHECK_CUDA(cudaMemcpy(tab.data(), bias_table, tab.size() * 4, cudaMemcpyDeviceToHost));
-    for (int hh = 0; hh < heads; ++hh)
-      for (int i = 0; i < 49; ++i)
-        for (int j = 0; j < 49; ++j)
-          dense[static_cast<size_t>(hh) * 2401 + i * 49 + j] =
-              tab[static_cast<size_t>((i / 7 - j / 7 + 6) * 13 + (i % 7 - j % 7 + 6)) * heads + hh];
-    float* dd = c->ws.get<float>(dense.size());
-    ALM_CHECK_CUDA(cudaMemcpyAsync(dd, dense.data(), dense.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    float* dd = window_bias_dense(c, bias_table, heads);
     window_attention(c, qkv, C, heads, nWh, nWw, B, shift, nWh * 7, nWw * 7, dd, static_cast<bf16*>(out_hi),
                      static_cast<bf16*>(out_lo), out_f32);
     ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
@@ -1781,6 +1788,27 @@ int alm_op_window_attention_ex(alm_ctx* h, const float* qkv, const float* bias_t
                                void* out_lo, int B, int nWh, int nWw, int C, int heads, int shift) {
   return guarded(h, [&] {
     op_window_attention(h, qkv, bias_table, out_f32, out_hi, out_lo, B, nWh, nWw, C, heads, shift);
+  });
+}
+
+int alm_op_window_attention_planes(alm_ctx* h, const void* qkv_hi, const void* qkv_lo, const float* bias_table,
+                                   float* out_f32, void* out_hi, void* out_lo, int B, int nWh, int nWw, int C, int heads,
+                                   int shift) {
+  return guarded(h, [&] {
+    // both kernels of window_attention_split read the lo plane at every nsplit
+    ALM_REQUIRE(qkv_hi && qkv_lo && bias_table && (out_f32 || out_hi) && (!out_lo || out_hi) && B > 0 && nWh > 0 &&
+                    nWw > 0 && heads > 0 && shift >= 0 && shift < 7,
+                ALM_ERR_INVALID, "alm_op_window_attention_planes arguments");
+    require_device({qkv_hi, qkv_lo, bias_table, out_f32}, 16, "alm_op_window_attention_planes");
+    require_device({out_hi, out_lo}, 8, "alm_op_window_attention_planes");
+    ALM_REQUIRE(C == heads * 32, ALM_ERR_UNSUPPORTED, "alm_op_window_attention_planes: head_dim must be 32");
+    Ctx* c = &h->c;
+    c->ensure_ws();
+    ArenaScope arena_scope(c->ws);
+    float* dd = window_bias_dense(c, bias_table, heads);
+    window_attention_split(c, static_cast<const bf16*>(qkv_hi), static_cast<const bf16*>(qkv_lo), C, heads, nWh, nWw, B,
+                           shift, nWh * 7, nWw * 7, dd, static_cast<bf16*>(out_hi), static_cast<bf16*>(out_lo), out_f32);
+    ALM_CHECK_CUDA(cudaStreamSynchronize(c->stream));
   });
 }
 

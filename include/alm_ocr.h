@@ -602,6 +602,17 @@ ALM_API int alm_op_window_attention(alm_ctx* ctx, const float* qkv, const float*
  * ALM_ERR_INVALID for null or host pointers, sizes < 1 or shift outside 0..6; ALM_ERR_UNSUPPORTED for C != 32 heads. */
 ALM_API int alm_op_window_attention_ex(alm_ctx* ctx, const float* qkv, const float* bias_table, float* out_f32,
                                        void* out_hi, void* out_lo, int B, int nWh, int nWw, int C, int heads, int shift);
+/* The same core on the operands the Swin blocks hand it: qkv as device bf16 planes qkv_hi / qkv_lo (uint16 buffers)
+ * [B*nWh*nWw*49, 3C], the q columns already multiplied by 32^-0.5 (the encoder folds the scale into the qkv weight and
+ * bias), so the kernel forms q k^T from the planes' values hi + lo with no further scaling.  Runs the encoder's
+ * tensor-core kernel under the context's wattn_impl (3: persistent over head pairs when heads is even; 0 and 1: per
+ * (window, head)); both read the lo plane at every nsplit.  bias_table, outputs and shift as in
+ * alm_op_window_attention_ex.  qkv planes and out_f32 are aligned to 16 bytes, out_hi / out_lo to 8.  ALM_ERR_INVALID,
+ * before any device work, for null (qkv_lo included) or host pointers, misalignment, sizes < 1 or shift outside 0..6;
+ * ALM_ERR_UNSUPPORTED for C != 32 heads. */
+ALM_API int alm_op_window_attention_planes(alm_ctx* ctx, const void* qkv_hi, const void* qkv_lo,
+                                           const float* bias_table, float* out_f32, void* out_hi, void* out_lo, int B,
+                                           int nWh, int nWw, int C, int heads, int shift);
 /* The encoder's gather + LayerNorm + split (gather_ln).  Output row r (width C = nsrc * Cs) concatenates source rows
  * map[r * nsrc + s] (s = 0 .. nsrc - 1; -1 gives zeros; map NULL: row r * nsrc + s) of src f32 (row stride lds, the
  * first Cs values of each row are read).  gamma / beta [C] (NULL: no LayerNorm) normalise the row with eps.

@@ -28,7 +28,8 @@ def test_header_declares_the_documented_surface():
               'alm_last_error', 'alm_op_cross_attention', 'alm_op_self_attention_step', 'alm_op_gemv',
               'alm_op_head_select', 'alm_op_gather_ln', 'alm_op_swin_map', 'alm_op_patch_im2col', 'alm_op_fpn_assemble',
               'alm_op_sine_pos', 'alm_op_softmax_rows', 'alm_op_window_attention_ex', 'alm_op_gemm_planes',
-              'alm_op_attention_ex', 'alm_op_row_select', 'alm_op_embed_ln', 'alm_op_gather_ln_joint'):
+              'alm_op_attention_ex', 'alm_op_row_select', 'alm_op_embed_ln', 'alm_op_gather_ln_joint',
+              'alm_op_window_attention_planes'):
         assert s in syms
 
 

@@ -12,7 +12,7 @@ interpolation tap.  Here each kernel is compared element by element with the sam
 * the patch im2col with canvas slots, odd sizes and unaligned rows; the FPN assembly with bilinear taps at both
   borders; the sine position embedding with masks up to the shared-memory bound; the row softmax with masks;
 * the Swin window-attention core with sharp scores and the shift mask, at every head count and across the persistent
-  kernel's schedule.
+  kernel's schedule, on fp32 qkv and on the encoder's own operand: the split planes of a q already scaled by 32^-0.5.
 
 Every output buffer is followed by a guard region that must come back bit for bit unchanged, and input memory the call
 must not read holds NaN.  Wherever a kernel writes a split pair it must be hi = bf16_rn(x), lo = bf16_rn(x - hi) of the
@@ -377,7 +377,6 @@ FPN_PAGES = [(2, 68, 900), (2, 100, 900), (1, 1024, 1024), (1, 1920, 1920)]
 
 @pytest.mark.parametrize('B,H,W', FPN_PAGES)
 def test_fpn_assemble_matches_fp64(ctx, B, H, W):
-    from oracle import omniparser_ref as O
     grids = _stage_grids(H, W)
     gen = torch.Generator(device='cuda').manual_seed(H + W)
     levels = []
@@ -391,22 +390,32 @@ def test_fpn_assemble_matches_fp64(ctx, B, H, W):
     ctx.check(_op(ctx, 'alm_op_fpn_assemble', *[p.data_ptr() for p in levels], B, H, W, hi.data_ptr(), lo.data_ptr()))
     _assert_guard(hfull, n, -1)
     _assert_guard(lfull, n, -1)
+    for s, (err, tol) in enumerate(_fpn_err_tol(hi, lo, levels, grids)):
+        assert bool((err <= tol).all()), (s, float(err.max()))
+
+
+def _fpn_err_tol(hi, lo, levels, grids):
+    """the split pair hi / lo (int16, [rows * 1024]) of alm_op_fpn_assemble on levels [B, hs, ws, 256] (grids: their
+    (hs, ws)) against fp64: p3's columns must be its exact split; -> (|got - ref|, bound) of the bilinear levels p2, p4
+    and p5"""
+    from oracle import omniparser_ref as O
     # fpn.py:38-44 in fp64, then the stride-2 1 x 1 input_proj's sampling of pixels (2i, 2j)
     cat = O.fpn_concat(*[p.double().permute(0, 3, 1, 2) for p in levels])[:, :, ::2, ::2]
     ref = cat.permute(0, 2, 3, 1).reshape(-1, 1024)
-    hi, lo = hi.view(-1, 1024), lo.view(-1, 1024)
+    hi, lo = hi.reshape(-1, 1024), lo.reshape(-1, 1024)
     # p3: exact copies
     _assert_split(hi[:, 256:512].contiguous(), lo[:, 256:512].contiguous(), levels[1][:, ::2, ::2].reshape(-1, 256), 'p3')
     # bilinear levels: the kernel computes the source coordinate scale * (dst + 0.5) - 0.5 in fp32 (3 roundings, each
     # <= 2^-24 * in), so a tap may move by 3 * 2^-24 * in along each axis, changing the value by that times
     # 2 * max|p|; plus 16 ulp of max|p| for the fp32 lerp and 2^-16 relative for the split pair (hi + lo)
     got = _joined(hi, lo)
+    out = []
     for s, c0 in ((0, 0), (2, 512), (3, 768)):
         hs, ws = grids[s]
         pmax = float(levels[s].abs().max())
         tol = pmax * U32 * (6 * (hs + ws) + 16) + 2.0 ** -16 * ref[:, c0:c0 + 256].abs()
-        err = (got[:, c0:c0 + 256] - ref[:, c0:c0 + 256]).abs()
-        assert bool((err <= tol).all()), (s, float(err.max()))
+        out.append(((got[:, c0:c0 + 256] - ref[:, c0:c0 + 256]).abs(), tol))
+    return out
 
 
 # ----------------------------------------------------------------------------------------------- sine position embedding
@@ -570,14 +579,15 @@ def _wattn_inputs(B, nWh, nWw, heads, shift, seed):
     return qkv, tab
 
 
-def _wattn_tol(qkv, heads, B, nWh, nWw):
+def _wattn_tol(qkv, heads, B, nWh, nWw, scale=32 ** -0.5):
     """|got - ref| bound per element for the three-term split (hi*hi + lo*hi + hi*lo of operands held to 2^-16 relative):
     each product is off by at most e = 3 * 2^-16 of its magnitude, so a score s_ij by e * A_ij, A_ij = sum_d
-    |q_d k_d| * 32^-0.5, which moves the output o_i by at most e * max_j A_ij * max_j |v_j - o_i| <= e * A_i * 2 V;
-    P.V adds e * V (V = max |v| of the window and head).  fp32 softmax terms are orders of magnitude below these."""
+    |q_d k_d| * scale, which moves the output o_i by at most e * max_j A_ij * max_j |v_j - o_i| <= e * A_i * 2 V;
+    P.V adds e * V (V = max |v| of the window and head).  fp32 softmax terms are orders of magnitude below these.
+    scale 1: q already scaled (the encoder's qkv planes)."""
     e = 3 * 2.0 ** -16
     q, k, v = qkv.double().view(-1, 49, 3, heads, 32).permute(2, 0, 3, 1, 4)
-    A = ((q.abs() * 32 ** -0.5) @ k.abs().transpose(-1, -2)).amax(-1)         # [nW, heads, 49]
+    A = ((q.abs() * scale) @ k.abs().transpose(-1, -2)).amax(-1)              # [nW, heads, 49]
     V = v.abs().amax((-1, -2))                                               # [nW, heads]
     t = e * (2 * A * V[..., None] + V[..., None])
     return t.transpose(1, 2).unsqueeze(-1).expand(-1, 49, heads, 32).reshape(qkv.shape[0], heads * 32)
@@ -597,11 +607,48 @@ def _run_wattn(ctx, qkv, tab, B, nWh, nWw, heads, shift, f32=True):
     return out.view(rows, C), hi, lo
 
 
+WATTN_QSCALE = 0.17677669529663687     # 32^-0.5 in fp32, folded into the encoder's q rows at load time
+
+
+def _qkv_planes(qkv, C):
+    """the encoder's qkv operand: q columns times WATTN_QSCALE in fp32, then split -> (hi, lo) int16 planes, each
+    followed by a guard"""
+    x = qkv.clone()
+    x[:, :C] *= torch.tensor(WATTN_QSCALE, dtype=torch.float32, device=x.device)
+    h = x.to(torch.bfloat16)
+    planes = []
+    for p in (h, (x - h.float()).to(torch.bfloat16)):
+        buf, _ = _guarded(x.numel(), torch.int16, -1)
+        buf.copy_(p.view(torch.int16).flatten())
+        planes.append(buf)
+    return planes
+
+
+def _run_wattn_planes(ctx, planes, tab, B, nWh, nWw, heads, shift, f32=True):
+    rows, C = planes[0].numel() // (3 * heads * 32), heads * 32
+    n = rows * C
+    out, ofull = _guarded(n)
+    (hi, hfull), (lo, lfull) = _planes(n)
+    ctx.check(_op(ctx, 'alm_op_window_attention_planes', planes[0].data_ptr(), planes[1].data_ptr(), tab.data_ptr(),
+                  out.data_ptr() if f32 else None, hi.data_ptr(), lo.data_ptr(), B, nWh, nWw, C, heads, shift))
+    for full, fill in ((ofull, NAN), (hfull, -1), (lfull, -1)):
+        _assert_guard(full, n, fill)
+    if not f32:
+        assert bool(torch.isnan(out).all()), 'fp32 output written without one'
+    return out.view(rows, C), hi, lo
+
+
 def _check_wattn(ctx, B, nWh, nWw, heads, shift, seed):
+    """alm_op_window_attention_ex on fp32 qkv, and alm_op_window_attention_planes on the planes of the pre-scaled
+    q (against fp64 of the planes' own values hi + lo, no further scaling), under every wattn_impl"""
     from tests.test_gpu_omniparser import window_attention_ref64
     qkv, tab = _wattn_inputs(B, nWh, nWw, heads, shift, seed)
     ref = window_attention_ref64(qkv, tab, B, nWh, nWw, heads, shift)
     tol = _wattn_tol(qkv, heads, B, nWh, nWw)
+    planes = _qkv_planes(qkv, heads * 32)
+    joined = _joined(*planes).view(qkv.shape)
+    ref_p = window_attention_ref64(joined, tab, B, nWh, nWw, heads, shift, scale=1.0)
+    tol_p = _wattn_tol(joined, heads, B, nWh, nWw, scale=1.0)
     for impl in (0, 1, 3):
         with options(ctx, wattn_impl=impl):
             out, hi, lo = _run_wattn(ctx, qkv, tab, B, nWh, nWw, heads, shift)
@@ -611,6 +658,13 @@ def _check_wattn(ctx, B, nWh, nWw, heads, shift, seed):
             _assert_split(hi, lo, out.flatten(), f'impl {impl}')
             _, hi2, lo2 = _run_wattn(ctx, qkv, tab, B, nWh, nWw, heads, shift, f32=False)   # the encoder's form
             assert torch.equal(hi2, hi) and torch.equal(lo2, lo), impl
+            out, hi, lo = _run_wattn_planes(ctx, planes, tab, B, nWh, nWw, heads, shift)
+            assert torch.isfinite(out).all(), ('planes', impl)
+            err = (out.double() - ref_p).abs()
+            assert bool((err <= tol_p).all()), ('planes', impl, float((err / tol_p).max()), float(err.max()))
+            _assert_split(hi, lo, out.flatten(), f'planes, impl {impl}')
+            _, hi2, lo2 = _run_wattn_planes(ctx, planes, tab, B, nWh, nWw, heads, shift, f32=False)
+            assert torch.equal(hi2, hi) and torch.equal(lo2, lo), ('planes', impl)
 
 
 @pytest.mark.parametrize('name', list(WATTN_EX_CASES))
@@ -711,6 +765,27 @@ def test_argument_errors_leave_the_context_usable(ctx):
     assert wattn(out=None) == ERR_INVALID                     # no output at all
     assert wattn(C=100) == ERR_UNSUPPORTED                    # head_dim 32 only
     assert _op(ctx, 'alm_op_window_attention', P(d), P(tab), None, 1, 1, 1, 128, 4, 3) == ERR_INVALID
+
+    (qh, _), (ql, _) = _planes(49 * 3 * 128)
+    (oh, _), (ol, _) = _planes(49 * 128)
+    out = torch.full((49 * 128,), NAN, device='cuda')
+
+    def planes(qkv_hi=qh, qkv_lo=ql, t=tab, f32=out, hi_=oh, lo_=ol, B=1, nWh=1, nWw=1, C=128, heads=4, shift=3):
+        return _op(ctx, 'alm_op_window_attention_planes', P(qkv_hi), P(qkv_lo), P(t), P(f32), P(hi_), P(lo_), B, nWh,
+                   nWw, C, heads, shift)
+    for kw in (dict(qkv_hi=None), dict(qkv_lo=None), dict(t=None), dict(f32=None, hi_=None, lo_=None),
+               dict(hi_=None),                                          # out_lo needs out_hi
+               dict(qkv_hi=torch.zeros(49 * 3 * 128, dtype=torch.int16)), dict(t=hst), dict(f32=hst),
+               dict(qkv_hi=qh[1:]), dict(qkv_lo=ql[4:]), dict(f32=out[1:]), dict(hi_=oh[1:]),   # misaligned
+               dict(B=0), dict(nWh=0), dict(nWw=-1), dict(heads=0), dict(shift=-1), dict(shift=7)):
+        assert planes(**kw) == ERR_INVALID, kw
+    assert planes(C=100) == ERR_UNSUPPORTED                   # head_dim 32 only
+    assert planes(C=256) == ERR_UNSUPPORTED
+    assert bool(torch.isnan(out).all()) and bool((oh == -1).all()) and bool((ol == -1).all()), 'written before an error'
+    qh.zero_()
+    ql.zero_()
+    assert planes() == 0
+    assert bool((out == 0).all())
 
     # the context still computes
     _check_maps(ctx, 2, 11, 5)

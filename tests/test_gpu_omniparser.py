@@ -95,14 +95,15 @@ def test_layernorm(ctx, C):
         assert float((y[:rows * C].view(rows, C).cpu().double() - ref).abs().max()) < 1e-5, rows
 
 
-def window_attention_ref64(qkv, tab, B, nWh, nWw, heads, shift):
+def window_attention_ref64(qkv, tab, B, nWh, nWw, heads, shift, scale=32 ** -0.5):
     """swin_transformer.py:127-148 without the projections, in fp64 on qkv's device: scale-then-dot, relative-position
-    bias, -100 shift mask, softmax, PV.  qkv [B*nWh*nWw*49, 3C] window-major, tab [169, heads] -> [rows, C]."""
+    bias, -100 shift mask, softmax, PV.  qkv [B*nWh*nWw*49, 3C] window-major, tab [169, heads] -> [rows, C].  scale 1:
+    q already scaled (the encoder's qkv planes)."""
     from oracle import omniparser_ref as O
     from oracle.weights import relative_position_index
     rows = qkv.shape[0]
     q, k, v = qkv.double().view(-1, 49, 3, heads, 32).permute(2, 0, 3, 1, 4)
-    attn = (q * 32 ** -0.5) @ k.transpose(-2, -1)
+    attn = (q * scale) @ k.transpose(-2, -1)
     idx = relative_position_index().view(-1).to(qkv.device)
     attn = attn + tab.double()[idx].view(49, 49, -1).permute(2, 0, 1).unsqueeze(0)
     if shift:
