@@ -228,6 +228,10 @@ SIGNATURES = {
     'alm_pre_omni_tiles_turned': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                             C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                             C.c_void_p]),
+    # alm_pre_omni_tiles_at's arguments with turns after n_pages
+    'alm_pre_omni_tiles_at_turned': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                               C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                               C.c_void_p]),
     # alm_omni_merge_tiles' arguments with turns after n_pages
     'alm_omni_merge_tiles_turned': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                               C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -269,6 +273,11 @@ SIGNATURES = {
     'alm_omni_char_boxes': (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
+    # ctx, n_regions, n_cand, frame_index, n_frames, frames, pt, poly, rec, rec_prob, rec_length, num_bins,
+    # recog_pad_index, rec_eos_index, kept, scores, pts, polys
+    'alm_omni_select_regions': (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     # ctx, n_pages, page_count, page_offset, polys, cos_tol, height_ratio, max_offset, max_overlap, max_gap, n_lines,
     # line_offset, line_first, line_words, order, line_of, rank_of, line_polys, cap
     'alm_omni_group_lines': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double,

@@ -12,6 +12,7 @@
 #include "omni.h"
 #include "pre.h"
 #include "ptx.cuh"
+#include "region_turn_core.h"
 
 using namespace alm;
 
@@ -855,6 +856,13 @@ int alm_pre_omni_tiles_turned(alm_ctx* h, const uint8_t* const* rgb, const int* 
                     idx.data(), static_cast<int>(idx.size()), test_min_size, test_max_size, tensors, mask);
 }
 
+int alm_pre_omni_tiles_at_turned(alm_ctx* h, const uint8_t* const* rgb, const int* heights, const int* widths,
+                                 int n_pages, const int32_t* turns, int tile, int overlap, const int32_t* index,
+                                 int count, int test_min_size, int test_max_size, float* tensors, uint8_t* mask) {
+  return omni_tiles(h, "alm_pre_omni_tiles_at_turned", rgb, heights, widths, n_pages, true, turns, tile, overlap, index,
+                    count, test_min_size, test_max_size, tensors, mask);
+}
+
 namespace {
 
 // The tiles of a tile merge's plan (alm_omni_merge_tiles, _turned, alm_omni_merge_kie_tiles), once the page sizes, the
@@ -1076,6 +1084,39 @@ int alm_omni_char_boxes(alm_ctx* h, long n_words, int rec_length, const double* 
                   std::string(fn) + ": word " + std::to_string(n) + ": frame index out of range");
     char_boxes(&h->c, n_words, rec_length, n_frames, fr.data(), frame_index, polys, rec, loc, recog_pad_index,
                rec_eos_index, n_chars, step, centre, cov, box);
+  });
+}
+
+int alm_omni_select_regions(alm_ctx* h, long n_regions, int n_cand, const int32_t* frame_index, int n_frames,
+                            const int32_t* frames, const int64_t* pt, const int64_t* poly, const int64_t* rec,
+                            const float* rec_prob, int rec_length, int num_bins, int recog_pad_index, int rec_eos_index,
+                            int32_t* kept, double* scores, double* pts, double* polys) {
+  return guarded(h, [&] {
+    const char* fn = "alm_omni_select_regions";
+    ALM_REQUIRE(n_regions >= 0 && n_cand >= 1 && n_cand <= region_turn_core::kMaxCandidates, ALM_ERR_INVALID,
+                std::string(fn) + ": n_regions must be >= 0 and n_cand in 1.." +
+                    std::to_string(region_turn_core::kMaxCandidates));
+    ALM_REQUIRE(rec_length >= 1 && rec_length <= rec_box_core::kMaxSteps && num_bins >= 1, ALM_ERR_INVALID,
+                std::string(fn) + ": rec_length must be in 1.." + std::to_string(rec_box_core::kMaxSteps) +
+                    " and num_bins >= 1");
+    if (n_regions == 0) return;
+    ALM_REQUIRE(frame_index && frames && pt && poly && rec && rec_prob && kept && scores && pts && polys,
+                ALM_ERR_INVALID, std::string(fn) + ": null argument");
+    ALM_REQUIRE(n_frames >= 1, ALM_ERR_INVALID, std::string(fn) + ": regions need at least one frame");
+    std::vector<rec_box_core::Frame> fr(static_cast<size_t>(n_frames));
+    for (int k = 0; k < n_frames; ++k) {
+      const int32_t* v = frames + 7L * k;
+      fr[static_cast<size_t>(k)] = rec_box_core::Frame{v[0], v[1], v[2], v[3], v[4], v[5], v[6]};
+      ALM_REQUIRE(rec_box_core::valid_frame(fr[static_cast<size_t>(k)]), ALM_ERR_INVALID,
+                  std::string(fn) + ": frame " + std::to_string(k) +
+                      ": need positive sizes, a turn in 0..3 and the tile inside its turned page");
+    }
+    for (long g = 0; g < n_regions * n_cand; ++g)
+      ALM_REQUIRE(frame_index[g] >= 0 && frame_index[g] < n_frames, ALM_ERR_INVALID,
+                  std::string(fn) + ": region " + std::to_string(g / n_cand) + ", candidate " +
+                      std::to_string(g % n_cand) + ": frame index out of range");
+    region_select(&h->c, n_regions, n_cand, rec_length, n_frames, fr.data(), frame_index, pt, poly, rec, rec_prob,
+                  num_bins, recog_pad_index, rec_eos_index, kept, scores, pts, polys);
   });
 }
 

@@ -1,16 +1,23 @@
-// Pages read turned by quarter-turns (DESIGN 4.14; rules: tile_core.h, fuse_core.h).
+// Pages and regions read turned by quarter-turns (DESIGN 4.14, 4.21; rules: tile_core.h, fuse_core.h,
+// region_turn_core.h).
 //   tile_gather_kernel     every tile of a chunk cut from its (turned) page into one [h][w][3] buffer per tile, one
 //                          launch for all tiles: grid (column blocks, tiles), each block strides over its tile's pixels
 //   orient_select_kernel   one block of four warps per page, warp k scores the page's reading at turn k: the lanes
 //                          compute 32 instances' scores at a time, and every lane adds them up in instance order from
 //                          shuffles, so the sum is the sequential one; thread 0 then picks the turn
-// Only the chosen turns and the P x 4 scores of the selection cross PCIe back.
+//   region_select_kernel   caller-given regions read at quarter-turns (DESIGN 4.21; rule: region_turn_core.h): one
+//                          warp per region, its C candidate readings scored in turn, the lanes splitting the L steps
+//                          (a ballot finds the first stop, a second numbers the kept steps, and their probabilities are
+//                          added in step order from shuffles, so the sum is the sequential one); lanes 0..16 then map
+//                          one of the kept reading's 17 points each.  One launch for all regions of all pages.
+// Only the chosen turns and scores, and the kept rows' kept index, scores and mapped points, cross PCIe back.
 #include <algorithm>
 #include <vector>
 
 #include "alm_internal.h"
 #include "fuse_core.h"
 #include "pre.h"
+#include "region_turn_core.h"
 #include "tile_core.h"
 
 namespace alm {
@@ -60,6 +67,53 @@ orient_select_kernel(int max_inst, int L, const int* __restrict__ n_inst, const 
   }
 }
 
+// regions per block of region_select_kernel: one warp each
+constexpr int kSelectWarps = 4;
+
+__global__ void __launch_bounds__(32 * kSelectWarps)
+region_select_kernel(long R, int C, int L, int num_bins, int64_t pad, int64_t eos,
+                     const rec_box_core::Frame* __restrict__ frames, const int* __restrict__ frame_index,
+                     const int64_t* __restrict__ pt, const int64_t* __restrict__ poly, const int64_t* __restrict__ rec,
+                     const float* __restrict__ prob, int* __restrict__ kept, double* __restrict__ scores,
+                     double* __restrict__ pts, double* __restrict__ polys) {
+  const int lane = threadIdx.x & 31;
+  const long r = static_cast<long>(blockIdx.x) * kSelectWarps + (threadIdx.x >> 5);
+  if (r >= R) return;  // uniform over the warp
+  int best = 0, kb = 0;  // the candidate kept so far (region_turn_core::pick, one candidate at a time)
+  double sb = 0.0;
+  for (int c = 0; c < C; ++c) {
+    const long row = (r * C + c) * L;
+    double acc = 0.0;
+    int n = 0;
+    for (int j0 = 0; j0 < L; j0 += 32) {
+      const int j = j0 + lane;
+      const int kind = j < L ? rec_box_core::step_kind(rec[row + j], pad, eos) : rec_box_core::kStop;
+      const unsigned stops = __ballot_sync(0xffffffffu, kind == rec_box_core::kStop);
+      const unsigned before = stops ? (1u << (__ffs(stops) - 1)) - 1u : 0xffffffffu;  // lanes before the first stop
+      const bool kp = (before >> lane & 1u) && kind == rec_box_core::kKeep;
+      const unsigned km = __ballot_sync(0xffffffffu, kp);
+      const double v = kp ? static_cast<double>(prob[row + j]) : 0.0;
+      for (unsigned m = km; m; m &= m - 1u) acc = __dadd_rn(acc, __shfl_sync(0xffffffffu, v, __ffs(m) - 1));
+      n += __popc(km);
+      if (stops) break;  // uniform over the warp
+    }
+    const double s = __ddiv_rn(acc, __dadd_rn(static_cast<double>(n), 1e-5));
+    const int k = frames[frame_index[r * C + c]].turn;
+    if (c == 0 || region_turn_core::ranks_above(s, k, sb, kb)) {
+      best = c;
+      kb = k;
+      sb = s;
+    }
+    if (lane == 0) scores[r * C + c] = s;
+  }
+  if (lane == 0) kept[r] = best;
+  if (lane < 17) {
+    const long g = r * C + best;
+    double* out = lane == 0 ? pts + 2 * r : polys + 32 * r + 2 * (lane - 1);
+    region_turn_core::map_row_point(frames[frame_index[g]], pt + 2 * g, poly + 32 * g, lane, num_bins, out);
+  }
+}
+
 }  // namespace
 
 void tile_gather(Ctx* c, const std::vector<PreImage>& pages, const std::vector<tile_core::Tile>& tiles,
@@ -100,6 +154,33 @@ void orient_select(Ctx* c, int n_pages, int max_inst, int L, int64_t pad, int64_
   count_launch(c); check_launch("orient_select");
   st.down(turns_out, d_turns, n_pages);
   st.down(scores, d_scores, R);
+  st.sync();
+}
+
+void region_select(Ctx* c, long R, int C, int L, int F, const rec_box_core::Frame* frames, const int* frame_index,
+                   const int64_t* pt, const int64_t* poly, const int64_t* rec, const float* prob, int num_bins,
+                   int64_t pad, int64_t eos, int* kept, double* scores, double* pts, double* polys) {
+  if (R == 0) return;
+  const size_t RC = static_cast<size_t>(R) * C;
+  Staging st(c);
+  const rec_box_core::Frame* d_frames = st.up(frames, F);
+  const int* d_fi = st.up(frame_index, RC);
+  const int64_t* d_pt = st.up(pt, RC * 2);
+  const int64_t* d_poly = st.up(poly, RC * 32);
+  const int64_t* d_rec = st.up(rec, RC * L);
+  const float* d_prob = st.up(prob, RC * L);
+  int* o_kept = st.out<int>(R);
+  double* o_scores = st.out<double>(RC);
+  double* o_pts = st.out<double>(R * 2);
+  double* o_polys = st.out<double>(R * 32);
+  region_select_kernel<<<static_cast<unsigned>((R + kSelectWarps - 1) / kSelectWarps), 32 * kSelectWarps, 0,
+                         c->stream>>>(R, C, L, num_bins, pad, eos, d_frames, d_fi, d_pt, d_poly, d_rec, d_prob, o_kept,
+                                      o_scores, o_pts, o_polys);
+  count_launch(c); check_launch("region_select");
+  st.down(kept, o_kept, R);
+  st.down(scores, o_scores, RC);
+  st.down(pts, o_pts, R * 2);
+  st.down(polys, o_polys, R * 32);
   st.sync();
 }
 

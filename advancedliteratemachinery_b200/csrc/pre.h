@@ -135,6 +135,13 @@ void tile_gather(Ctx* c, const std::vector<PreImage>& pages, const std::vector<t
                  const std::vector<int>& idx, std::vector<PreImage>* imgs);
 void orient_select(Ctx* c, int n_pages, int max_inst, int L, int64_t pad, int64_t eos, const int* n_inst,
                    const int64_t* rec, const float* prob, int* turns_out, double* scores);
+// Caller-given regions read at quarter-turns (page_turn.cu; rule: region_turn_core.h, DESIGN 4.21).  Host inputs: R
+// regions of C candidate readings, frame_index [R][C] into frames [F] (checked by the caller), read_at's pt [R][C][2],
+// poly [R][C][32], rec / prob [R][C][L].  Host outputs: kept [R], scores [R][C], the kept reading's pts [R][2] and polys
+// [R][32] in upright page pixels.  One launch; none when R = 0.
+void region_select(Ctx* c, long R, int C, int L, int F, const rec_box_core::Frame* frames, const int* frame_index,
+                   const int64_t* pt, const int64_t* poly, const int64_t* rec, const float* prob, int num_bins,
+                   int64_t pad, int64_t eos, int* kept, double* scores, double* pts, double* polys);
 
 // A page's nr readings merged into one set of words (tile_merge.cu; rule: turn_core.h): its four turned readings
 // (nr = 4, DESIGN 4.15) or a dense page's window readings (DESIGN 4.16).  Host inputs in the layout

@@ -601,6 +601,96 @@ def tile_to_page(origin, size, ids, num_bins: int) -> np.ndarray:
     return np.array([origin[1], origin[0]], dtype=np.float64) + v.astype(np.float64)
 
 
+def turn_points(points, hw, turns) -> np.ndarray:
+    """Points (x, y) f64 [N, 2] in pixels of upright pages of size hw [N, 2] = (h, w) -> the same points on
+    ``np.rot90(page, turns[n])``, pixel-edge coordinates: k = 1: (y, W - x), k = 2: (W - x, H - y), k = 3: (H - y, x).
+    The inverse of ``tile_core::map_back`` (exactly, on integer inputs)."""
+    p = np.asarray(points, dtype=np.float64).reshape(-1, 2)
+    hw = np.asarray(hw, dtype=np.float64).reshape(-1, 2)
+    k = np.asarray(turns).reshape(-1)
+    x, y, H, W = p[:, 0], p[:, 1], hw[:, 0], hw[:, 1]
+    u = np.select([k == 1, k == 2, k == 3], [y, W - x, H - y], x)
+    v = np.select([k == 1, k == 2, k == 3], [W - x, H - y, x], y)
+    return np.stack([u, v], axis=1)
+
+
+def turn_boxes(boxes, hw, turns) -> np.ndarray:
+    """Boxes (x0, y0, x1, y1) f64 [N, 4] of upright pages of size hw [N, 2] -> the boxes of their corners turned by
+    ``turn_points``: what ``route_regions`` places in the tiles of the turned page."""
+    b = np.asarray(boxes, dtype=np.float64).reshape(-1, 4)
+    a, c = turn_points(b[:, :2], hw, turns), turn_points(b[:, 2:], hw, turns)
+    return np.concatenate([np.minimum(a, c), np.maximum(a, c)], axis=1)
+
+
+def region_turn_candidates(sizes, regions, page_index, kind: str) -> np.ndarray:
+    """The two turns ``read_regions(orientation='auto')`` reads each region at, int32 [R, 2] (rule: DESIGN 4.21): 1 and
+    3 for a tall region (2 h >= 3 w, MGP-STR's rule), else 0 and 2.  h and w: the crop size ``preprocess.quad_plan`` /
+    ``curve_plan`` give a 'quad' / 'polygon' on its page, a 'box''s own size; a 'point' is never tall."""
+    from . import preprocess as Pre
+    pi = np.asarray(page_index).reshape(-1)
+    if kind == 'point':
+        tall = np.zeros(len(pi), bool)
+    elif kind == 'box':
+        b = region_boxes(regions, kind)
+        tall = 2 * (b[:, 3] - b[:, 1]) >= 3 * (b[:, 2] - b[:, 0])
+    else:
+        plan = Pre.quad_plan if kind == 'quad' else Pre.curve_plan
+        cs = plan(sizes, regions, pi)['sizes'].astype(np.int64)  # (width, height)
+        tall = 2 * cs[:, 1] >= 3 * cs[:, 0]
+    return np.stack([np.where(tall, 1, 0), np.where(tall, 3, 2)], axis=1).astype(np.int32)
+
+
+def plan_region_turns(sizes, boxes, page_index, turns, tile: int = 1200, overlap: int = 256) -> dict:
+    """Where ``read_regions`` reads each region at each of its candidate turns (rule: DESIGN 4.21).  sizes: the upright
+    (h, w) of every page; boxes f64 [R, 4] in page pixels (``region_boxes``); turns int [R, C].  A reading is a distinct
+    (page, turn) pair that holds a region, and is a page of its own: np.rot90(page, turn), tiled by
+    ``preprocess.omni_tile_plan``.  Candidate (r, c) is routed by ``route_regions`` on its reading with the box's
+    corners turned (``turn_boxes``).
+    Returns dict(readings int32 [n, 2] = (page, turn) in (page, turn) order, reading int64 [R, C] (the candidate's
+    reading), plan int32 [tiles, 5] (the readings' plan, 'page' = reading), route int64 [R, C] (an index into plan, or
+    -1 for the reading read whole))."""
+    from . import preprocess as Pre
+    pi = np.asarray(page_index, dtype=np.int64).reshape(-1)
+    t = np.asarray(turns, dtype=np.int64).reshape(len(pi), -1)
+    R, C = t.shape
+    uniq, inv = np.unique(pi[:, None] * 4 + t, return_inverse=True)
+    readings = np.stack([uniq // 4, uniq % 4], axis=1).astype(np.int32).reshape(-1, 2)
+    reading = inv.reshape(R, C).astype(np.int64)
+    read = Pre.turned_sizes([sizes[p] for p in readings[:, 0]], readings[:, 1])
+    plan = Pre.omni_tile_plan(read, tile, overlap)
+    hw = np.asarray(sizes, dtype=np.float64).reshape(-1, 2)[np.repeat(pi, C)]
+    tb = turn_boxes(np.repeat(np.asarray(boxes, dtype=np.float64).reshape(-1, 4), C, axis=0), hw, t.reshape(-1))
+    route = route_regions(read, plan, tb, reading.reshape(-1)).reshape(R, C)
+    return dict(readings=readings, reading=reading, plan=plan, route=route)
+
+
+def select_regions(ctx: _lib.Context, frames, frame_index, pt, poly, rec, prob, num_bins: int, recog_pad_index: int,
+                   rec_eos_index: int) -> dict:
+    """Of every region's C (1..4) candidate readings the one kept, and its point and polygon in upright page pixels, on
+    the device (``alm_omni_select_regions``; rule: DESIGN 4.21).  frames int [F, 7] = (H, W, turn, y0, x0, h, w)
+    (``alm_omni_char_boxes``' frames), frame_index int [R, C]; candidate (r, c)'s ``read_at`` outputs in bins of its
+    frame: pt int64 [R, C, 2], poly [R, C, 32], rec [R, C, L], prob f32 [R, C, L].  A candidate scores
+    ``decode_pred_seq``'s 'score'; the larger score is kept, the lower turn on a tie, and a NaN score never ranks above
+    another.
+    Returns dict(kept int32 [R] (the candidate), scores f64 [R, C], pts f64 [R, 2], polys f64 [R, 32])."""
+    fi = np.ascontiguousarray(frame_index, dtype=np.int32)
+    frames = np.ascontiguousarray(frames, dtype=np.int32).reshape(-1, 7)
+    pt, poly, rec = (np.ascontiguousarray(a, dtype=np.int64) for a in (pt, poly, rec))
+    prob = np.ascontiguousarray(prob, dtype=np.float32)
+    if fi.ndim != 2 or rec.ndim != 3:
+        raise ValueError(f'select_regions: frame_index must be [R, C] and rec [R, C, L], got {fi.shape}, {rec.shape}')
+    R, C = fi.shape
+    if pt.shape != (R, C, 2) or poly.shape != (R, C, 32) or rec.shape[:2] != (R, C) or prob.shape != rec.shape:
+        raise ValueError(f'select_regions: pt {pt.shape}, poly {poly.shape}, rec {rec.shape} and prob {prob.shape} '
+                         f'do not match frame_index {fi.shape}')
+    out = dict(kept=np.zeros(R, np.int32), scores=np.zeros((R, C)), pts=np.zeros((R, 2)), polys=np.zeros((R, 32)))
+    ctx.check(ctx.lib.alm_omni_select_regions(ctx.h, R, C, fi.ctypes.data, len(frames), frames.ctypes.data,
+                                              pt.ctypes.data, poly.ctypes.data, rec.ctypes.data, prob.ctypes.data,
+                                              rec.shape[2], int(num_bins), int(recog_pad_index), int(rec_eos_index),
+                                              *[out[k].ctypes.data for k in ('kept', 'scores', 'pts', 'polys')]))
+    return out
+
+
 class OmniParserB200:
     """Inference-only stand-in for the reference ``OmniParser`` module (``--tfm_pre_norm --use_fpn``)."""
 
@@ -1203,7 +1293,8 @@ class OmniParserB200:
 
     def read_regions(self, pages, regions, page_index, kind: str = 'quad', tile: int = 1200, overlap: int = 256,
                      max_batch: int = 16, test_min_size: int = 1200, test_max_size: int = 1920, rec_candidates: int = 0,
-                     rec_beams: int = 0, length_penalty: float = 1.0, rec_locations: bool = False) -> List[dict]:
+                     rec_beams: int = 0, length_penalty: float = 1.0, rec_locations: bool = False,
+                     orientation='upright') -> List[dict]:
         """Read caller-given regions of raw pages of any size (rule: DESIGN 4.19): OmniParser as the recogniser of
         another detector's regions, each word read in place on the page and returned with its 16-point polygon.
         pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch); regions of one kind, in page
@@ -1226,8 +1317,17 @@ class OmniParserB200:
         ``read_at`` also keeps the character locations, ``last_rec_locations`` [R, rec_length, 5] in region order (each
         in its tile's or page's frame), and one ``char_boxes`` call gives each region 'chars', ``postprocess.
         rec_char_boxes``' list (char, centre, cov, box) in page pixels.
-        Not offered: orientation, KIE checkpoints, and any merge or dedupe of overlapping regions -- each region is read
-        as given."""
+        orientation (rule: DESIGN 4.21): 'upright' reads every region as the page lies.  int [R] in 0..3 reads region r
+        on ``np.rot90(page, turns[r])`` (counter-clockwise quarter-turns), in the tiles of the turned page's plan: its
+        point and box are turned into that frame (``turn_points``, ``turn_boxes``) and routed there, and its reading is
+        mapped back to the page.  'auto' reads every region at two turns (``region_turn_candidates``: 1 and 3 for a tall
+        region, else 0 and 2) and keeps, on the device, the reading with the larger 'score', the lower turn on a tie
+        (``select_regions``).  Each distinct (page, turn) reading is cut and encoded as a page of its own (only its tiles
+        and whole readings that hold a region).  The dicts gain 'turns', the turn kept, with 'tile' in that reading's
+        plan; candidates, beams and 'chars' follow the kept reading.  ``last_regions`` gains 'readings' ((page, turn)
+        pairs), 'reading', 'route' and the readings' 'rec' / 'prob' per (region, candidate), 'turns' [R], 'frames' /
+        'frame_index' (the frames of ``select_regions``), and for 'auto' 'candidates' [R, 2] and 'scores' f64 [R, 2].
+        Not offered: KIE checkpoints, and any merge or dedupe of overlapping regions -- each region is read as given."""
         from . import postprocess
         from . import preprocess as Pre
         v = self.vocab
@@ -1235,6 +1335,10 @@ class OmniParserB200:
             raise ValueError('read_regions reads text spotting checkpoints; this one is a KIE checkpoint')
         if int(max_batch) < 1:
             raise ValueError(f'max_batch must be >= 1, got {max_batch}')
+        if not (isinstance(orientation, str) and orientation == 'upright'):
+            return self._read_regions_turned(pages, regions, page_index, kind, tile, overlap, max_batch, test_min_size,
+                                             test_max_size, rec_candidates, rec_beams, length_penalty, rec_locations,
+                                             orientation)
         dev = torch.device('cuda', self.ctx.device)
         pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
         sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
@@ -1317,6 +1421,120 @@ class OmniParserB200:
                  'rec': texts[r], 'page': int(pi[r]),
                  'tile': int(route[r] - first_tile[pi[r]]) if route[r] >= 0 else -1,
                  **({} if chars is None else {'chars': chars[r]})} for r in range(R)]
+
+    def _read_regions_turned(self, pages, regions, page_index, kind, tile, overlap, max_batch, test_min_size,
+                             test_max_size, rec_candidates, rec_beams, length_penalty, rec_locations, orientation):
+        """read_regions with orientation other than 'upright' (rule: DESIGN 4.21): every argument checked before any
+        device work, each candidate reading read at its turned point in its reading's tile (or the reading read
+        whole), then one ``select_regions`` and, with rec_locations, one ``char_boxes`` call."""
+        from . import postprocess
+        from . import preprocess as Pre
+        v = self.vocab
+        nb, L = v.num_bins, v.rec_length
+        sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
+        centres = postprocess.region_points(regions, kind)
+        R = len(centres)
+        pi = np.asarray(page_index).reshape(-1)
+        if len(pi) != R or (R and (pi.dtype.kind not in 'iu' or pi.min() < 0 or pi.max() >= len(pages))):
+            raise ValueError(f'page_index must be {R} integers in 0 .. {len(pages) - 1}')
+        pi = pi.astype(np.int64)
+        for r in range(R):   # every point on its page (ValueError otherwise)
+            postprocess.point_bins(centres[r], sizes[pi[r]], nb)
+        auto = isinstance(orientation, str)
+        if auto:
+            if orientation != 'auto':
+                raise ValueError(f"orientation must be 'upright', 'auto' or one turn per region, got {orientation!r}")
+            cand = region_turn_candidates(sizes, regions, pi, kind)
+        else:
+            cand = Pre.check_turns(orientation, R).reshape(R, 1)
+        K, W = int(rec_candidates), int(rec_beams)
+        self._set_rec_candidates(K, W, length_penalty, rec_locations)   # refused before device work
+        C = cand.shape[1]
+        rp = plan_region_turns(sizes, region_boxes(regions, kind), pi, cand, tile, overlap)
+        readings, plan = rp['readings'], rp['plan']
+        route, reading = rp['route'].reshape(-1), rp['reading'].reshape(-1)   # per candidate g = C r + c
+        rturns = np.ascontiguousarray(readings[:, 1])
+        rsizes = [sizes[p] for p in readings[:, 0]]
+        tsizes = Pre.turned_sizes(rsizes, rturns)
+        tpts = turn_points(np.repeat(centres, C, axis=0), np.asarray(rsizes, np.float64).reshape(-1, 2)[reading],
+                           cand.reshape(-1))
+        dev = torch.device('cuda', self.ctx.device)
+        pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
+        rpages = [pages[p] for p in readings[:, 0]]   # each page once on the device, listed once per reading
+        # the readings' tiles that hold a candidate, then the readings read whole, in chunks of their own kind
+        tiles = [('tile', int(t)) for t in np.unique(route[route >= 0])]
+        whole = [('whole', int(q)) for q in np.unique(reading[route < 0])]
+        mb, RC = int(max_batch), R * C
+        pt, poly = np.zeros((RC, 2), np.int64), np.zeros((RC, 32), np.int64)
+        rec, prob = np.zeros((RC, L), np.int64), np.zeros((RC, L), np.float32)
+        cands = (np.zeros((RC, L, K), np.int64), np.zeros((RC, L, K), np.float32)) if K > 0 else None
+        beams = (np.zeros((RC, W, L), np.int64), np.zeros((RC, W, L), np.float32), np.zeros((RC, W), np.float32)) \
+            if W > 0 else None
+        loc = np.zeros((RC, L, 5), np.float32) if rec_locations else None
+        chunks = []
+        T_whole = max([64] + [max(tsizes[q]) for _, q in whole])
+        for chunk in [tiles[i:i + mb] for i in range(0, len(tiles), mb)] + \
+                [whole[i:i + mb] for i in range(0, len(whole), mb)]:
+            frames, rows = [], []   # (y0, x0, h, w) of each image in its turned page, and its candidates
+            for what, i in chunk:
+                if what == 'tile':
+                    frames.append((int(plan[i, 1]), int(plan[i, 2]), int(plan[i, 3]), int(plan[i, 4])))
+                    rows.append(np.nonzero(route == i)[0])
+                else:
+                    frames.append((0, 0) + tsizes[i])
+                    rows.append(np.nonzero((route < 0) & (reading == i))[0])
+            idx = [i for _, i in chunk]
+            if chunk[0][0] == 'tile':
+                nt = Pre.omni_tiles_at(self.ctx, rpages, idx, tile, overlap, test_min_size, test_max_size,
+                                       turns=rturns)
+            else:
+                nt = Pre.omni_tiles(self.ctx, [rpages[i] for i in idx], T_whole, 0, test_min_size, test_max_size,
+                                    turns=rturns[idx])
+            resized, _ = Pre.omni_plan([f[2:] for f in frames], test_min_size, test_max_size)
+            if len(set(resized)) == 1:
+                self.encode(nt.tensors)
+            else:
+                self.encode_pages(nt.tensors, resized)
+            local = [postprocess.point_bins(tpts[r_] - np.array([f[1], f[0]]), f[2:], nb) for f, r_ in zip(frames, rows)]
+            n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty, rec_locations)
+            for j, r_ in enumerate(rows):
+                k = len(r_)
+                pt[r_], poly[r_], rec[r_], prob[r_] = xy[j, :k], pl[j, :k], rc[j, :k], pb[j, :k]
+                for mine, got in ((cands, self.last_rec_candidates), (beams, self.last_rec_beams)):
+                    if mine is not None:
+                        for a, b in zip(mine, got):
+                            a[r_] = b[j, :k]
+                if loc is not None:
+                    loc[r_] = self.last_rec_locations[j, :k]
+            chunks.append(dict(kind=chunk[0][0], index=np.array(idx), n=n, pt=xy, poly=pl, rec=rc, prob=pb))
+        # frames: the readings' tiles, then every reading read whole; (H, W, turn) of the reading's upright page
+        tl = np.concatenate([plan, [(q, 0, 0) + tsizes[q] for q in range(len(readings))]]).astype(np.int64).reshape(-1, 5)
+        hw = np.asarray(rsizes, np.int64).reshape(-1, 2)[tl[:, 0]]
+        frames = np.concatenate([hw, rturns[tl[:, 0], None], tl[:, 1:]], axis=1).astype(np.int32)
+        fidx = np.where(route >= 0, route, len(plan) + reading).reshape(R, C)
+        sel = select_regions(self.ctx, frames, fidx, pt.reshape(R, C, 2), poly.reshape(R, C, 32), rec.reshape(R, C, L),
+                             prob.reshape(R, C, L), nb, v.recog_pad_index, v.rec_eos_index)
+        g = np.arange(R) * C + sel['kept']   # each region's kept candidate
+        texts, scores = postprocess.rec_texts(rec[g], prob[g], v)
+        chars = None
+        if loc is not None:
+            boxes = char_boxes(self.ctx, rsizes, tl, sel['polys'], rec[g], loc[g], fidx.reshape(-1)[g],
+                               v.recog_pad_index, v.rec_eos_index, turns=rturns)
+            chars = char_dicts(boxes, rec[g], v)
+        turns = cand.reshape(-1)[g].astype(np.int32)
+        first_tile = np.searchsorted(plan[:, 0], np.arange(len(readings)))
+        self.last_rec_candidates = None if cands is None else tuple(a[g] for a in cands)
+        self.last_rec_beams = None if beams is None else tuple(a[g] for a in beams)
+        self.last_rec_locations = None if loc is None else loc[g]
+        self.last_regions = dict(plan=plan, route=rp['route'], points=centres, chunks=chunks, readings=readings,
+                                 reading=rp['reading'], turns=turns, frames=frames, frame_index=fidx,
+                                 rec=rec.reshape(R, C, L), prob=prob.reshape(R, C, L))
+        if auto:
+            self.last_regions.update(candidates=cand, scores=sel['scores'])
+        return [{'pts': [sel['pts'][r].tolist()], 'score': float(scores[r]),
+                 'polys': sel['polys'][r].reshape(16, 2).tolist(), 'rec': texts[r], 'page': int(pi[r]),
+                 'tile': int(route[g[r]] - first_tile[reading[g[r]]]) if route[g[r]] >= 0 else -1,
+                 'turns': int(turns[r]), **({} if chars is None else {'chars': chars[r]})} for r in range(R)]
 
     def kie_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                   band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200, test_max_size: int = 1920,

@@ -21,6 +21,7 @@
     omni_tiles(ctx, pages, tile, overlap, ...)       those tiles cut from the pages (optionally turned by quarter-turns)
                                                      + omni_pages' transform, on the device
     omni_tiles_at(ctx, pages, index, tile, overlap, ...)  the tiles of a list of plan indices, cut the same way
+                                                     (optionally of turned pages)
 
 `images`: decoded 8-bit RGB pages, each a uint8 array / tensor [h, w, 3] (host numpy / torch, or CUDA torch).
 """
@@ -351,12 +352,18 @@ def omni_tiles(ctx: _lib.Context, pages: List, tile: int = 1200, overlap: int = 
 
 
 def omni_tiles_at(ctx: _lib.Context, pages: List, index, tile: int = 1200, overlap: int = 256,
-                  test_min_size: int = 1200, test_max_size: int = 1920) -> NestedTensor:
+                  test_min_size: int = 1200, test_max_size: int = 1920, turns=None) -> NestedTensor:
     """The tiles index[0], index[1], ... of omni_tile_plan(sizes, tile, overlap) (any order, repeats allowed) cut from
     the pages and put through the validation transform, each as an image of its own: what omni_tiles gives for each
-    of those tiles, bit for bit (``alm_pre_omni_tiles_at``).  pages: uint8 [h, w, 3] each (host or CUDA)."""
+    of those tiles, bit for bit (``alm_pre_omni_tiles_at``).  pages: uint8 [h, w, 3] each (host or CUDA).  turns:
+    None, or int [P] in 0..3: the plan is that of the turned pages, as in omni_tiles
+    (``alm_pre_omni_tiles_at_turned``)."""
     keep, ptrs, hs, ws, n = _image_args(pages)
-    plan = omni_tile_plan(list(zip(hs.tolist(), ws.tolist())), tile, overlap)
+    sizes = list(zip(hs.tolist(), ws.tolist()))
+    if turns is not None:
+        turns = check_turns(turns, n)
+        sizes = turned_sizes(sizes, turns)
+    plan = omni_tile_plan(sizes, tile, overlap)
     idx = np.ascontiguousarray(np.asarray(index).reshape(-1), dtype=np.int32)
     if idx.size == 0 or ((idx < 0) | (idx >= len(plan))).any():
         raise ValueError(f'tile indices must be a non-empty list in 0 .. {len(plan) - 1}')
@@ -366,8 +373,14 @@ def omni_tiles_at(ctx: _lib.Context, pages: List, index, tile: int = 1200, overl
     tensors = torch.empty(len(idx), 3, Hc, Wc, dtype=torch.float32, device=dev)
     mask = torch.empty(len(idx), Hc, Wc, dtype=torch.uint8, device=dev)
     ctx.wait_torch(*keep)
-    ctx.check(ctx.lib.alm_pre_omni_tiles_at(ctx.h, ptrs, hs.ctypes.data, ws.ctypes.data, n, tile, overlap,
-                                            idx.ctypes.data, len(idx), test_min_size, test_max_size,
-                                            tensors.data_ptr(), mask.data_ptr()))
+    if turns is None:
+        ctx.check(ctx.lib.alm_pre_omni_tiles_at(ctx.h, ptrs, hs.ctypes.data, ws.ctypes.data, n, tile, overlap,
+                                                idx.ctypes.data, len(idx), test_min_size, test_max_size,
+                                                tensors.data_ptr(), mask.data_ptr()))
+    else:
+        ctx.check(ctx.lib.alm_pre_omni_tiles_at_turned(ctx.h, ptrs, hs.ctypes.data, ws.ctypes.data, n,
+                                                       turns.ctypes.data, tile, overlap, idx.ctypes.data, len(idx),
+                                                       test_min_size, test_max_size, tensors.data_ptr(),
+                                                       mask.data_ptr()))
     ctx.synchronize()
     return NestedTensor(tensors, mask.bool())

@@ -899,6 +899,14 @@ ALM_API int alm_omni_merge_tiles_turned(alm_ctx* ctx, const int* heights, const 
                                         int rec_length, int num_bins, double margin, double band, double iou,
                                         int* page_count, int* page_offset, double* pts, double* polys,
                                         int64_t* rec_out, float* prob_out, int32_t* source, long cap);
+/* Turned tiles by plan index (DESIGN 4.21): tiles index[0 .. count) of the plan of the pages turned by turns[p]
+ * (0..3; the plan alm_pre_omni_tiles_turned lays out, any order, repeats allowed), each cut as alm_pre_omni_tiles_turned
+ * cuts it, bit for bit; alm_pre_omni_tiles_at is this call with every turn 0.  A page listed twice at two turns is two
+ * pages of the plan.  ALM_ERR_INVALID for a null turns, a turn outside 0..3 and as alm_pre_omni_tiles_at. */
+ALM_API int alm_pre_omni_tiles_at_turned(alm_ctx* ctx, const uint8_t* const* rgb, const int* heights, const int* widths,
+                                         int n_pages, const int32_t* turns, int tile, int overlap, const int32_t* index,
+                                         int count, int test_min_size, int test_max_size, float* tensors,
+                                         uint8_t* mask);
 /* Page orientation from four probe readings per page (DESIGN 4.14).  Inputs, HOST buffers: the decodes of 4 n_pages
  * readings in the layout of alm_omni_decode, reading 4 p + k = page p read whole at turn k: n_inst int32 [4 n_pages],
  * rec int64 [4 n_pages][max_inst][rec_length], rec_prob f32 [..].  An instance scores decode_pred_seq's 'score' (stop
@@ -998,6 +1006,27 @@ ALM_API int alm_omni_char_boxes(alm_ctx* ctx, long n_words, int rec_length, cons
                                 const float* loc, const int32_t* frame_index, int n_frames, const int32_t* frames,
                                 int recog_pad_index, int rec_eos_index, int32_t* n_chars, int32_t* step,
                                 double* centre, double* cov, double* box);
+/* Caller-given regions read at quarter-turns: of each region's candidate readings the one kept, and its point and
+ * polygon in upright page pixels (DESIGN 4.21; the rule in full is in region_turn_core.h).  Inputs, HOST buffers:
+ * n_regions regions of n_cand (1..4) candidate readings each, candidate c of region r read by alm_omni_decode_at in
+ * the frame frames[frame_index[r][c]], frames int32 [n_frames][7] = (H, W, turn, y0, x0, h, w) as alm_omni_char_boxes
+ * takes them (one frames array serves both calls); pt int64 [n_regions][n_cand][2] and poly [..][32] in bins of that
+ * frame, rec [..][rec_length] and rec_prob f32 [..][rec_length].
+ *   score  decode_pred_seq's 'score' of each candidate's rec / rec_prob (as alm_omni_orient_select scores an instance);
+ *   keep   the candidate of the largest score, on equal scores the lower turn, then the lower index; a NaN score never
+ *          ranks above another and every other ranks above it;
+ *   map    the kept candidate's point and 16 vertices: y0 / x0 + f32(f32(id / num_bins) * h / w) in double, as
+ *          alm_omni_merge_tiles maps a tile's reading, then to the upright page as alm_omni_merge_tiles_turned maps a
+ *          turned row, vertex order kept.  Turn 0 with one candidate is the tile merge's mapping alone.
+ * Outputs, HOST: kept int32 [n_regions] (the candidate index), scores f64 [n_regions][n_cand], pts f64 [n_regions][2]
+ * and polys f64 [n_regions][32].  One kernel launch whatever n_regions is (one warp per region, no atomics:
+ * bit-reproducible), none for n_regions = 0.  ALM_ERR_INVALID, before any device work, for n_regions < 0, n_cand
+ * outside 1..4, rec_length outside 1..1021, num_bins < 1, a null buffer or n_frames < 1 (with n_regions > 0), a frame
+ * index out of range, a turn outside 0..3, a non-positive size or a tile outside its turned page. */
+ALM_API int alm_omni_select_regions(alm_ctx* ctx, long n_regions, int n_cand, const int32_t* frame_index, int n_frames,
+                                    const int32_t* frames, const int64_t* pt, const int64_t* poly, const int64_t* rec,
+                                    const float* rec_prob, int rec_length, int num_bins, int recog_pad_index,
+                                    int rec_eos_index, int32_t* kept, double* scores, double* pts, double* polys);
 /* KIE on pages larger than the model's input or turned by quarter-turns: the entities decoded from every tile merged
  * into page coordinates on the device (DESIGN 4.18; the rule in full is in kie_tile_core.h).  Page p of upright size
  * heights[p] x widths[p], read as np.rot90(page, turns[p]) (turns null = all upright), tiled with (tile, overlap) as
