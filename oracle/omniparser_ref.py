@@ -226,7 +226,7 @@ def _mha(query, key, value, sd, p, attn_mask=None, key_padding_mask=None, nhead=
     v = v.view(S, B * nhead, hd).transpose(0, 1)
     mask = attn_mask
     if key_padding_mask is not None:
-        kpm = torch.zeros(key_padding_mask.shape, dtype=torch.float32).masked_fill(key_padding_mask, float('-inf'))
+        kpm = torch.zeros(key_padding_mask.shape, dtype=q.dtype).masked_fill(key_padding_mask, float('-inf'))
         kpm = kpm.view(B, 1, 1, S).expand(-1, nhead, -1, -1).reshape(B * nhead, 1, S)
         mask = kpm if mask is None else mask + kpm
     q = q * (1.0 / math.sqrt(hd))
@@ -253,14 +253,15 @@ def decoder_layer_pre(tgt, memory, sd, p, tgt_mask, mem_kpm, pos, query_pos):  #
     return tgt + t2
 
 
-def causal_mask(sz):  # transformer.py:331-337
+def causal_mask(sz, dtype=torch.float32):  # transformer.py:331-337
     m = (torch.triu(torch.ones(sz, sz)) == 1).transpose(0, 1)
-    return m.float().masked_fill(m == 0, float('-inf')).masked_fill(m == 1, 0.0)
+    return m.to(dtype).masked_fill(m == 0, float('-inf')).masked_fill(m == 1, 0.0)
 
 
 def decode_logits(seq, memory, mem_kpm, pos, sd, kind):
     """Transformer.decode (transformer.py:74-100) for ONE image: seq int64 [Bs, t] ->
-    logits [Bs, t, V].  memory/pos [M,512], mem_kpm [M] bool; repeated per sequence like :88-96."""
+    logits [Bs, t, V].  memory/pos [M,512], mem_kpm [M] bool; repeated per sequence like :88-96.  Runs in the dtype of
+    memory and the state dict (float64 for the tests' high-precision reference)."""
     t = 'transformer.'
     Bs, T = seq.shape
     emb = sd[t + 'embedding.word_embeddings.weight'][seq]          # transformer.py:313
@@ -272,7 +273,7 @@ def decode_logits(seq, memory, mem_kpm, pos, sd, kind):
     mem = memory[:, None, :].repeat(1, Bs, 1)
     ps = pos[:, None, :].repeat(1, Bs, 1)
     kpm = mem_kpm[None, :].repeat(Bs, 1)
-    tm = causal_mask(T)
+    tm = causal_mask(T, x.dtype)
     for l in range(W.DEC_LAYERS):
         tgt = decoder_layer_pre(tgt, mem, sd, f'{t}{kind}_decoder.layers.{l}.', tm, kpm, ps, qpos)
     tgt = _ln(tgt, sd, f'{t}{kind}_decoder.norm')                  # shared final LN, :369-370
