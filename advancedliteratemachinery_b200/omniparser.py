@@ -171,6 +171,24 @@ def check_merge_args(margin, band, iou):
     return margin, band, iou
 
 
+def check_rec_args(k, beams, length_penalty, locations):
+    """The recognition options every decode accepts (ValueError otherwise), as (k, beams, length_penalty, locations):
+    rec_candidates k in 0..MAX_CANDIDATES, rec_beams in 0..MAX_BEAMS, length_penalty in [0, 2], beams with neither
+    candidates nor locations."""
+    k, beams, lp, locations = int(k), int(beams), float(length_penalty), bool(locations)
+    if not 0 <= k <= _lib.MAX_CANDIDATES:
+        raise ValueError(f'rec_candidates must be 0..{_lib.MAX_CANDIDATES}, got {k}')
+    if not 0 <= beams <= _lib.MAX_BEAMS:
+        raise ValueError(f'rec_beams must be 0..{_lib.MAX_BEAMS}, got {beams}')
+    if not 0.0 <= lp <= 2.0:
+        raise ValueError(f'length_penalty must be in [0, 2], got {lp}')
+    if k and beams:
+        raise ValueError('rec_candidates and rec_beams cannot be combined')
+    if locations and beams:
+        raise ValueError('rec_locations and rec_beams cannot be combined')
+    return k, beams, lp, locations
+
+
 def _size_arrays(sizes):
     """The heights and widths int32 [P] of pages given as (h, w) sizes."""
     hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
@@ -814,17 +832,7 @@ class OmniParserB200:
                               v.vie_categories, max_instances)
 
     def _set_rec_candidates(self, k: int, beams: int = 0, length_penalty: float = 1.0, locations: bool = False):
-        k, beams, lp, locations = int(k), int(beams), float(length_penalty), bool(locations)
-        if not 0 <= k <= _lib.MAX_CANDIDATES:
-            raise ValueError(f'rec_candidates must be 0..{_lib.MAX_CANDIDATES}, got {k}')
-        if not 0 <= beams <= _lib.MAX_BEAMS:
-            raise ValueError(f'rec_beams must be 0..{_lib.MAX_BEAMS}, got {beams}')
-        if not 0.0 <= lp <= 2.0:
-            raise ValueError(f'length_penalty must be in [0, 2], got {lp}')
-        if k and beams:
-            raise ValueError('rec_candidates and rec_beams cannot be combined')
-        if locations and beams:
-            raise ValueError('rec_locations and rec_beams cannot be combined')
+        k, beams, lp, locations = check_rec_args(k, beams, length_penalty, locations)
         # the library refuses beams together with candidates or locations: whichever is being turned off goes first
         if k == 0 and self._rec_k:
             self.ctx.check(self.lib.alm_omni_set_rec_candidates(self.ctx.h, 0))
@@ -1184,7 +1192,8 @@ class OmniParserB200:
     def spot_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                    band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200,
                    test_max_size: int = 1920, orientation='upright', whole_page: bool = False,
-                   rec_locations: bool = False) -> List[List[dict]]:
+                   rec_locations: bool = False, rec_candidates: int = 0, rec_beams: int = 0,
+                   length_penalty: float = 1.0) -> List[List[dict]]:
         """Text spotting of pages larger than the model's input, read in overlapping tiles (rule: DESIGN 4.11).
         pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch).  Every page is cut into the tiles
         of ``preprocess.omni_tile_plan(sizes, tile, overlap)``; each tile goes through the reference's validation
@@ -1225,7 +1234,18 @@ class OmniParserB200:
         one tile, to its probe reading; 'mixed': through the turn merge to its reading's tile) and one ``char_boxes``
         call for all pages gives each word 'chars', ``postprocess.rec_char_boxes``' list (char, centre, cov, box) in
         pixels of the page as passed in.  ``last_tiles`` gains 'loc', every tile's locations.  Not together with
-        whole_page: whole-page readings go through ``decode_dense``, which has no locations."""
+        whole_page: whole-page readings go through ``decode_dense``, which has no locations.
+        rec_candidates / rec_beams / length_penalty (rule: DESIGN 4.11): as in ``decode``; every tile decode, and
+        'auto''s probes, run with them, and each kept word is followed back to its tile instance as for rec_locations.
+        ``last_rec_candidates`` (ids int64, probs f32 [N, rec_length, k]) or ``last_rec_beams`` (ids, probs [N, W,
+        rec_length], scores [N, W]) hold the N returned words in result order (page by page, each page's words in
+        order), as ``read_regions`` holds its regions; ``last_tiles`` gains 'candidates' or 'beams', every tile
+        decode's arrays, indexed by (tile row, instance) like 'rec'.  Candidates leave every word as it is without
+        them, candidate 0 being its rec ids and probabilities.  Beams change only 'rec' / 'score', to hypothesis 0:
+        the point and polygon loops stay greedy and the tile merge decides on boxes and tile edges, so for 'upright'
+        and explicit turns the words, points, polygons, 'tile' and 'instance' are those without beams; 'auto' and
+        'mixed' choose on hypothesis 0's score.  Candidates combine with rec_locations; beams do not, and neither
+        combines with whole_page (``decode_dense`` offers neither).  Refusals come before any device work."""
         from . import postprocess
         from . import preprocess as Pre
         v = self.vocab
@@ -1235,6 +1255,10 @@ class OmniParserB200:
             raise ValueError(f'max_batch must be >= 1, got {max_batch}')
         if rec_locations and whole_page:
             raise ValueError('rec_locations cannot be combined with whole_page: whole-page readings have no locations')
+        K, W, lp, rec_locations = check_rec_args(rec_candidates, rec_beams, length_penalty, rec_locations)
+        if (K or W) and whole_page:
+            raise ValueError('rec_candidates and rec_beams cannot be combined with whole_page: whole-page readings '
+                             'have neither')
         auto = isinstance(orientation, str) and orientation == 'auto'
         if isinstance(orientation, str):
             if orientation not in ('upright', 'auto', 'mixed'):
@@ -1247,19 +1271,20 @@ class OmniParserB200:
         pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
         sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
+        decode = self._tile_decode(K, W, lp, rec_locations)
         if isinstance(orientation, str) and orientation == 'mixed':
             return self._spot_mixed(pages, sizes, tile, overlap, max_batch, margin, band, iou, test_min_size,
-                                    test_max_size, whole_page, rec_locations)
-        decode = self._decode_loc_arrays if rec_locations else self._decode_arrays
+                                    test_max_size, whole_page, rec_locations, decode)
         extra = {}
         if auto:
             Pre.omni_tile_plan(sizes, tile, overlap)  # a bad layout is refused before the probes run
             probe, turns, extra['page_scores'] = self._probe_turns(pages, sizes, max_batch, test_min_size, test_max_size,
                                                                    decode)
             extra['probe'] = probe
-        plan, (n_inst, pt, poly, rec, prob, *loc) = self._read_tiles(pages, sizes, turns, extra.get('probe'), tile,
-                                                                     overlap, max_batch, test_min_size, test_max_size,
-                                                                     decode)
+        plan, arrays = self._read_tiles(pages, sizes, turns, extra.get('probe'), tile, overlap, max_batch, test_min_size,
+                                        test_max_size, decode)
+        n_inst, pt, poly, rec, prob = arrays[:5]
+        loc, lists = arrays[5:5 + rec_locations], arrays[5 + rec_locations:]
         m = merge_tiles(self.ctx, sizes, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band, iou,
                         turns=turns)
         out, whole = m, None
@@ -1289,6 +1314,7 @@ class OmniParserB200:
             self.last_tiles.update(whole=whole, whole_merge=out)
         if turns is not None:
             self.last_tiles.update(turns=turns, **extra)
+        self._keep_tile_lists(lists, out['source'])
         return results
 
     def read_regions(self, pages, regions, page_index, kind: str = 'quad', tile: int = 1200, overlap: int = 256,
@@ -1668,10 +1694,10 @@ class OmniParserB200:
         return out
 
     def _spot_mixed(self, pages, sizes, tile, overlap, max_batch, margin, band, iou, test_min_size, test_max_size,
-                    whole_page=False, rec_locations=False):
-        """spot_tiled(orientation='mixed'): every page read in tiles at turns 0..3 (reading 4 p + k), one merge of the
-        4 P readings, with whole_page each reading merged with its whole-page partner (merge_whole_page), then one
-        merge of each page's four readings (merge_turns)."""
+                    whole_page, rec_locations, decode):
+        """spot_tiled(orientation='mixed'): every page read in tiles at turns 0..3 (reading 4 p + k) by decode
+        (``_tile_decode``), one merge of the 4 P readings, with whole_page each reading merged with its whole-page
+        partner (merge_whole_page), then one merge of each page's four readings (merge_turns)."""
         from . import postprocess
         from . import preprocess as Pre
         v = self.vocab
@@ -1679,9 +1705,10 @@ class OmniParserB200:
         t4 = np.tile(np.arange(4, dtype=np.int32), P)
         sizes4 = [s for s in sizes for _ in range(4)]
         plan = Pre.omni_tile_plan(Pre.turned_sizes(sizes4, t4), tile, overlap)
-        n_inst, pt, poly, rec, prob, *loc = self._decode_tiles(
-            [p for p in pages for _ in range(4)], plan, tile, overlap, t4, max_batch, test_min_size, test_max_size,
-            self._decode_loc_arrays if rec_locations else self._decode_arrays)
+        arrays = self._decode_tiles([p for p in pages for _ in range(4)], plan, tile, overlap, t4, max_batch,
+                                    test_min_size, test_max_size, decode)
+        n_inst, pt, poly, rec, prob = arrays[:5]
+        loc, lists = arrays[5:5 + rec_locations], arrays[5 + rec_locations:]
         rd = merge_tiles(self.ctx, sizes4, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band,
                          iou, turns=t4)
         tiles_rd, whole = rd, None
@@ -1713,12 +1740,32 @@ class OmniParserB200:
             self.last_tiles.update(loc=loc[0])
         if whole is not None:
             self.last_tiles.update(whole=whole, whole_merge=rd)
+        self._keep_tile_lists(lists, src)
         return results
 
-    def _decode_loc_arrays(self):
-        """``_decode_arrays`` with character locations on, the locations appended: (n_inst, pt, poly, rec, prob, loc f32
-        [B, max_inst, rec_length, 5])."""
-        return self._decode_arrays(rec_locations=True) + (self.last_rec_locations,)
+    def _tile_decode(self, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False):
+        """The decode of spot_tiled's tiles and probes: a function giving ``_decode_arrays``' five arrays, then with
+        rec_locations the locations f32 [B, max_inst, rec_length, 5], then with rec_candidates the candidates (ids,
+        probs) or with rec_beams the n-best lists (ids, probs, scores), in ``decode``'s layouts."""
+        def decode():
+            out = self._decode_arrays(None, rec_candidates, rec_beams, length_penalty, rec_locations)
+            if rec_locations:
+                out += (self.last_rec_locations,)
+            return out + (self.last_rec_candidates or self.last_rec_beams or ())
+        return decode
+
+    def _keep_tile_lists(self, lists, source):
+        """After spot_tiled: lists, every tile decode's candidates (ids, probs) or n-best lists (ids, probs, scores),
+        one row per tile (empty when neither was asked for), go to last_tiles['candidates'] / ['beams'], and each
+        merged row's, followed back to its (tile, instance) = source [N, 2], to last_rec_candidates / last_rec_beams in
+        row order; the other is None."""
+        s = np.asarray(source, dtype=np.int64).reshape(-1, 2)
+        rows = tuple(a[s[:, 0], s[:, 1]] for a in lists) if lists else None
+        beams = len(lists) == 3
+        self.last_rec_candidates = None if beams else rows
+        self.last_rec_beams = rows if beams else None
+        if lists:
+            self.last_tiles['beams' if beams else 'candidates'] = lists
 
     def _tile_chars(self, sizes, plan, turns, rows, source, loc) -> List[List[dict]]:
         """'chars' of merged rows (rows: a merge's dict, 'polys' and 'rec' in page pixels; source int [K, 2]: each row's
