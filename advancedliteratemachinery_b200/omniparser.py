@@ -189,6 +189,25 @@ def check_rec_args(k, beams, length_penalty, locations):
     return k, beams, lp, locations
 
 
+def _check_max_batch(max_batch) -> int:
+    """The most tiles or pages a reader encodes at once, >= 1 (ValueError otherwise)."""
+    if int(max_batch) < 1:
+        raise ValueError(f'max_batch must be >= 1, got {max_batch}')
+    return int(max_batch)
+
+
+def _parse_orientation(orientation, n: int, modes, per: str):
+    """A reader's orientation -> (mode, turns): one of the strings modes with turns None, or None with turns int32 [n],
+    one turn per `per` (``preprocess.check_turns``).  ValueError otherwise."""
+    from .preprocess import check_turns
+    if isinstance(orientation, str):
+        if orientation not in modes:
+            raise ValueError(f"orientation must be {', '.join(repr(m) for m in modes)} or one turn per {per}, got "
+                             f"{orientation!r}")
+        return orientation, None
+    return None, check_turns(orientation, n)
+
+
 def _size_arrays(sizes):
     """The heights and widths int32 [P] of pages given as (h, w) sizes."""
     hs = np.ascontiguousarray([int(s[0]) for s in sizes], dtype=np.int32)
@@ -825,6 +844,29 @@ class OmniParserB200:
         self.ctx.check(self.lib.alm_omni_get_memory(self.ctx.h, which, out.data_ptr(), out.numel()))
         return out
 
+    def _check_checkpoint(self, reader: str, kie: bool = False):
+        """ValueError unless the checkpoint is of the kind `reader` reads: KIE (kie) or text spotting."""
+        if bool(self.vocab.vie_categories) != kie:
+            want, got = ('KIE', 'text spotting') if kie else ('text spotting', 'KIE')
+            raise ValueError(f'{reader} reads {want} checkpoints; this one is a {got} checkpoint')
+
+    def _device_pages(self, pages):
+        """Pages (host numpy / torch or CUDA torch) on the context's device, and their (h, w) sizes."""
+        dev = torch.device('cuda', self.ctx.device)
+        pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
+        return pages, [(int(p.shape[0]), int(p.shape[1])) for p in pages]
+
+    def _encode_chunk(self, images: NestedTensor, sizes, test_min_size: int, test_max_size: int):
+        """A chunk of tiles or pages cut by ``preprocess.omni_tiles`` / ``omni_tiles_at`` (sizes: each image's (h, w)
+        before the validation transform) encoded: ``encode`` when the transform gives them one size, ``encode_pages``
+        otherwise."""
+        from . import preprocess as Pre
+        resized, _ = Pre.omni_plan(sizes, test_min_size, test_max_size)
+        if len(set(resized)) == 1:
+            self.encode(images.tensors)
+        else:
+            self.encode_pages(images.tensors, resized)
+
     def _cfg(self, max_instances):
         v = self.vocab
         return _lib.DecodeCfg(v.num_bins, v.pt_eos_index, v.poly_eos_index, v.rec_eos_index, v.pt_sos_index,
@@ -853,40 +895,40 @@ class OmniParserB200:
         self.last_rec_beams = None
         self.last_rec_locations = None
 
-    def _take_rec_locations(self, rec: np.ndarray):
-        """After a decode with locations on: last_rec_locations f32, the layout of `rec` + [5] = (cx, cy, sxx, sxy, syy)
-        divided by the page's encoded size (w, h) -- cx / w, cy / h, sxx / w^2, sxy / (w h), syy / h^2 -- the
-        normalised frame of poly / num_bins."""
-        if not self._rec_loc:
-            return
-        loc = np.zeros(rec.shape + (5,), dtype=np.float32)
-        self.ctx.check(self.lib.alm_omni_get_rec_locations(self.ctx.h, loc.ctypes.data, loc.size))
-        sizes = self._page_sizes if self._page_sizes is not None else page_sizes_from_mask(self._keep_mask)
-        for b, (h, w) in enumerate(sizes):
-            loc[b] /= np.array([w, h, w * w, w * h, h * h], dtype=np.float32)
-        self.last_rec_locations = loc
+    def _take_rec_lists(self, rec: np.ndarray):
+        """After a decode, the lists switched on by ``_set_rec_candidates``, None for the others:
+        last_rec_candidates = (ids int64, probs f32) in the layout of `rec` + [k];
+        last_rec_beams = (ids int64, probs f32, scores f32), ids / probs in the layout of `rec` with [W] inserted before
+        rec_length, scores [..., max_inst, W];
+        last_rec_locations f32, the layout of `rec` + [5] = (cx, cy, sxx, sxy, syy) divided by the page's encoded size
+        (w, h) -- cx / w, cy / h, sxx / w^2, sxy / (w h), syy / h^2 -- the normalised frame of poly / num_bins."""
+        cand = beams = loc = None
+        k, W = self._rec_k, self._rec_beams[0]
+        if k:
+            ids = np.zeros(rec.shape + (k,), dtype=np.int64)
+            probs = np.zeros(ids.shape, dtype=np.float32)
+            self.ctx.check(self.lib.alm_omni_get_rec_candidates(self.ctx.h, ids.ctypes.data, probs.ctypes.data,
+                                                                ids.size))
+            cand = (ids, probs)
+        if W:
+            ids = np.zeros(rec.shape[:-1] + (W, rec.shape[-1]), dtype=np.int64)
+            probs = np.zeros(ids.shape, dtype=np.float32)
+            scores = np.zeros(rec.shape[:-1] + (W,), dtype=np.float32)
+            self.ctx.check(self.lib.alm_omni_get_rec_beams(self.ctx.h, ids.ctypes.data, probs.ctypes.data,
+                                                           scores.ctypes.data, ids.size))
+            beams = (ids, probs, scores)
+        if self._rec_loc:
+            loc = np.zeros(rec.shape + (5,), dtype=np.float32)
+            self.ctx.check(self.lib.alm_omni_get_rec_locations(self.ctx.h, loc.ctypes.data, loc.size))
+            sizes = self._page_sizes if self._page_sizes is not None else page_sizes_from_mask(self._keep_mask)
+            for b, (h, w) in enumerate(sizes):
+                loc[b] /= np.array([w, h, w * w, w * h, h * h], dtype=np.float32)
+        self.last_rec_candidates, self.last_rec_beams, self.last_rec_locations = cand, beams, loc
 
-    def _take_rec_candidates(self, rec: np.ndarray):
-        """After a decode with k > 0: last_rec_candidates = (ids int64, probs f32), the layout of `rec` + [k]."""
-        if self._rec_k == 0:
-            return
-        ids = np.zeros(rec.shape + (self._rec_k,), dtype=np.int64)
-        probs = np.zeros(ids.shape, dtype=np.float32)
-        self.ctx.check(self.lib.alm_omni_get_rec_candidates(self.ctx.h, ids.ctypes.data, probs.ctypes.data, ids.size))
-        self.last_rec_candidates = (ids, probs)
-
-    def _take_rec_beams(self, rec: np.ndarray):
-        """After a decode with W > 0: last_rec_beams = (ids int64, probs f32, scores f32), ids / probs in the layout of
-        `rec` with [W] inserted before rec_length, scores [..., max_inst, W]."""
-        W = self._rec_beams[0]
-        if W == 0:
-            return
-        ids = np.zeros(rec.shape[:-1] + (W, rec.shape[-1]), dtype=np.int64)
-        probs = np.zeros(ids.shape, dtype=np.float32)
-        scores = np.zeros(rec.shape[:-1] + (W,), dtype=np.float32)
-        self.ctx.check(self.lib.alm_omni_get_rec_beams(self.ctx.h, ids.ctypes.data, probs.ctypes.data, scores.ctypes.data,
-                                                       ids.size))
-        self.last_rec_beams = (ids, probs, scores)
+    def _prompt(self, pt_prompt) -> torch.Tensor:
+        """The point prompt the decode entries take: pt_prompt (default ``vocab.pt_prompt()``) as host int64 [L]."""
+        return (pt_prompt if pt_prompt is not None else self.vocab.pt_prompt()).reshape(-1).to(torch.long).cpu() \
+            .contiguous()
 
     def decode(self, pt_prompt: Optional[torch.Tensor] = None, rec_candidates: int = 0, rec_beams: int = 0,
                length_penalty: float = 1.0, rec_locations: bool = False):
@@ -914,7 +956,7 @@ class OmniParserB200:
         [B, max_inst, 32], rec [B, max_inst, rec_length], prob f32 [B, max_inst, rec_length]."""
         v = self.vocab
         B = len(self.page_shapes())
-        prompt = (pt_prompt if pt_prompt is not None else v.pt_prompt()).reshape(-1).to(torch.long).cpu().contiguous()
+        prompt = self._prompt(pt_prompt)
         maxi = max(1, v.pt_seq_length // 2)
         n_inst = np.zeros(B, dtype=np.int32)
         pt = np.zeros((B, maxi, 2), dtype=np.int64)
@@ -926,9 +968,7 @@ class OmniParserB200:
         self.ctx.check(self.lib.alm_omni_decode(self.ctx.h, prompt.data_ptr(), prompt.numel(), C.byref(cfg),
                                                 n_inst.ctypes.data, pt.ctypes.data, poly.ctypes.data, rec.ctypes.data,
                                                 prob.ctypes.data))
-        self._take_rec_candidates(rec)
-        self._take_rec_beams(rec)
-        self._take_rec_locations(rec)
+        self._take_rec_lists(rec)
         return n_inst, pt, poly, rec, prob
 
     def read_at(self, points, rec_candidates: int = 0, rec_beams: int = 0, length_penalty: float = 1.0,
@@ -951,8 +991,7 @@ class OmniParserB200:
         given points), poly [B, N, 32], rec [B, N, rec_length], prob f32 [B, N, rec_length], N = max_instances times
         the number of calls."""
         v = self.vocab
-        if v.vie_categories:
-            raise ValueError('read_at reads text spotting checkpoints; this one is a KIE checkpoint')
+        self._check_checkpoint('read_at')
         B = len(self.page_shapes())
         if len(points) != B:
             raise ValueError(f'{len(points)} point lists for {B} encoded pages')
@@ -983,9 +1022,7 @@ class OmniParserB200:
             prob = np.zeros((B, maxi, v.rec_length), dtype=np.float32)
             self.ctx.check(self.lib.alm_omni_decode_at(self.ctx.h, xy.ctypes.data, cnt.ctypes.data, maxi, C.byref(cfg),
                                                        poly.ctypes.data, rec.ctypes.data, prob.ctypes.data))
-            self._take_rec_candidates(rec)
-            self._take_rec_beams(rec)
-            self._take_rec_locations(rec)
+            self._take_rec_lists(rec)
             outs.append((xy.astype(np.int64), poly, rec, prob))
             lists.append((self.last_rec_candidates, self.last_rec_beams, self.last_rec_locations))
         if calls > 1:
@@ -1026,9 +1063,7 @@ class OmniParserB200:
         self.ctx.check(self.lib.alm_omni_decode_prompts(self.ctx.h, p.data_ptr(), P, p.shape[2], C.byref(cfg),
                                                         n_inst.ctypes.data, pt.ctypes.data, poly.ctypes.data,
                                                         rec.ctypes.data, prob.ctypes.data))
-        self._take_rec_candidates(rec)
-        self._take_rec_beams(rec)
-        self._take_rec_locations(rec)
+        self._take_rec_lists(rec)
         return [[_spotting_result(n_inst[b, k], pt[b, k], poly[b, k], rec[b, k], prob[b, k]) for k in range(P)]
                 for b in range(B)]
 
@@ -1063,7 +1098,7 @@ class OmniParserB200:
         if not (math.isfinite(iou) and 0 < iou <= 1):
             raise ValueError(f'iou must be in (0, 1], got {iou}')
         B = len(self.page_shapes())
-        prompt = (pt_prompt if pt_prompt is not None else v.pt_prompt()).reshape(-1).to(torch.long).cpu().contiguous()
+        prompt = self._prompt(pt_prompt)
         maxi = max(1, v.pt_seq_length // 2)
         cap = maxi * (nx * ny if nx else 9)
         n_inst = np.zeros(B, dtype=np.int32)
@@ -1099,7 +1134,7 @@ class OmniParserB200:
         probs f32 [n]) -- the long single-sequence decode of structure heads (BASELINE config 5: 512 tokens)."""
         v = self.vocab
         B = len(self.page_shapes())
-        prompt = (pt_prompt if pt_prompt is not None else v.pt_prompt()).reshape(-1).to(torch.long).cpu().contiguous()
+        prompt = self._prompt(pt_prompt)
         P = v.pt_seq_length
         n_tok = np.zeros(B, dtype=np.int32)
         toks = np.zeros((B, P), dtype=np.int64)
@@ -1168,7 +1203,7 @@ class OmniParserB200:
         v = self.vocab
         assert v.vie_categories > 0 and v.classes is not None and len(v.classes) == v.vie_categories
         B = len(self.page_shapes())
-        prompt = (pt_prompt if pt_prompt is not None else v.pt_prompt()).reshape(-1).to(torch.long).cpu().contiguous()
+        prompt = self._prompt(pt_prompt)
         maxi, L, P = max(1, v.pt_seq_length // 2), v.rec_length, v.pt_seq_length
         n_tok = np.zeros(B, dtype=np.int32)
         toks = np.zeros((B, P), dtype=np.int64)
@@ -1184,9 +1219,7 @@ class OmniParserB200:
                                                     n_tok.ctypes.data, toks.ctypes.data, tprob.ctypes.data,
                                                     n_inst.ctypes.data, pos.ctypes.data, poly.ctypes.data, rec.ctypes.data,
                                                     prob.ctypes.data))
-        self._take_rec_candidates(rec)
-        self._take_rec_beams(rec)
-        self._take_rec_locations(rec)
+        self._take_rec_lists(rec)
         return n_inst, pos, poly, rec, prob, n_tok, toks, tprob
 
     def spot_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
@@ -1247,74 +1280,75 @@ class OmniParserB200:
         'mixed' choose on hypothesis 0's score.  Candidates combine with rec_locations; beams do not, and neither
         combines with whole_page (``decode_dense`` offers neither).  Refusals come before any device work."""
         from . import postprocess
-        from . import preprocess as Pre
         v = self.vocab
-        if v.vie_categories:
-            raise ValueError('spot_tiled reads text spotting checkpoints; this one is a KIE checkpoint')
-        if int(max_batch) < 1:
-            raise ValueError(f'max_batch must be >= 1, got {max_batch}')
+        self._check_checkpoint('spot_tiled')
+        _check_max_batch(max_batch)
         if rec_locations and whole_page:
             raise ValueError('rec_locations cannot be combined with whole_page: whole-page readings have no locations')
         K, W, lp, rec_locations = check_rec_args(rec_candidates, rec_beams, length_penalty, rec_locations)
         if (K or W) and whole_page:
             raise ValueError('rec_candidates and rec_beams cannot be combined with whole_page: whole-page readings '
                              'have neither')
-        auto = isinstance(orientation, str) and orientation == 'auto'
-        if isinstance(orientation, str):
-            if orientation not in ('upright', 'auto', 'mixed'):
-                raise ValueError(f"orientation must be 'upright', 'auto', 'mixed' or one turn per page, got "
-                                 f"{orientation!r}")
-            turns = None
-        else:
-            turns = Pre.check_turns(orientation, len(pages))
-        dev = torch.device('cuda', self.ctx.device)
-        pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
-        sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
+        mode, turns = _parse_orientation(orientation, len(pages), ('upright', 'auto', 'mixed'), 'page')
+        pages, sizes = self._device_pages(pages)
+        P = len(sizes)
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
         decode = self._tile_decode(K, W, lp, rec_locations)
-        if isinstance(orientation, str) and orientation == 'mixed':
-            return self._spot_mixed(pages, sizes, tile, overlap, max_batch, margin, band, iou, test_min_size,
-                                    test_max_size, whole_page, rec_locations, decode)
         extra = {}
-        if auto:
-            Pre.omni_tile_plan(sizes, tile, overlap)  # a bad layout is refused before the probes run
-            probe, turns, extra['page_scores'] = self._probe_turns(pages, sizes, max_batch, test_min_size, test_max_size,
-                                                                   decode)
-            extra['probe'] = probe
-        plan, arrays = self._read_tiles(pages, sizes, turns, extra.get('probe'), tile, overlap, max_batch, test_min_size,
-                                        test_max_size, decode)
+        if mode == 'auto':
+            turns, extra = self._probe_turns(pages, sizes, tile, overlap, max_batch, test_min_size, test_max_size,
+                                             decode)
+        # the readings the tiles are cut from: page p at turns[p] (None: upright), or for 'mixed' reading 4 p + k, page
+        # p at turn k
+        rpages, rsizes, rturns = pages, sizes, turns
+        if mode == 'mixed':
+            rpages, rsizes = [p for p in pages for _ in range(4)], [s for s in sizes for _ in range(4)]
+            rturns = np.tile(np.arange(4, dtype=np.int32), P)
+        plan, arrays = self._read_tiles(rpages, rsizes, rturns, extra.get('probe'), tile, overlap, max_batch,
+                                        test_min_size, test_max_size, decode)
         n_inst, pt, poly, rec, prob = arrays[:5]
         loc, lists = arrays[5:5 + rec_locations], arrays[5 + rec_locations:]
-        m = merge_tiles(self.ctx, sizes, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band, iou,
-                        turns=turns)
+        m = merge_tiles(self.ctx, rsizes, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band,
+                        iou, turns=rturns)
         out, whole = m, None
         if whole_page and any(max(s) > tile for s in sizes):
-            if auto:  # the probe at the chosen turn is the whole-page reading
-                whole = tuple(a[4 * np.arange(len(sizes)) + turns] for a in extra['probe'])
+            if mode == 'auto':  # the probe at the chosen turn is the whole-page reading
+                whole = tuple(a[4 * np.arange(P) + turns] for a in extra['probe'])
             else:
-                whole = self._read_whole(pages, sizes, turns, tile, max_batch, test_min_size, test_max_size)
-            out = merge_whole_page(self.ctx, sizes, tile, overlap, m, *whole, v.num_bins, margin, turns=turns)
-        texts, scores = postprocess.rec_texts(out['rec'], out['prob'], v)
-        chars = self._tile_chars(sizes, plan, turns, out, out['source'], loc[0]) if rec_locations else None
-        first_tile = np.searchsorted(plan[:, 0], np.arange(len(sizes)))
+                whole = self._read_whole(rpages, rsizes, rturns, tile, max_batch, test_min_size, test_max_size)
+            out = merge_whole_page(self.ctx, rsizes, tile, overlap, m, *whole, v.num_bins, margin, turns=rturns)
+        # the words of every page, each with its reading and its (tile, instance) in the readings' plan
+        if mode == 'mixed':
+            words = merge_turns(self.ctx, out['count'], out['offset'], out['pts'], out['polys'], out['rec'],
+                                out['prob'], v.recog_pad_index, v.rec_eos_index, iou)
+            reading = 4 * np.repeat(np.arange(P), words['count']) + words['source'][:, 0]
+            source = out['source'][out['offset'][reading] + words['source'][:, 1]].reshape(-1, 2)
+        else:
+            words, reading, source = out, np.repeat(np.arange(P), out['count']), out['source']
+        texts, scores = postprocess.rec_texts(words['rec'], words['prob'], v)
+        chars = self._tile_chars(rsizes, plan, rturns, words, source, loc[0]) if rec_locations else None
+        first_tile = np.searchsorted(plan[:, 0], np.arange(len(rsizes)))
         results = []
-        for p in range(len(sizes)):
-            rows = range(int(out['offset'][p]), int(out['offset'][p]) + int(out['count'][p]))
-            turn = {} if turns is None else {'turns': int(turns[p])}
-            results.append([{'pts': [[float(out['pts'][r, 0]), float(out['pts'][r, 1])]], 'score': float(scores[r]),
-                             'polys': out['polys'][r].reshape(-1, 2).tolist(), 'rec': texts[r],
-                             'tile': _tile_of(out['source'][r, 0], first_tile[p]),
-                             'instance': int(out['source'][r, 1]), **turn,
+        for p in range(P):
+            rows = range(int(words['offset'][p]), int(words['offset'][p]) + int(words['count'][p]))
+            results.append([{'pts': [[float(words['pts'][r, 0]), float(words['pts'][r, 1])]], 'score': float(scores[r]),
+                             'polys': words['polys'][r].reshape(-1, 2).tolist(), 'rec': texts[r],
+                             'tile': _tile_of(source[r, 0], first_tile[reading[r]]), 'instance': int(source[r, 1]),
+                             **({} if rturns is None else {'turns': int(rturns[reading[r]])}),
                              **({} if chars is None else {'chars': chars[r]})}
                             for r in rows])
-        self.last_tiles = dict(plan=plan, n_inst=n_inst, pt=pt, poly=poly, rec=rec, prob=prob, merged=m)
+        self.last_tiles = dict(plan=plan, n_inst=n_inst, pt=pt, poly=poly, rec=rec, prob=prob)
+        if mode == 'mixed':
+            self.last_tiles.update(turns=rturns, readings=m, turn_merge=words)
+        else:
+            self.last_tiles.update(merged=m)
         if rec_locations:
             self.last_tiles.update(loc=loc[0])
         if whole is not None:
             self.last_tiles.update(whole=whole, whole_merge=out)
         if turns is not None:
             self.last_tiles.update(turns=turns, **extra)
-        self._keep_tile_lists(lists, out['source'])
+        self._keep_tile_lists(lists, source)
         return results
 
     def read_regions(self, pages, regions, page_index, kind: str = 'quad', tile: int = 1200, overlap: int = 256,
@@ -1357,106 +1391,9 @@ class OmniParserB200:
         from . import postprocess
         from . import preprocess as Pre
         v = self.vocab
-        if v.vie_categories:
-            raise ValueError('read_regions reads text spotting checkpoints; this one is a KIE checkpoint')
-        if int(max_batch) < 1:
-            raise ValueError(f'max_batch must be >= 1, got {max_batch}')
-        if not (isinstance(orientation, str) and orientation == 'upright'):
-            return self._read_regions_turned(pages, regions, page_index, kind, tile, overlap, max_batch, test_min_size,
-                                             test_max_size, rec_candidates, rec_beams, length_penalty, rec_locations,
-                                             orientation)
-        dev = torch.device('cuda', self.ctx.device)
-        pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
-        sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
-        centres = postprocess.region_points(regions, kind)
-        R = len(centres)
-        pi = np.asarray(page_index).reshape(-1)
-        if len(pi) != R or (R and (pi.dtype.kind not in 'iu' or pi.min() < 0 or pi.max() >= len(pages))):
-            raise ValueError(f'page_index must be {R} integers in 0 .. {len(pages) - 1}')
-        pi = pi.astype(np.int64)
-        for r in range(R):   # every point on its page (ValueError otherwise)
-            postprocess.point_bins(centres[r], sizes[pi[r]], v.num_bins)
-        self._set_rec_candidates(rec_candidates, rec_beams, length_penalty, rec_locations)   # refused before device work
-        plan = Pre.omni_tile_plan(sizes, tile, overlap)
-        route = route_regions(sizes, plan, region_boxes(regions, kind), pi)
-        # the plan's tiles that hold a region, then the pages read whole, in chunks of their own kind
-        tiles = [('tile', int(t)) for t in np.unique(route[route >= 0])]
-        whole = [('whole', int(p)) for p in np.unique(pi[route < 0])]
-        mb = int(max_batch)
-        L = v.rec_length
-        rec = np.zeros((R, L), np.int64)
-        prob = np.zeros((R, L), np.float32)
-        pts = np.zeros((R, 2))
-        polys = np.zeros((R, 32))
-        K, W = int(rec_candidates), int(rec_beams)
-        cand = (np.zeros((R, L, K), np.int64), np.zeros((R, L, K), np.float32)) if K > 0 else None
-        beams = (np.zeros((R, W, L), np.int64), np.zeros((R, W, L), np.float32), np.zeros((R, W), np.float32)) \
-            if W > 0 else None
-        loc = np.zeros((R, L, 5), np.float32) if rec_locations else None
-        chunks = []
-        T_whole = max([64] + [max(sizes[p]) for _, p in whole])
-        for chunk in [tiles[i:i + mb] for i in range(0, len(tiles), mb)] + \
-                [whole[i:i + mb] for i in range(0, len(whole), mb)]:
-            frames, rows = [], []   # (y0, x0, h, w) of each image and its regions
-            for what, i in chunk:
-                if what == 'tile':
-                    frames.append((int(plan[i, 1]), int(plan[i, 2]), int(plan[i, 3]), int(plan[i, 4])))
-                    rows.append(np.nonzero(route == i)[0])
-                else:
-                    frames.append((0, 0) + sizes[i])
-                    rows.append(np.nonzero((route < 0) & (pi == i))[0])
-            if chunk[0][0] == 'tile':
-                nt = Pre.omni_tiles_at(self.ctx, pages, [i for _, i in chunk], tile, overlap, test_min_size,
-                                       test_max_size)
-            else:
-                nt = Pre.omni_tiles(self.ctx, [pages[i] for _, i in chunk], T_whole, 0, test_min_size, test_max_size)
-            resized, _ = Pre.omni_plan([f[2:] for f in frames], test_min_size, test_max_size)
-            if len(set(resized)) == 1:
-                self.encode(nt.tensors)
-            else:
-                self.encode_pages(nt.tensors, resized)
-            local = [postprocess.point_bins(centres[r_] - np.array([f[1], f[0]]), f[2:], v.num_bins)
-                     for f, r_ in zip(frames, rows)]
-            n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty, rec_locations)
-            for j, (f, r_) in enumerate(zip(frames, rows)):
-                k = len(r_)
-                rec[r_], prob[r_] = rc[j, :k], pb[j, :k]
-                pts[r_] = tile_to_page(f[:2], f[2:], xy[j, :k], v.num_bins)
-                polys[r_] = tile_to_page(f[:2], f[2:], pl[j, :k].reshape(-1, 2), v.num_bins).reshape(k, 32)
-                if cand is not None:
-                    for a, b in zip(cand, self.last_rec_candidates):
-                        a[r_] = b[j, :k]
-                if beams is not None:
-                    for a, b in zip(beams, self.last_rec_beams):
-                        a[r_] = b[j, :k]
-                if loc is not None:
-                    loc[r_] = self.last_rec_locations[j, :k]
-            chunks.append(dict(kind=chunk[0][0], index=np.array([i for _, i in chunk]), n=n, pt=xy, poly=pl, rec=rc,
-                               prob=pb))
-        texts, scores = postprocess.rec_texts(rec, prob, v)
-        chars = None
-        if loc is not None:  # frames: the plan's tiles, then every page read whole
-            frames = np.concatenate([plan, [(p, 0, 0) + sizes[p] for p in range(len(sizes))]])
-            boxes = char_boxes(self.ctx, sizes, frames, polys, rec, loc, np.where(route >= 0, route, len(plan) + pi),
-                               v.recog_pad_index, v.rec_eos_index)
-            chars = char_dicts(boxes, rec, v)
-        first_tile = np.searchsorted(plan[:, 0], np.arange(len(sizes)))
-        self.last_rec_candidates, self.last_rec_beams, self.last_rec_locations = cand, beams, loc
-        self.last_regions = dict(plan=plan, route=route, points=centres, chunks=chunks)
-        return [{'pts': [pts[r].tolist()], 'score': float(scores[r]), 'polys': polys[r].reshape(16, 2).tolist(),
-                 'rec': texts[r], 'page': int(pi[r]),
-                 'tile': int(route[r] - first_tile[pi[r]]) if route[r] >= 0 else -1,
-                 **({} if chars is None else {'chars': chars[r]})} for r in range(R)]
-
-    def _read_regions_turned(self, pages, regions, page_index, kind, tile, overlap, max_batch, test_min_size,
-                             test_max_size, rec_candidates, rec_beams, length_penalty, rec_locations, orientation):
-        """read_regions with orientation other than 'upright' (rule: DESIGN 4.21): every argument checked before any
-        device work, each candidate reading read at its turned point in its reading's tile (or the reading read
-        whole), then one ``select_regions`` and, with rec_locations, one ``char_boxes`` call."""
-        from . import postprocess
-        from . import preprocess as Pre
-        v = self.vocab
         nb, L = v.num_bins, v.rec_length
+        self._check_checkpoint('read_regions')
+        mb = _check_max_batch(max_batch)
         sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
         centres = postprocess.region_points(regions, kind)
         R = len(centres)
@@ -1466,31 +1403,34 @@ class OmniParserB200:
         pi = pi.astype(np.int64)
         for r in range(R):   # every point on its page (ValueError otherwise)
             postprocess.point_bins(centres[r], sizes[pi[r]], nb)
-        auto = isinstance(orientation, str)
-        if auto:
-            if orientation != 'auto':
-                raise ValueError(f"orientation must be 'upright', 'auto' or one turn per region, got {orientation!r}")
+        mode, cand = _parse_orientation(orientation, R, ('upright', 'auto'), 'region')
+        if mode == 'auto':
             cand = region_turn_candidates(sizes, regions, pi, kind)
         else:
-            cand = Pre.check_turns(orientation, R).reshape(R, 1)
+            cand = (np.zeros(R, np.int32) if mode == 'upright' else cand).reshape(R, 1)
         K, W = int(rec_candidates), int(rec_beams)
         self._set_rec_candidates(K, W, length_penalty, rec_locations)   # refused before device work
         C = cand.shape[1]
-        rp = plan_region_turns(sizes, region_boxes(regions, kind), pi, cand, tile, overlap)
-        readings, plan = rp['readings'], rp['plan']
-        route, reading = rp['route'].reshape(-1), rp['reading'].reshape(-1)   # per candidate g = C r + c
+        boxes = region_boxes(regions, kind)
+        if mode == 'upright':   # every page a reading at turn 0, the plan and routing of the pages as they are
+            readings = np.stack([np.arange(len(sizes)), np.zeros(len(sizes), int)], axis=1).astype(np.int32)
+            plan = Pre.omni_tile_plan(sizes, tile, overlap)
+            route, reading = route_regions(sizes, plan, boxes, pi), pi
+        else:
+            rp = plan_region_turns(sizes, boxes, pi, cand, tile, overlap)
+            readings, plan = rp['readings'], rp['plan']
+            route, reading = rp['route'].reshape(-1), rp['reading'].reshape(-1)   # per candidate g = C r + c
         rturns = np.ascontiguousarray(readings[:, 1])
         rsizes = [sizes[p] for p in readings[:, 0]]
         tsizes = Pre.turned_sizes(rsizes, rturns)
         tpts = turn_points(np.repeat(centres, C, axis=0), np.asarray(rsizes, np.float64).reshape(-1, 2)[reading],
                            cand.reshape(-1))
-        dev = torch.device('cuda', self.ctx.device)
-        pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
+        pages, _ = self._device_pages(pages)
         rpages = [pages[p] for p in readings[:, 0]]   # each page once on the device, listed once per reading
         # the readings' tiles that hold a candidate, then the readings read whole, in chunks of their own kind
         tiles = [('tile', int(t)) for t in np.unique(route[route >= 0])]
         whole = [('whole', int(q)) for q in np.unique(reading[route < 0])]
-        mb, RC = int(max_batch), R * C
+        RC = R * C
         pt, poly = np.zeros((RC, 2), np.int64), np.zeros((RC, 32), np.int64)
         rec, prob = np.zeros((RC, L), np.int64), np.zeros((RC, L), np.float32)
         cands = (np.zeros((RC, L, K), np.int64), np.zeros((RC, L, K), np.float32)) if K > 0 else None
@@ -1516,11 +1456,7 @@ class OmniParserB200:
             else:
                 nt = Pre.omni_tiles(self.ctx, [rpages[i] for i in idx], T_whole, 0, test_min_size, test_max_size,
                                     turns=rturns[idx])
-            resized, _ = Pre.omni_plan([f[2:] for f in frames], test_min_size, test_max_size)
-            if len(set(resized)) == 1:
-                self.encode(nt.tensors)
-            else:
-                self.encode_pages(nt.tensors, resized)
+            self._encode_chunk(nt, [f[2:] for f in frames], test_min_size, test_max_size)
             local = [postprocess.point_bins(tpts[r_] - np.array([f[1], f[0]]), f[2:], nb) for f, r_ in zip(frames, rows)]
             n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty, rec_locations)
             for j, r_ in enumerate(rows):
@@ -1552,15 +1488,19 @@ class OmniParserB200:
         self.last_rec_candidates = None if cands is None else tuple(a[g] for a in cands)
         self.last_rec_beams = None if beams is None else tuple(a[g] for a in beams)
         self.last_rec_locations = None if loc is None else loc[g]
-        self.last_regions = dict(plan=plan, route=rp['route'], points=centres, chunks=chunks, readings=readings,
-                                 reading=rp['reading'], turns=turns, frames=frames, frame_index=fidx,
-                                 rec=rec.reshape(R, C, L), prob=prob.reshape(R, C, L))
-        if auto:
+        if mode == 'upright':   # the pages' own plan and routing
+            self.last_regions = dict(plan=plan, route=route, points=centres, chunks=chunks)
+        else:
+            self.last_regions = dict(plan=plan, route=rp['route'], points=centres, chunks=chunks, readings=readings,
+                                     reading=rp['reading'], turns=turns, frames=frames, frame_index=fidx,
+                                     rec=rec.reshape(R, C, L), prob=prob.reshape(R, C, L))
+        if mode == 'auto':
             self.last_regions.update(candidates=cand, scores=sel['scores'])
         return [{'pts': [sel['pts'][r].tolist()], 'score': float(scores[r]),
                  'polys': sel['polys'][r].reshape(16, 2).tolist(), 'rec': texts[r], 'page': int(pi[r]),
                  'tile': int(route[g[r]] - first_tile[reading[g[r]]]) if route[g[r]] >= 0 else -1,
-                 'turns': int(turns[r]), **({} if chars is None else {'chars': chars[r]})} for r in range(R)]
+                 **({} if mode == 'upright' else {'turns': int(turns[r])}),
+                 **({} if chars is None else {'chars': chars[r]})} for r in range(R)]
 
     def kie_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                   band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200, test_max_size: int = 1920,
@@ -1587,31 +1527,18 @@ class OmniParserB200:
         of ``group_lines``, ``preprocess.curve_crops`` and ``recognize_polygons``); with an orientation also 'turns',
         and for 'auto' 'page_scores' and the probe decodes 'probe'.  Recognition candidates, beams and character
         locations are not offered here."""
-        from . import preprocess as Pre
         v = self.vocab
-        if not v.vie_categories:
-            raise ValueError('kie_tiled reads KIE checkpoints; this one is a text spotting checkpoint')
+        self._check_checkpoint('kie_tiled', kie=True)
         if rec_candidates or rec_beams or rec_locations:
             raise ValueError('kie_tiled offers no recognition candidates, beams or character locations')
-        if int(max_batch) < 1:
-            raise ValueError(f'max_batch must be >= 1, got {max_batch}')
-        auto = isinstance(orientation, str) and orientation == 'auto'
-        if isinstance(orientation, str):
-            if orientation not in ('upright', 'auto'):
-                raise ValueError(f"orientation must be 'upright', 'auto' or one turn per page, got {orientation!r}")
-            turns = None
-        else:
-            turns = Pre.check_turns(orientation, len(pages))
-        dev = torch.device('cuda', self.ctx.device)
-        pages = [(p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p))).to(dev) for p in pages]
-        sizes = [(int(p.shape[0]), int(p.shape[1])) for p in pages]
+        _check_max_batch(max_batch)
+        mode, turns = _parse_orientation(orientation, len(pages), ('upright', 'auto'), 'page')
+        pages, sizes = self._device_pages(pages)
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
         extra = {}
-        if auto:
-            Pre.omni_tile_plan(sizes, tile, overlap)  # a bad layout is refused before the probes run
-            probe, turns, extra['page_scores'] = self._probe_turns(pages, sizes, max_batch, test_min_size, test_max_size,
-                                                                   self._decode_kie_arrays)
-            extra['probe'] = probe
+        if mode == 'auto':
+            turns, extra = self._probe_turns(pages, sizes, tile, overlap, max_batch, test_min_size, test_max_size,
+                                             self._decode_kie_arrays)
         plan, (n_inst, pos, poly, rec, prob, n_tok, toks, tprob) = self._read_tiles(
             pages, sizes, turns, extra.get('probe'), tile, overlap, max_batch, test_min_size, test_max_size,
             self._decode_kie_arrays)
@@ -1662,16 +1589,12 @@ class OmniParserB200:
         and decoded by decode (``_decode_arrays``, ``_decode_dense_arrays`` or ``_decode_kie_arrays``): its arrays, one
         row per tile."""
         from . import preprocess as Pre
-        resized, _ = Pre.omni_plan([(int(h), int(w)) for h, w in plan[:, 3:5]], test_min_size, test_max_size)
         outs = []
         for first in range(0, len(plan), int(max_batch)):
             count = min(int(max_batch), len(plan) - first)
             nt = Pre.omni_tiles(self.ctx, pages, tile, overlap, test_min_size, test_max_size, first, count, turns=turns)
-            chunk = resized[first:first + count]
-            if len(set(chunk)) == 1:
-                self.encode(nt.tensors)
-            else:
-                self.encode_pages(nt.tensors, chunk)
+            self._encode_chunk(nt, [(int(h), int(w)) for h, w in plan[first:first + count, 3:5]], test_min_size,
+                               test_max_size)
             outs.append(decode())
         return tuple(np.concatenate(a) for a in zip(*outs))
 
@@ -1692,56 +1615,6 @@ class OmniParserB200:
         for a, b in zip(out, sub):
             a[big] = b
         return out
-
-    def _spot_mixed(self, pages, sizes, tile, overlap, max_batch, margin, band, iou, test_min_size, test_max_size,
-                    whole_page, rec_locations, decode):
-        """spot_tiled(orientation='mixed'): every page read in tiles at turns 0..3 (reading 4 p + k) by decode
-        (``_tile_decode``), one merge of the 4 P readings, with whole_page each reading merged with its whole-page
-        partner (merge_whole_page), then one merge of each page's four readings (merge_turns)."""
-        from . import postprocess
-        from . import preprocess as Pre
-        v = self.vocab
-        P = len(pages)
-        t4 = np.tile(np.arange(4, dtype=np.int32), P)
-        sizes4 = [s for s in sizes for _ in range(4)]
-        plan = Pre.omni_tile_plan(Pre.turned_sizes(sizes4, t4), tile, overlap)
-        arrays = self._decode_tiles([p for p in pages for _ in range(4)], plan, tile, overlap, t4, max_batch,
-                                    test_min_size, test_max_size, decode)
-        n_inst, pt, poly, rec, prob = arrays[:5]
-        loc, lists = arrays[5:5 + rec_locations], arrays[5 + rec_locations:]
-        rd = merge_tiles(self.ctx, sizes4, tile, overlap, plan, n_inst, pt, poly, rec, prob, v.num_bins, margin, band,
-                         iou, turns=t4)
-        tiles_rd, whole = rd, None
-        if whole_page and any(max(s) > tile for s in sizes):
-            whole = self._read_whole([p for p in pages for _ in range(4)], sizes4, t4, tile, max_batch, test_min_size,
-                                     test_max_size)
-            rd = merge_whole_page(self.ctx, sizes4, tile, overlap, tiles_rd, *whole, v.num_bins, margin, turns=t4)
-        m = merge_turns(self.ctx, rd['count'], rd['offset'], rd['pts'], rd['polys'], rd['rec'], rd['prob'],
-                        v.recog_pad_index, v.rec_eos_index, iou)
-        texts, scores = postprocess.rec_texts(m['rec'], m['prob'], v)
-        # each kept row's (tile, instance) in the 4 P readings' plan, through its reading's row
-        page_of = np.repeat(np.arange(P), m['count'])
-        src = rd['source'][rd['offset'][4 * page_of + m['source'][:, 0]] + m['source'][:, 1]].reshape(-1, 2)
-        chars = self._tile_chars(sizes4, plan, t4, m, src, loc[0]) if rec_locations else None
-        first_tile = np.searchsorted(plan[:, 0], np.arange(4 * P))
-        results = []
-        for p in range(P):
-            page = []
-            for r in range(int(m['offset'][p]), int(m['offset'][p]) + int(m['count'][p])):
-                k = int(m['source'][r, 0])
-                page.append({'pts': [[float(m['pts'][r, 0]), float(m['pts'][r, 1])]], 'score': float(scores[r]),
-                             'polys': m['polys'][r].reshape(-1, 2).tolist(), 'rec': texts[r],
-                             'tile': _tile_of(src[r, 0], first_tile[4 * p + k]), 'instance': int(src[r, 1]), 'turns': k,
-                             **({} if chars is None else {'chars': chars[r]})})
-            results.append(page)
-        self.last_tiles = dict(plan=plan, n_inst=n_inst, pt=pt, poly=poly, rec=rec, prob=prob, turns=t4,
-                               readings=tiles_rd, turn_merge=m)
-        if rec_locations:
-            self.last_tiles.update(loc=loc[0])
-        if whole is not None:
-            self.last_tiles.update(whole=whole, whole_merge=rd)
-        self._keep_tile_lists(lists, src)
-        return results
 
     def _tile_decode(self, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False):
         """The decode of spot_tiled's tiles and probes: a function giving ``_decode_arrays``' five arrays, then with
@@ -1776,11 +1649,13 @@ class OmniParserB200:
                            source[:, 0], v.recog_pad_index, v.rec_eos_index, turns=turns)
         return char_dicts(boxes, rows['rec'], v)
 
-    def _probe_turns(self, pages, sizes, max_batch, test_min_size, test_max_size, decode):
-        """Every page read whole at turns 0..3 (reading 4 p + k; one tile no smaller than any page) by decode and the
-        choice of orient_select on the readings' instance rows (the first five arrays: n_inst, _, _, rec, prob) ->
-        (probe decode arrays, turns int32 [P], scores f64 [P, 4])."""
+    def _probe_turns(self, pages, sizes, tile, overlap, max_batch, test_min_size, test_max_size, decode):
+        """'auto''s probes: every page read whole at turns 0..3 (reading 4 p + k; one tile no smaller than any page) by
+        decode and the choice of orient_select on the readings' instance rows (the first five arrays: n_inst, _, _, rec,
+        prob) -> (turns int32 [P], dict(page_scores=f64 [P, 4], probe=the probe decode arrays)).  A tile layout the
+        pages cannot be read in (tile, overlap) is refused before the probes run."""
         from . import preprocess as Pre
+        Pre.omni_tile_plan(sizes, tile, overlap)
         P = len(pages)
         t4 = np.tile(np.arange(4, dtype=np.int32), P)
         T = max(64, max(max(s) for s in sizes))
@@ -1791,7 +1666,7 @@ class OmniParserB200:
         turns, scores = orient_select(self.ctx, n_inst.reshape(P, 4), rec.reshape((P, 4) + rec.shape[1:]),
                                       prob.reshape((P, 4) + prob.shape[1:]), self.vocab.recog_pad_index,
                                       self.vocab.rec_eos_index)
-        return probe, turns, scores
+        return turns, dict(page_scores=scores, probe=probe)
 
     def group_lines(self, results, **params) -> List[List[dict]]:
         """The words of every page assembled into text lines in reading order (rule: DESIGN 4.12).  results: per page

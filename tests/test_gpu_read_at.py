@@ -362,6 +362,8 @@ def test_read_regions_on_an_a4_page_with_candidates_and_beams(golden_dir):
     rng = np.random.default_rng(9)
     a4 = rng.integers(0, 256, (3508, 2480, 3), dtype=np.uint8)
     small = rng.integers(0, 256, (500, 700, 3), dtype=np.uint8)
+    empty = np.zeros((1300, 900, 3), np.uint8)   # two tiles and no region, before a page with regions
+    pages = [a4, empty, small]
     kw = dict(tile=1200, overlap=256, test_min_size=1200, test_max_size=1920)
     R = 40
     xy = rng.uniform([0, 0], [2480 - 400, 3508 - 60], (R, 2))   # every centre on the page
@@ -369,12 +371,12 @@ def test_read_regions_on_an_a4_page_with_candidates_and_beams(golden_dir):
     boxes = np.concatenate([xy, xy + wh], 1)
     boxes[R - 1] = [1100, 1500, 2200, 1540]   # across two column seams, in no tile: read whole
     pi = np.zeros(R + 3, int)
-    pi[-3:] = 1
+    pi[-3:] = 2
     boxes = np.concatenate([boxes, [[10, 10, 100, 40], [600, 450, 700, 500], [0, 0, 700, 500]]])
-    res = check_regions(m, [a4, small], boxes, pi, 'box', kw, max_batch=3)
+    res = check_regions(m, pages, boxes, pi, 'box', kw, max_batch=3)
     assert res[R - 1]['tile'] == -1 and all(r['tile'] == 0 for r in res[R:])
     for extra in (dict(rec_candidates=3), dict(rec_beams=2)):
-        got = m.read_regions([a4, small], boxes, pi, kind='box', max_batch=3, **extra, **kw)
+        got = m.read_regions(pages, boxes, pi, kind='box', max_batch=3, **extra, **kw)
         if 'rec_candidates' in extra:   # candidate 0 is the greedy reading
             assert [g['rec'] for g in got] == [r['rec'] for r in res]
         lst = m.last_rec_candidates if 'rec_candidates' in extra else m.last_rec_beams
