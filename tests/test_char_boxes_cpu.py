@@ -3,30 +3,20 @@ reference's own slicing (OCR/MGP-STR/demo.py:119-124) on the fixture maps, of th
 host against the oracle (bit for bit), and of the geometry the boxes land in."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+from tests.support import emu
 from tests.test_curve_crops_cpu import random_polygons
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 
 
-def build_emu():
-    """Build tests/emu/char_box_emu.cpp (host compile of char_box_kernel's body) and bind it."""
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'char_box_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'char_box_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/char_box_emu.cpp (host compile of char_box_kernel's body)."""
     lib.emu_char_boxes.restype = None
     lib.emu_char_boxes.argtypes = [C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 7
-    return lib
 
 
 def emu_char_boxes(lib, maps, ids, head, kind=0, sizes=None, geom=None):
@@ -156,7 +146,7 @@ def test_kernel_body_on_the_host_equals_oracle(kind):
     maps, ids = random_maps(rng, B), random_ids(rng, B)
     q, cv = plans(rng, B)
     sizes, geom = {0: (None, None), 1: (q['sizes'], q['minv']), 2: (cv['sizes'], cv['ctrl'])}[kind]
-    lib = build_emu()
+    lib = emu('char_box_emu', bind)
     for head in (0, 1, 2):
         hid = ids if head == 0 else np.where(ids == 1, V.END_ID[head], ids)
         got = emu_char_boxes(lib, maps, hid, head, kind, sizes, geom)
@@ -177,7 +167,7 @@ def test_one_hot_column_maps_to_its_span():
         col = rng.random(8).astype(np.float32)
         maps[0, x + 1, 1 + 32 * np.arange(8) + x] = col / col.sum()
     ids = np.full((1, 27), 5, np.int32); ids[0, 0] = 0
-    n, boxes, centres = emu_char_boxes(build_emu(), maps, ids, 1)  # BPE head without an end id: 26 boxes
+    n, boxes, centres = emu_char_boxes(emu('char_box_emu', bind), maps, ids, 1)  # BPE head without an end id: 26 boxes
     assert n[0] == 26
     for x in range(26):
         L, R, xc, _ = V.reduce_map(maps[0, x + 1])
@@ -199,7 +189,7 @@ def test_axis_aligned_region_gives_affine_boxes():
     cw, ch = (int(v) for v in plan['sizes'][0])
     maps, ids = random_maps(rng, 1), random_ids(rng, 1)
     ids[0, 20] = 1; ids[0, :20] = 7
-    n, boxes, centres = emu_char_boxes(build_emu(), maps, ids, 0, 1, plan['sizes'], plan['minv'])
+    n, boxes, centres = emu_char_boxes(emu('char_box_emu', bind), maps, ids, 0, 1, plan['sizes'], plan['minv'])
     assert n[0] == 19
     sx, sy = (x1 - x0) / (cw - 1), (y1 - y0) / (ch - 1)
     for j in range(n[0]):
@@ -230,7 +220,7 @@ def test_curved_boxes_follow_the_arc():
     rng = np.random.default_rng(6)
     maps = random_maps(rng, 1)
     ids = np.full((1, 27), 9, np.int32); ids[0, 0] = 0
-    n, boxes, centres = emu_char_boxes(build_emu(), maps, ids, 2, 2, plan['sizes'], plan['ctrl'])
+    n, boxes, centres = emu_char_boxes(emu('char_box_emu', bind), maps, ids, 2, 2, plan['sizes'], plan['ctrl'])
     assert n[0] == 26
     extent = float(np.ptp(poly, axis=0).max())
     for j in range(26):
@@ -245,7 +235,7 @@ def test_curved_boxes_follow_the_arc():
     maps[0, 1:] = 0
     maps[0, 1, 1] = 1
     maps[0, 2, 1 + 31] = 1
-    _, boxes, _ = emu_char_boxes(build_emu(), maps, ids, 2, 2, plan['sizes'], plan['ctrl'])
+    _, boxes, _ = emu_char_boxes(emu('char_box_emu', bind), maps, ids, 2, 2, plan['sizes'], plan['ctrl'])
     assert np.abs(boxes[0, 0, 0] - poly[0]).max() < 3 and np.abs(boxes[0, 1, 1] - poly[7]).max() < 3
 
 

@@ -5,13 +5,12 @@ oracle/gen_golden_curves.py).  Bar: bit-exact crops and tensors everywhere; cont
 polygon's extent of bezier_fit_quad (the library solves the same least-squares problem in its own code)."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
+
+from tests.support import emu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 REF_MISC = '/root/reference/OCR/OmniParser/utils/misc.py'
@@ -71,18 +70,10 @@ def curve_regions(seed, n_pages=16, per_page=64, size=1024):
     return pages, polys, np.repeat(np.arange(n_pages, dtype=np.int32), per_page)
 
 
-def build_emu():
-    """Build tests/emu/curve_emu.cpp (host compile of the kernels' per-pixel bodies) and bind it."""
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'curve_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'curve_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/curve_emu.cpp (host compile of the kernels' per-pixel bodies)."""
     lib.emu_curve_crops.restype = None
     lib.emu_curve_crops.argtypes = [C.c_int] + [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-    return lib
 
 
 def emu_curve_crops(lib, pages, polys, page_index, imgH=32, imgW=128):
@@ -242,7 +233,7 @@ def test_kernel_bodies_on_the_host_equal_fixture():
     run over every launch's grid with the library's plan and weights, reproduce every reference crop and the final
     tensor bit for bit."""
     z, pages, crops, out = curve_fixture()
-    warped, plan, got = emu_curve_crops(build_emu(), pages, z['polys'], z['page_index'])
+    warped, plan, got = emu_curve_crops(emu('curve_emu', bind), pages, z['polys'], z['page_index'])
     assert np.array_equal(plan['sizes'], z['sizes'])
     for r, (a, b) in enumerate(zip(unpack(warped, plan['sizes']), crops)):
         assert np.array_equal(a, b), r
@@ -258,7 +249,7 @@ def test_kernel_bodies_equal_oracle_on_random_polygons():
     pages = [rng.integers(0, 256, (1024, 1024, 3), dtype=np.uint8)]
     polys = random_polygons(rng, 1000, 1024, 1024)
     pidx = np.zeros(1000, np.int32)
-    warped, plan, got = emu_curve_crops(build_emu(), pages, polys, pidx)
+    warped, plan, got = emu_curve_crops(emu('curve_emu', bind), pages, polys, pidx)
     plans = [(plan['ctrl'][r], int(w), int(h)) for r, (w, h) in enumerate(plan['sizes'])]
     crops, ref = V.curve_crops(pages, polys, pidx, plans=plans)
     for r, (a, b) in enumerate(zip(unpack(warped, plan['sizes']), crops)):

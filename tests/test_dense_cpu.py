@@ -4,33 +4,20 @@ must partition the page, the point filter must keep exactly the owned points, an
 equal the oracle bit for bit (and alm_omni_merge_turns' emulation at n = 4)."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import dense_ref as D
-from tests.test_tiles_cpu import assert_same
+from tests.support import assert_same, emu
 from tests.test_turn_merge_cpu import EOS, PAD, emu_merge, fixture_rows, poly_of
 
 _EMU = None
 NB = 1000
 
 
-def build_emu():
-    """Build tests/emu/dense_emu.cpp (host compile of the kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'dense_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'dense_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/dense_emu.cpp (host compile of the kernels' bodies)."""
     lib.emu_window.argtypes = [C.c_int] * 4 + [C.c_void_p]
     lib.emu_owns.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
     lib.emu_trained_grid.argtypes = [C.c_int, C.c_int]
@@ -38,19 +25,17 @@ def build_emu():
     lib.emu_merge_readings.restype = C.c_long
     lib.emu_merge_readings.argtypes = ([C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int64, C.c_int64, C.c_double]
                                        + [C.c_void_p] * 7)
-    _EMU = lib
-    return lib
 
 
 def emu_window(nx, ny, w, nb=NB):
     box = np.zeros(4, np.int32)
-    build_emu().emu_window(nb, nx, ny, w, box.ctypes.data)
+    emu('dense_emu', bind).emu_window(nb, nx, ny, w, box.ctypes.data)
     return box.tolist()
 
 
 def emu_merge_readings(nr, count, offset, pts, polys, rec, prob, pad=PAD, eos=EOS, iou=0.5):
     """alm_omni_merge_readings' three launches on the host -> the dict merge_readings / dense_ref.merge return."""
-    lib = build_emu()
+    lib = emu('dense_emu', bind)
     count = np.ascontiguousarray(count, np.int32)
     offset = np.ascontiguousarray(offset, np.int32)
     pts = np.ascontiguousarray(pts, np.float64).reshape(-1, 2)
@@ -127,7 +112,7 @@ def test_window_table_at_1000_bins():
 
 
 def test_only_the_trained_grids_are_allowed():
-    lib = build_emu()
+    lib = emu('dense_emu', bind)
     for nx in range(-1, 6):
         for ny in range(-1, 6):
             assert lib.emu_trained_grid(nx, ny) == ((nx, ny) in D.TRAINED)
@@ -136,7 +121,7 @@ def test_only_the_trained_grids_are_allowed():
 @pytest.mark.parametrize('nx,ny', D.TRAINED)
 @pytest.mark.parametrize('nb', [1000, 7, 3])
 def test_ownership_partitions_the_page(nx, ny, nb):
-    lib = build_emu()
+    lib = emu('dense_emu', bind)
     boxes = [np.array(emu_window(nx, ny, w, nb), np.int32) for w in range(nx * ny)]
     v = np.arange(nb)
     for x in v[::max(1, nb // 97)].tolist() + [nb - 1]:
@@ -150,7 +135,7 @@ def test_ownership_partitions_the_page(nx, ny, nb):
 
 
 def test_point_filter_keeps_the_owned_points_in_order():
-    lib = build_emu()
+    lib = emu('dense_emu', bind)
     rng = np.random.default_rng(3)
     for nx, ny in D.TRAINED:
         for w in range(nx * ny):

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from tests.beam_ref import beam_rec
+from tests.support import close_models, omni_model, options, release_models
 from tests.test_pages_cpu import pages_case, pages_page
 from tests.test_prompts_cpu import prompt_case, prompt_page
 
@@ -21,25 +22,8 @@ ERR_INVALID, ERR_STATE = -1, -4
 NEAR_TIE = 1e-4   # selection / ranking margin below which the oracle's order is not compared
 
 
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
 def spot_model(wseed, bias):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    key = ('spot', wseed, bias)
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(omni_sd(wseed, bias), OmniVocab(), workspace_mb=8192)
-    return _MODELS[key]
+    return omni_model(dict(wseed=wseed, pt_eos_bias=bias), workspace_mb=8192)
 
 
 def _terminal_end(v, row):
@@ -106,14 +90,11 @@ def test_width_one_is_greedy_on_the_full_and_masked_fixtures(graphs):
         v = m.vocab
         v.pt_seq_length, v.rec_length = case['pt_seq_length'], case['rec_length']
         img, mask = omni_inputs(case)
-        m.ctx.set_option('use_graphs', graphs)
-        try:
+        with options(m.ctx, use_graphs=graphs):
             m.encode(img, mask)
             n, _, rec, prob = _decode_raw(m)
             assert m.last_rec_beams is None
             n1, _, rec1, prob1 = _decode_raw(m, rec_beams=1)
-        finally:
-            m.ctx.set_option('use_graphs', 1)
         assert np.array_equal(n, n1) and n.sum() > 0
         _assert_greedy_prefix(v, rec, prob, rec1, prob1, name)
         ids, bp, sc = m.last_rec_beams
@@ -127,8 +108,7 @@ def test_width_one_is_greedy_for_kie():
     from advancedliteratemachinery_b200 import NestedTensor, OmniParserB200, OmniVocab
     from advancedliteratemachinery_b200 import synthetic as W
     from oracle.gen_golden import KIE_CASES, omni_inputs
-    for key in list(_MODELS):
-        _MODELS.pop(key).ctx.close()
+    close_models()
     case = KIE_CASES['kie']
     sd = W.omniparser_state_dict(seed=case['wseed'], vie_categories=case['vie'], pt_eos_bias=case['pt_eos_bias'])
     v = OmniVocab(vie_categories=case['vie'], pt_seq_length=case['pt_seq_length'], rec_length=case['rec_length'])
@@ -263,9 +243,7 @@ def test_full_fixture_hypotheses_match_teacher_forcing_and_the_cpu_rule():
     mem, pos, kpm, _ = O.encode(img.cpu(), mask.cpu(), sd)
     compared = 0
     for xattn in (0, 2):
-        m.ctx.set_option('xattn_impl', xattn)
-        m.ctx.set_option('nsplit', 3)
-        try:
+        with options(m.ctx, xattn_impl=xattn, nsplit=3):
             m.encode(img, mask)
             for width, alpha in ((2, 0.0), (4, 1.0), (8, 1.0)):
                 n_inst, pt, _, _ = _decode_raw(m, rec_beams=width, length_penalty=alpha)
@@ -282,9 +260,6 @@ def test_full_fixture_hypotheses_match_teacher_forcing_and_the_cpu_rule():
                         np.testing.assert_allclose(sc[0, :n], rs, atol=5e-4)
                         np.testing.assert_allclose(bp[0, :n], rp, rtol=5e-5, atol=0)   # GPU vs CPU fp32 logits
                         compared += 1
-        finally:
-            m.ctx.set_option('xattn_impl', 0)
-            m.ctx.set_option('nsplit', 1)
     print(f'{compared} beam runs compared with the CPU rule id for id')
 
 
@@ -292,8 +267,7 @@ def test_config2_scale_hypotheses_match_teacher_forcing():
     from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
     from oracle.gen_golden import CONFIG2_CASE, config2_page
     from tests.conftest import omni_sd
-    for key in list(_MODELS):
-        _MODELS.pop(key).ctx.close()
+    close_models()
     case = CONFIG2_CASE
     v = OmniVocab(pt_seq_length=case['pt_seq_length'], rec_length=case['rec_length'])
     m = OmniParserB200(omni_sd(case['wseed'], case['pt_eos_bias']), v, workspace_mb=20480)
@@ -480,12 +454,9 @@ def test_op_self_attention_step_with_ancestry(t):
     out = torch.zeros(S, 512)
     d = [x.cuda().contiguous() for x in (qkv, kc, vc, out, anc)]
     for wide in (1, 0):
-        m.ctx.set_option('sattn_wide', wide)
-        try:
+        with options(m.ctx, sattn_wide=wide):
             m.ctx.check(m.lib.alm_op_self_attention_step_anc(m.ctx.h, d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(),
                                                              d[3].data_ptr(), S, t, Tmax, d[4].data_ptr()))
-        finally:
-            m.ctx.set_option('sattn_wide', 1)
         got = d[3].cpu().double()
         q = qkv[:, :512].double().reshape(S, 8, 64) / 8
         for s in range(S):

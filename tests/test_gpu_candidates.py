@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import close_models, omni_model, options, release_models
 from tests.test_pages_cpu import pages_case, pages_page
 from tests.test_prompts_cpu import prompt_case, prompt_page
 
@@ -159,25 +160,8 @@ def assert_candidates_head(rec, prob, cand):
     assert (probs[..., 1:] <= probs[..., :-1]).all()
 
 
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
 def spot_model(wseed, bias):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    key = ('spot', wseed, bias)
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(omni_sd(wseed, bias), OmniVocab(), workspace_mb=8192)
-    return _MODELS[key]
+    return omni_model(dict(wseed=wseed, pt_eos_bias=bias), workspace_mb=8192)
 
 
 @pytest.mark.parametrize('k', [1, 4])
@@ -210,13 +194,10 @@ def test_omni_full_candidates_match_teacher_forcing_and_graphs(k, golden_dir):
     check_teacher_forced(m, 0, pt.reshape(n, 2), rec[0].numpy(), ids[0, :n], cp[0, :n], report)
     assert report.get('near_tie_steps', 0) <= MAX_NEAR_TIE_FLIPS, report
     # the eager decode (no captured graphs) gives the same bits
-    m.ctx.set_option('use_graphs', 0)
-    try:
+    with options(m.ctx, use_graphs=0):
         m.encode(img, mask)
         m.decode(rec_candidates=k)
         ids2, cp2 = m.last_rec_candidates
-    finally:
-        m.ctx.set_option('use_graphs', 1)
     assert np.array_equal(ids, ids2) and np.array_equal(cp.view(np.uint32), cp2.view(np.uint32))
 
 
@@ -225,8 +206,7 @@ def test_omni_kie_candidates_use_the_kie_softmax(k):
     from advancedliteratemachinery_b200 import NestedTensor, OmniParserB200, OmniVocab
     from advancedliteratemachinery_b200 import synthetic as W
     from oracle.gen_golden import KIE_CASES, omni_inputs
-    for key in list(_MODELS):
-        _MODELS.pop(key).ctx.close()
+    close_models()
     case = KIE_CASES['kie']
     sd = W.omniparser_state_dict(seed=case['wseed'], vie_categories=case['vie'], pt_eos_bias=case['pt_eos_bias'])
     v = OmniVocab(vie_categories=case['vie'], pt_seq_length=case['pt_seq_length'], rec_length=case['rec_length'])

@@ -2,12 +2,12 @@
 (alm_mgpstr_forward_boxes, recognize* with char_boxes=True).  Bar: the device boxes equal the oracle bit for bit when
 the oracle is fed the device's own maps (read back through forward(is_eval=True)); ids and probabilities are the same
 bits with boxes on and off; boxes add exactly one launch per head."""
-
 import numpy as np
 import pytest
 import torch
 
-from tests.test_char_boxes_cpu import build_emu, emu_char_boxes
+from tests.support import emu, mgp_model, options, release_models
+from tests.test_char_boxes_cpu import bind, emu_char_boxes
 from tests.test_curve_crops_cpu import curve_fixture, curve_regions
 from tests.test_quad_crops_cpu import quad_fixture
 
@@ -17,11 +17,7 @@ ALM_ERR_INVALID, ALM_ERR_STATE = -1, -4
 
 @pytest.fixture(scope='module')
 def model():
-    from advancedliteratemachinery_b200 import MGPSTRB200
-    from tests.conftest import mgp_sd
-    m = MGPSTRB200(mgp_sd(0))
-    yield m
-    m.ctx.close()
+    return mgp_model()
 
 
 def device_maps(m, crops):
@@ -58,8 +54,7 @@ def test_boxes_equal_oracle_on_device_maps(model, nsplit):
     without boxes bit for bit."""
     from advancedliteratemachinery_b200 import _lib, preprocess as P
     m = model
-    m.ctx.set_option('nsplit', nsplit)
-    try:
+    with options(m.ctx, nsplit=nsplit):
         zc, cpages, ccrops, _ = curve_fixture()
         crops = P.mgp_crops(m.ctx, ccrops)
         ref_ids, ref_prob = m.recognize(crops)
@@ -88,8 +83,6 @@ def test_boxes_equal_oracle_on_device_maps(model, nsplit):
         assert np.array_equal(dids, ids.numpy())
         plan = P.curve_plan([p.shape[:2] for p in cpages], zc['polys'], zc['page_index'])
         assert_oracle(maps, dids, got, _lib.BOX_CURVE, plan['sizes'], plan['ctrl'])
-    finally:
-        m.ctx.set_option('nsplit', 3)
 
 
 def test_thousand_regions_equal_oracle(model):
@@ -101,7 +94,7 @@ def test_thousand_regions_equal_oracle(model):
     pages, polys, pidx = curve_regions(seed=5)
     dev = [torch.from_numpy(p).cuda() for p in pages]
     sizes = [p.shape[:2] for p in pages]
-    lib = build_emu()
+    lib = emu('char_box_emu', bind)
     rows = np.arange(0, 1024, 16)
     quads = Post.quads_from_polygons(polys)
     for kind, crop, regions, recog, planner in (

@@ -23,11 +23,10 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import omni_model, options, release_models
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
-
-DEFAULT = dict(enc_grid_cap=0, dec_grid_cap=0, small_grid_cap=0, decode_streams=2, decode_priority=0, use_graphs=1)
-_MODELS = {}
 
 
 def _settings():
@@ -40,31 +39,9 @@ def _settings():
             'all': dict(enc_grid_cap=7, dec_grid_cap=5, small_grid_cap=3, decode_streams=1, decode_priority=1)}
 
 
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def omni_model(wseed, pt_eos_bias, vie=0):
+def omni_for(wseed, pt_eos_bias, vie=0):
     """one resident OmniParserB200 per synthetic checkpoint"""
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from advancedliteratemachinery_b200 import synthetic as W
-    from tests.conftest import omni_sd
-    key = (wseed, pt_eos_bias, vie)
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        sd = W.omniparser_state_dict(seed=wseed, vie_categories=vie, pt_eos_bias=pt_eos_bias) if vie else \
-            omni_sd(wseed, pt_eos_bias)
-        _MODELS[key] = OmniParserB200(sd, OmniVocab(vie_categories=vie), workspace_mb=4096)
-    return _MODELS[key]
-
-
-def set_knobs(ctx, **opts):
-    for k, v in dict(DEFAULT, **opts).items():
-        ctx.set_option(k, v)
+    return omni_model(dict(wseed=wseed, pt_eos_bias=pt_eos_bias, vie=vie), kie=bool(vie))
 
 
 def _flat(x):
@@ -91,19 +68,15 @@ def _assert_same(base, got, label):
 
 def sweep(ctx, run, what):
     """run() under the default options, then under every setting with graphs on and off: bit for bit the default"""
-    set_knobs(ctx)
     base = run()
     n = 0
-    try:
-        for graphs in (1, 0):
-            for name, opts in _settings().items():
-                if name == 'default' and graphs:
-                    continue
-                set_knobs(ctx, use_graphs=graphs, **opts)
+    for graphs in (1, 0):
+        for name, opts in _settings().items():
+            if name == 'default' and graphs:
+                continue
+            with options(ctx, use_graphs=graphs, **opts):
                 _assert_same(base, run(), f'{what}: {name}, use_graphs {graphs}')
-                n += 1
-    finally:
-        set_knobs(ctx)
+            n += 1
     print(f'[coschedule] {what}: {n} settings bit-identical to the default')
     return base
 
@@ -114,7 +87,7 @@ def _fixture_spotting(name, golden_dir):
     from oracle.gen_golden import OMNI_CASES, omni_inputs
     case = OMNI_CASES[name]
     gold = np.load(os.path.join(golden_dir, f'omni_{name}.npz'))
-    m = omni_model(case['wseed'], case['pt_eos_bias'])
+    m = omni_for(case['wseed'], case['pt_eos_bias'])
     m.vocab.pt_seq_length, m.vocab.rec_length = case['pt_seq_length'], case['rec_length']
     img, mask = omni_inputs(case)
     return case, gold, m, img, mask, _spotting_result
@@ -172,7 +145,7 @@ def test_pages_fixture_under_every_knob(golden_dir):
     from tests.test_gpu_omni_pages import ORDER, fixture_batch
     from tests.test_pages_cpu import pages_case
     gold = pages_case(golden_dir)
-    m = omni_model(int(gold['wseed'][0]), float(gold['pt_eos_bias'][0]))
+    m = omni_for(int(gold['wseed'][0]), float(gold['pt_eos_bias'][0]))
     m.vocab.pt_seq_length, m.vocab.rec_length = int(gold['pt_seq_length'][0]), int(gold['rec_length'][0])
     _, (t, mask) = fixture_batch(gold)
     t, mask = t.cuda(), mask.cuda()
@@ -195,7 +168,7 @@ def test_window_prompts_fixture_under_every_knob(golden_dir):
     from tests.test_gpu_omni_prompts import check_against_fixture
     from tests.test_prompts_cpu import prompt_case, prompt_page
     gold = prompt_case(golden_dir)
-    m = omni_model(int(gold['wseed'][0]), float(gold['pt_eos_bias'][0]))
+    m = omni_for(int(gold['wseed'][0]), float(gold['pt_eos_bias'][0]))
     m.vocab.pt_seq_length, m.vocab.rec_length = int(gold['pt_seq_length'][0]), int(gold['rec_length'][0])
     pages = [prompt_page(gold, b) for b in range(2)]
     imgs, masks = torch.cat([p[0] for p in pages]), torch.cat([p[1] for p in pages])
@@ -215,7 +188,7 @@ def test_kie_fixture_under_every_knob(golden_dir):
     from oracle.gen_golden import KIE_CASES, omni_inputs
     case = KIE_CASES['kie']
     gold = np.load(os.path.join(golden_dir, 'omni_kie.npz'))
-    m = omni_model(case['wseed'], case['pt_eos_bias'], vie=case['vie'])
+    m = omni_for(case['wseed'], case['pt_eos_bias'], vie=case['vie'])
     v = m.vocab
     v.pt_seq_length, v.rec_length = case['pt_seq_length'], case['rec_length']
     img, mask = omni_inputs(case)
@@ -235,19 +208,15 @@ def test_kie_fixture_under_every_knob(golden_dir):
 def test_page_encoded_with_one_cta_per_gemm():
     """1024 x 1024 page with every encoder GEMM on one CTA: hundreds of tiles per CTA through the ping-pong loop.
     Memory bit for bit the full grid's."""
-    m = omni_model(0, -30.0)
+    m = omni_for(0, -30.0)
     img = torch.randn(1, 3, 1024, 1024, generator=torch.Generator().manual_seed(1000)).cuda()
-    set_knobs(m.ctx)
     m.encode(img)
     base = m.memory(0)
-    try:
-        set_knobs(m.ctx, enc_grid_cap=1)
+    with options(m.ctx, enc_grid_cap=1):
         t = time.time()
         m.encode(img)
         got = m.memory(0)
         print(f'[coschedule] 1024 x 1024 encode at enc_grid_cap 1: {time.time() - t:.2f} s')
-    finally:
-        set_knobs(m.ctx)
     assert torch.equal(got.view(torch.int32), base.view(torch.int32))
 
 
@@ -282,7 +251,7 @@ def test_contexts_in_flight_with_their_own_knobs():
     each from their own host threads with nothing synchronising them: each context gives its single-context bits"""
     from advancedliteratemachinery_b200 import MGPSTRB200, NestedTensor, OmniParserB200
     from tests.conftest import mgp_sd
-    owner = omni_model(0, -30.0)
+    owner = omni_for(0, -30.0)
     owner.vocab.pt_seq_length, owner.vocab.rec_length = 8, 25
     g = torch.Generator().manual_seed(44)
     pages = torch.randn(2, 3, 96, 128, generator=g)
@@ -305,10 +274,10 @@ def test_contexts_in_flight_with_their_own_knobs():
     try:
         single = []
         for j in range(5):
-            set_knobs((omni + mgp)[j].ctx)
             single.append(work(j))
         for j in range(5):
-            set_knobs((omni + mgp)[j].ctx, **knobs[j])
+            for k, v in knobs[j].items():
+                (omni + mgp)[j].ctx.set_option(k, v)
         results = [[None, None] for _ in range(5)]
         errors = []
 
@@ -341,7 +310,7 @@ def test_settings_end_with_the_call_and_the_caller_stream_is_restored(golden_dir
     context enqueues on S again), and the results equal a fresh context's bit for bit."""
     from advancedliteratemachinery_b200 import AlmError, NestedTensor, OmniParserB200, OmniVocab
     from oracle.gen_golden import OMNI_CASES, omni_inputs
-    owner = omni_model(0, -30.0)
+    owner = omni_for(0, -30.0)
     S = torch.cuda.Stream()
     v = OmniVocab(pt_seq_length=8, rec_length=25)
     m = OmniParserB200(None, v, stream=S.cuda_stream, workspace_mb=2048, share_from=owner)
@@ -351,7 +320,8 @@ def test_settings_end_with_the_call_and_the_caller_stream_is_restored(golden_dir
     try:
         want = fresh.forward_batch(NestedTensor(page, None))
         want_mem = fresh.memory(0)
-        set_knobs(m.ctx, enc_grid_cap=7, dec_grid_cap=5, decode_priority=1)
+        for k, v in dict(enc_grid_cap=7, dec_grid_cap=5, decode_priority=1).items():
+            m.ctx.set_option(k, v)
         img, mask = omni_inputs(OMNI_CASES['oddlen'])
         m.vocab.pt_seq_length = 1024
         with pytest.raises(AlmError, match='position table'):

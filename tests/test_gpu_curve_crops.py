@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_curve_crops_cpu import build_emu, curve_fixture, curve_regions, emu_curve_crops
+from tests.support import emu
+from tests.test_curve_crops_cpu import bind, curve_fixture, curve_regions, emu_curve_crops
 from tests.test_quad_crops_cpu import quad_fixture
 
 pytestmark = pytest.mark.gpu
@@ -27,7 +28,7 @@ def test_thousand_curved_regions_equal_host_emulation():
     """16 pages of 1024 x 1024, 64 curved regions each: every output bit equals the host run of the kernel bodies."""
     from advancedliteratemachinery_b200 import _lib, preprocess as P
     pages, polys, pidx = curve_regions(seed=7)
-    _, _, ref = emu_curve_crops(build_emu(), pages, polys, pidx)
+    _, _, ref = emu_curve_crops(emu('curve_emu', bind), pages, polys, pidx)
     ctx = _lib.Context(0)
     got = P.curve_crops(ctx, [torch.from_numpy(p).cuda() for p in pages], polys, pidx)
     assert np.array_equal(got.cpu().numpy().view(np.uint32), ref.view(np.uint32))

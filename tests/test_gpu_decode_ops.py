@@ -18,59 +18,18 @@ shapes where its schedule changes and at the edges of its arithmetic:
 Every output buffer is followed by a guard region that must come back bit for bit unchanged.  Shapes that depend on the
 schedule are derived from the SM count, so the cases hold on any H100.
 """
-import contextlib
 import ctypes as C
 
 import pytest
 import torch
 
+from tests.support import NAN, assert_guard, bits, ctx, guarded, options, sms
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
-GUARD = 1024
-NAN = float('nan')
+WORKSPACE_MB = 8192  # the largest cross-attention case builds 3.2 GB of caches
 ERR_INVALID, ERR_UNSUPPORTED = -1, -5
-DEFAULTS = {'nsplit': 3, 'xattn_impl': 0, 'xattn_wg': 1, 'xattn_ctas_per_sm': 2, 'sattn_wide': 1}
-
-
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 8192)  # the largest cross-attention case builds 3.2 GB of caches
-    yield c
-    c.close()
-
-
-@contextlib.contextmanager
-def options(ctx, **kw):
-    try:
-        for k, v in kw.items():
-            ctx.set_option(k, v)
-        yield
-    finally:
-        for k in kw:
-            ctx.set_option(k, DEFAULTS[k])
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _guarded(n, dtype=torch.float32, fill=NAN):
-    """(first n elements, whole buffer) of a device buffer with GUARD elements of `fill` after it"""
-    full = torch.full((n + GUARD,), fill, dtype=dtype, device='cuda')
-    return full[:n], full
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _assert_guard(full, n, fill=NAN):
-    g = full[n:]
-    assert torch.equal(_bits(g), _bits(torch.full_like(g, fill))), 'write past the end of the output'
 
 
 def _ptr(t):
@@ -169,10 +128,10 @@ def _xattn_ref(q, k, v, kpm, img0):
 def _run_xattn(ctx, q, k, v, kpm, img0, M, dl, q_split, launches):
     nimg, ncap = q.shape[0], q.shape[1]
     n = nimg * ncap * 512
-    out, full = _guarded(n)
+    out, full = guarded(n)
     ctx.check(_op(ctx, 'alm_op_cross_attention', q.data_ptr(), k.data_ptr(), v.data_ptr(), _ptr(kpm), out.data_ptr(),
                   k.shape[0], img0, nimg, ncap, M, dl, q_split, launches))
-    _assert_guard(full, n)
+    assert_guard(full, n)
     return out.view(nimg, ncap, 512).clone()
 
 
@@ -181,7 +140,7 @@ def test_cross_attention_matches_fp64(ctx, case):
     impl, nsplit, wg, cps, q_split, ncap, M, imgs, mask = case
     if imgs == 'wide':
         nqb = (ncap + 63) // 64
-        nimg = -(-2 * _sms() // (8 * nqb)) + 1
+        nimg = -(-2 * sms() // (8 * nqb)) + 1
         imgs = (nimg + 1, 1, nimg)
     total, img0, nimg = imgs
     assert total * M <= 65536
@@ -200,7 +159,7 @@ def test_cross_attention_matches_fp64(ctx, case):
             err = float((got.double() - ref).abs().max() / ref.abs().max())
             assert err <= tol, (dl, err)
         again = _run_xattn(ctx, q, k, v, kpm, img0, M, 11, q_split, 2)   # replay on the same partials / counters
-        assert torch.equal(_bits(again), _bits(got))
+        assert torch.equal(bits(again), bits(got))
 
 
 def test_cross_attention_argument_errors(ctx):
@@ -227,7 +186,7 @@ def test_cross_attention_argument_errors(ctx):
 
 # ----------------------------------------------------------------------------------------------- self-attention step
 def _s_values():
-    last_wide = 4 * _sms() // 8                 # the wide kernel serves 8 S <= 4 SMs
+    last_wide = 4 * sms() // 8                 # the wide kernel serves 8 S <= 4 SMs
     return {'1': 1, '16': 16, 'last_wide': last_wide, 'first_narrow': last_wide + 1, '300': 300}
 
 
@@ -255,23 +214,23 @@ def test_self_attention_step_matches_fp64(ctx, S_name, wide):
                 K[1::3, 0] = -120 * unit[1::3]
             qkv[:, 512:1024] = K[:, t]
             n = S * Tmax * 512
-            kc, kfull = _guarded(n)
-            vc, vfull = _guarded(n)
+            kc, kfull = guarded(n)
+            vc, vfull = guarded(n)
             kc.view(S, Tmax, 512)[:, :t] = K[:, :t]
             vc.view(S, Tmax, 512)[:, :t] = V[:, :t]
             kbefore, vbefore = kc.clone(), vc.clone()
-            out, ofull = _guarded(S * 512)
+            out, ofull = guarded(S * 512)
             ctx.check(_op(ctx, 'alm_op_self_attention_step', qkv.data_ptr(), kc.data_ptr(), vc.data_ptr(),
                           out.data_ptr(), S, t, Tmax))
             for full in (kfull, vfull):
-                _assert_guard(full, n)
+                assert_guard(full, n)
             for after, before, new in ((kc, kbefore, qkv[:, 512:1024]), (vc, vbefore, qkv[:, 1024:])):
                 a, b = after.view(S, Tmax, 512), before.view(S, Tmax, 512)
-                assert torch.equal(_bits(a[:, t].contiguous()), _bits(new.contiguous())), (t, Tmax)
+                assert torch.equal(bits(a[:, t].contiguous()), bits(new.contiguous())), (t, Tmax)
                 keep = torch.ones(Tmax, dtype=torch.bool, device='cuda')
                 keep[t] = False
-                assert torch.equal(_bits(a[:, keep].contiguous()), _bits(b[:, keep].contiguous())), (t, Tmax)
-            _assert_guard(ofull, S * 512)
+                assert torch.equal(bits(a[:, keep].contiguous()), bits(b[:, keep].contiguous())), (t, Tmax)
+            assert_guard(ofull, S * 512)
             qd = qkv[:, :512].double().view(S, 8, 64) / 8
             Kd, Vd = K.double().view(S, t + 1, 8, 64), V.double().view(S, t + 1, 8, 64)
             p = torch.einsum('shd,sjhd->shj', qd, Kd).softmax(-1)
@@ -284,11 +243,11 @@ def test_self_attention_step_matches_fp64(ctx, S_name, wide):
 
 # ----------------------------------------------------------------------------------------------- GEMV
 def _gemv(ctx, x, x2, n_split, W, b, resid, M, N, K, act, ln_g=None, ln_b=None, pos=None, pos_split=0):
-    out, full = _guarded(M * N)
+    out, full = guarded(M * N)
     rc = _op(ctx, 'alm_op_gemv', x.data_ptr(), _ptr(x2), n_split, W.data_ptr(), _ptr(b), _ptr(resid), out.data_ptr(), M,
              N, K, act, _ptr(ln_g), _ptr(ln_b), _ptr(pos), pos_split)
     ctx.check(rc)
-    _assert_guard(full, M * N)
+    assert_guard(full, M * N)
     return out.view(M, N).clone()
 
 
@@ -347,7 +306,7 @@ def test_gemv_matches_fp64(ctx, M, K):
         for pos_split in (0, 1024, 1 << 30):
             fused = _gemv(ctx, xr, None, 1 << 30, W, b, None, M, N, 512, 2, gam, bet, pos, pos_split)
             plain = _gemv(ctx, lnp, ln, pos_split, W, b, None, M, N, 512, 2)
-            assert torch.equal(_bits(fused), _bits(plain)), (N, pos_split)
+            assert torch.equal(bits(fused), bits(plain)), (N, pos_split)
             ref, mag = _split_dot(ln64 + pos.double(), ln64, pos_split, W)
             _assert_close_to_terms(fused, torch.relu(ref + b.double()), mag + b.double().abs(), ('ln', N, pos_split))
 
@@ -356,7 +315,7 @@ def test_gemv_argument_errors(ctx):
     x = torch.zeros(40 * 1024, device='cuda')
     W = torch.zeros(8 * 1024, device='cuda')
     g = torch.ones(1024, device='cuda')
-    out, full = _guarded(40 * 8)
+    out, full = guarded(40 * 8)
 
     def call(M, K, ln=False):
         return _op(ctx, 'alm_op_gemv', x.data_ptr(), None, 1 << 30, W.data_ptr(), None, None, out.data_ptr(), M, 8, K,
@@ -367,7 +326,7 @@ def test_gemv_argument_errors(ctx):
     assert call(4, 1024, ln=True) == ERR_INVALID
     assert call(4, 256, ln=True) == ERR_INVALID
     assert torch.isnan(out).all()               # nothing was launched
-    _assert_guard(full, 40 * 8)
+    assert_guard(full, 40 * 8)
 
 
 # ----------------------------------------------------------------------------------------------- token selection
@@ -450,12 +409,12 @@ def test_head_select_matches_reference_rule(ctx, case):
     logits = _head_rows(allowed, nsoft, V, g)
     S = logits.shape[0]
     cfg = _lib.DecodeCfg(NB, PT_EOS, POLY_EOS, REC_EOS, PT_SOS, 1101, 1102, RECOG_PAD, 1024, 25, 32, vie, 512)
-    token, tfull = _guarded(S, torch.int32, -7)
-    prob, pfull = _guarded(S)
+    token, tfull = guarded(S, torch.int32, -7)
+    prob, pfull = guarded(S)
     fin0 = (torch.arange(S) % 4 == 3).int()
     ntok0 = torch.full((S,), 3, dtype=torch.int32)
-    fin, ffull = _guarded(S, torch.int32, -7)
-    ntok, nfull = _guarded(S, torch.int32, -7)
+    fin, ffull = guarded(S, torch.int32, -7)
+    ntok, nfull = guarded(S, torch.int32, -7)
     fin.copy_(fin0)
     ntok.copy_(ntok0)
     track = phase == 0        # EOS bookkeeping runs in the point loop
@@ -464,7 +423,7 @@ def test_head_select_matches_reference_rule(ctx, case):
                   token.data_ptr(), prob.data_ptr(), fin.data_ptr() if track else None,
                   ntok.data_ptr() if track else None))
     for full, fill in ((tfull, -7), (pfull, NAN), (ffull, -7), (nfull, -7)):
-        _assert_guard(full, S, fill)
+        assert_guard(full, S, fill)
     cand = logits.masked_fill(~allowed, float('-inf'))
     best = cand.max(-1, keepdim=True).values
     want = (cand == best).int().argmax(-1)                  # the lowest id among the maxima

@@ -34,6 +34,8 @@ import time
 import pytest
 import torch
 
+from tests.support import options
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
@@ -56,10 +58,8 @@ def _file_clock():
 
 
 def _close_models():
-    from tests.test_gpu_omniparser import _MODELS
-    for d in (_MODEL, _MODELS):
-        for k in list(d):
-            d.pop(k).ctx.close()
+    for k in list(_MODEL):
+        _MODEL.pop(k).ctx.close()
 
 
 def _model(key, sd, vocab=None, workspace_mb=8192):
@@ -215,10 +215,9 @@ def test_teacher_forced_logits_against_fp64(page):
     if page == 'pos1023':
         _assert_large_self_attention_scores(sd, m.vocab)
     report, worst = {}, 0.0
-    try:
-        for nsplit in spec['nsplit']:
-            m.ctx.set_option('nsplit', nsplit)
-            m.ctx.set_option('xattn_impl', 1)   # the unfused path's V_c^T is built by the encode; 0 and 2 ignore it
+    for nsplit in spec['nsplit']:
+        # xattn_impl 1 for the encode: the unfused path's V_c^T is built by the encode; 0 and 2 ignore it
+        with options(m.ctx, nsplit=nsplit, xattn_impl=1):
             image, mem, pos, kpm = _encode(m, spec['enc'])
             for kind, length, ns in spec['cases']:
                 seq = tf_seqs(m.vocab, kind, max(ns), length, seed=length + len(kind))
@@ -230,9 +229,6 @@ def test_teacher_forced_logits_against_fp64(page):
                         r = worst_ratio(got, f64[:n], f32[:n], nsplit)
                         report[f'{kind} n{n} x{impl} s{nsplit}'] = round(r, 4)
                         worst = max(worst, r)
-    finally:
-        m.ctx.set_option('xattn_impl', 0)
-        m.ctx.set_option('nsplit', 3)
     print(f'{page}: worst err/bound {worst:.4f} ({time.time() - t0:.1f} s)', json.dumps(report))
     bad = {k: r for k, r in report.items() if r > 1.0}
     assert not bad, bad

@@ -12,8 +12,8 @@ import pytest
 import torch
 
 from oracle import dense_ref as D
+from tests.support import assert_same, omni_model, release_models
 from tests.test_dense_cpu import emu_merge_readings, fabricate
-from tests.test_tiles_cpu import assert_same
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
@@ -21,29 +21,11 @@ torch.set_grad_enabled(False)
 ALM_ERR_INVALID = -1  # include/alm_ocr.h
 PROB_RTOL = 5e-5  # the poly / rec loops at another batch shape: probabilities differ in the last bits, ids not at all
 
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
 
 def model(bias, pt_seq_length=12, workspace_mb=8192):
     """A synthetic checkpoint (seed 0) with pt_eos_bias `bias`; one resident at a time."""
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    key = (bias, workspace_mb)
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(omni_sd(0, bias), OmniVocab(), workspace_mb=workspace_mb)
-    m = _MODELS[key]
-    m.vocab.pt_seq_length = pt_seq_length
-    m.vocab.rec_length = 25
-    return m
+    return omni_model(dict(wseed=0, pt_eos_bias=bias, pt_seq_length=pt_seq_length, rec_length=25),
+                      workspace_mb=workspace_mb)
 
 
 def pages(n, size=64, seed=0):

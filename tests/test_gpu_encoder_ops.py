@@ -18,61 +18,18 @@ Every output buffer is followed by a guard region that must come back bit for bi
 must not read holds NaN.  Wherever a kernel writes a split pair it must be hi = bf16_rn(x), lo = bf16_rn(x - hi) of the
 fp32 value it writes (or would write).  Shapes that depend on the schedule are derived from the SM count.
 """
-import contextlib
-import math
-
 import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.support import NAN, assert_guard, bits, ctx, guarded, options, sms
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
-GUARD = 1024
-NAN = float('nan')
+WORKSPACE_MB = 4096
 ERR_INVALID, ERR_UNSUPPORTED = -1, -5
-DEFAULTS = {'nsplit': 3, 'wattn_impl': 3}
 U32 = 2.0 ** -24        # fp32 unit roundoff
-
-
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 4096)
-    yield c
-    c.close()
-
-
-@contextlib.contextmanager
-def options(ctx, **kw):
-    try:
-        for k, v in kw.items():
-            ctx.set_option(k, v)
-        yield
-    finally:
-        for k in kw:
-            ctx.set_option(k, DEFAULTS[k])
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _guarded(n, dtype=torch.float32, fill=NAN):
-    """(first n elements, whole buffer) of a device buffer with GUARD elements of `fill` after it"""
-    full = torch.full((n + GUARD,), fill, dtype=dtype, device='cuda')
-    return full[:n], full
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _assert_guard(full, n, fill=NAN):
-    g = full[n:]
-    assert torch.equal(_bits(g), _bits(torch.full_like(g, fill))), 'write past the end of the output'
 
 
 def _ptr(t):
@@ -88,7 +45,7 @@ def _op(ctx, name, *args):
 
 def _planes(n):
     """a bf16 (hi, lo) output pair as int16 bit buffers prefilled with 0xffff (a NaN), each with a guard"""
-    return _guarded(n, torch.int16, -1), _guarded(n, torch.int16, -1)
+    return guarded(n, torch.int16, -1), guarded(n, torch.int16, -1)
 
 
 def _assert_split(hi, lo, x, what=''):
@@ -150,9 +107,9 @@ def _nearest_map_ref(B, H, W):
 
 def _swin_map(ctx, kind, B, H, W, shift):
     n = {0: B * -(-H // 7) * -(-W // 7) * 49, 1: B * ((H + 1) // 2) * ((W + 1) // 2) * 4, 2: B * H * W}[kind]
-    m, full = _guarded(n, torch.int32, -7)
+    m, full = guarded(n, torch.int32, -7)
     ctx.check(_op(ctx, 'alm_op_swin_map', kind, B, H, W, shift, m.data_ptr()))
-    _assert_guard(full, n, -7)
+    assert_guard(full, n, -7)
     return m
 
 
@@ -191,7 +148,7 @@ def _run_gather(ctx, src, map_, nsrc, Cs, rows, gamma=None, beta=None, zero_miss
     bufs = {}
     for name in outs:
         f32 = name.startswith('f32')
-        bufs[name] = _guarded(rows * (ldo_f32 if f32 else ldo_bf), torch.float32 if f32 else torch.int16,
+        bufs[name] = guarded(rows * (ldo_f32 if f32 else ldo_bf), torch.float32 if f32 else torch.int16,
                               NAN if f32 else -1)
 
     def p(k):
@@ -202,11 +159,11 @@ def _run_gather(ctx, src, map_, nsrc, Cs, rows, gamma=None, beta=None, zero_miss
     res = {}
     for k, (buf, full) in bufs.items():
         fill = NAN if k.startswith('f32') else -1
-        _assert_guard(full, buf.numel(), fill)
+        assert_guard(full, buf.numel(), fill)
         v = buf.view(rows, -1)
         if v.shape[1] > C:
             gap = v[:, C:]
-            assert torch.equal(_bits(gap), _bits(torch.full_like(gap, fill))), (k, 'wrote past the row width')
+            assert torch.equal(bits(gap), bits(torch.full_like(gap, fill))), (k, 'wrote past the row width')
         res[k] = v[:, :C].contiguous()
     return res
 
@@ -234,7 +191,7 @@ def _check_gather(ctx, res, ref, tol, args, kwargs, dead=None):
         _assert_split(res['hi2'], res['lo2'], res['f322'], 'out2')
     if dead is not None and bool(dead.any()):
         for k, v in res.items():
-            assert not bool(_bits(v[dead]).any()), (k, 'a pad row is not +0')
+            assert not bool(bits(v[dead]).any()), (k, 'a pad row is not +0')
     split_only = _run_gather(ctx, *args, **kwargs, outs=('hi', 'lo'))
     assert torch.equal(split_only['hi'], res['hi']) and torch.equal(split_only['lo'], res['lo'])
 
@@ -305,8 +262,8 @@ def test_gather_ln_memory_plus_pos(ctx):
     kw = dict(add=pos, ldo_f32=C + 4, ldo_bf=C + 8)
     res = _run_gather(ctx, *args, **kw)
     m32, p32 = mem[:, :C], pos[:, :C]
-    assert torch.equal(_bits(res['f32']), _bits(m32.contiguous()))
-    assert torch.equal(_bits(res['f322']), _bits((m32 + p32).contiguous()))
+    assert torch.equal(bits(res['f32']), bits(m32.contiguous()))
+    assert torch.equal(bits(res['f322']), bits((m32 + p32).contiguous()))
     _assert_split(res['hi'], res['lo'], m32, 'memory')
     _assert_split(res['hi2'], res['lo2'], m32 + p32, 'memory + pos')
     enc = _run_gather(ctx, *args, add=pos, outs=('hi', 'lo', 'hi2', 'lo2'))   # the encoder's form: split pairs only
@@ -346,7 +303,7 @@ def test_patch_im2col_exact(ctx, name):
     from oracle import omniparser_ref as O
     B, H, W, Hc, Wc, n_canvas, slots = IM2COL_CASES[name]
     gen = torch.Generator(device='cuda').manual_seed(H * W)
-    canvas, _ = _guarded(n_canvas * 3 * Hc * Wc)
+    canvas, _ = guarded(n_canvas * 3 * Hc * Wc)
     canvas = canvas.view(n_canvas, 3, Hc, Wc)
     order = slots if slots is not None else list(range(B))
     for s in order:     # NaN everywhere outside each image's H x W, and in the unused slot
@@ -361,8 +318,8 @@ def test_patch_im2col_exact(ctx, name):
         (hi, hfull), (lo, lfull) = _planes(n)
         ctx.check(_op(ctx, 'alm_op_patch_im2col', canvas.data_ptr(), n_canvas, Hc, Wc, _ptr(d_slots), B, H, W,
                       hi.data_ptr(), lo.data_ptr() if with_lo else None))
-        _assert_guard(hfull, n, -1)
-        _assert_guard(lfull, n, -1)
+        assert_guard(hfull, n, -1)
+        assert_guard(lfull, n, -1)
         if with_lo:
             _assert_split(hi, lo, ref, name)
         else:
@@ -381,15 +338,15 @@ def test_fpn_assemble_matches_fp64(ctx, B, H, W):
     gen = torch.Generator(device='cuda').manual_seed(H + W)
     levels = []
     for hs, ws in grids:
-        buf, _ = _guarded(B * hs * ws * 256)     # NaN past the end of every level
+        buf, _ = guarded(B * hs * ws * 256)     # NaN past the end of every level
         buf.copy_(torch.randn(B * hs * ws * 256, generator=gen, device='cuda'))
         levels.append(buf.view(B, hs, ws, 256))
     mh, mw = grids[2]
     n = B * mh * mw * 1024
     (hi, hfull), (lo, lfull) = _planes(n)
     ctx.check(_op(ctx, 'alm_op_fpn_assemble', *[p.data_ptr() for p in levels], B, H, W, hi.data_ptr(), lo.data_ptr()))
-    _assert_guard(hfull, n, -1)
-    _assert_guard(lfull, n, -1)
+    assert_guard(hfull, n, -1)
+    assert_guard(lfull, n, -1)
     for s, (err, tol) in enumerate(_fpn_err_tol(hi, lo, levels, grids)):
         assert bool((err <= tol).all()), (s, float(err.max()))
 
@@ -433,12 +390,12 @@ def _sine_masks(kind, B, H, W, gen):
 
 def _sine_pos(ctx, mask, B, H, W, h, w):
     n = B * h * w
-    pos, pfull = _guarded(n * 512)
-    kpm, kfull = _guarded(n, torch.uint8, 7)
+    pos, pfull = guarded(n * 512)
+    kpm, kfull = guarded(n, torch.uint8, 7)
     d_mask = mask.cuda() if mask is not None else None
     rc = _op(ctx, 'alm_op_sine_pos', _ptr(d_mask), B, H, W, h, w, pos.data_ptr(), kpm.data_ptr())
-    _assert_guard(pfull, n * 512)
-    _assert_guard(kfull, n, 7)
+    assert_guard(pfull, n * 512)
+    assert_guard(kfull, n, 7)
     return rc, pos, kpm
 
 
@@ -497,7 +454,7 @@ def test_softmax_rows_matches_fp64(ctx, n, masked):
             for i in range(2):                                                # the row maximum in a masked column
                 j = int(kpm[i].nonzero()[0])
                 s[i * rpm:(i + 1) * rpm, j] = s[:, :n].max() + 30
-    out, ofull = _guarded(rows * ldo)
+    out, ofull = guarded(rows * ldo)
     (hi, hfull), (lo, lfull) = _planes(rows * ldo)
 
     def run(f32, hi_, lo_):
@@ -505,7 +462,7 @@ def test_softmax_rows_matches_fp64(ctx, n, masked):
                       _ptr(lo_), ldo))
     run(out, hi, lo)
     for full, fill in ((ofull, NAN), (hfull, -1), (lfull, -1)):
-        _assert_guard(full, rows * ldo, fill)
+        assert_guard(full, rows * ldo, fill)
     o, h, l = out.view(rows, ldo), hi.view(rows, ldo), lo.view(rows, ldo)
     assert bool(torch.isnan(o[:, n:]).all()) and bool((h[:, n:] == -1).all()) and bool((l[:, n:] == -1).all()), \
         'columns n..ldo-1 written'
@@ -522,7 +479,7 @@ def test_softmax_rows_matches_fp64(ctx, n, masked):
     err = (got.double() - ref).abs()
     assert bool((err <= ref * rel + 2.0 ** -126).all()), float((err / (ref * rel + 2.0 ** -126)).max())
     if kpm is not None:
-        assert not bool(_bits(got)[ref == 0].any()), 'a masked column is not +0'
+        assert not bool(bits(got)[ref == 0].any()), 'a masked column is not +0'
     _assert_split(h[:, :n].contiguous(), l[:, :n].contiguous(), got, 'P')
     (hi2, _), (lo2, _) = _planes(rows * ldo)
     run(None, hi2, lo2)
@@ -531,7 +488,7 @@ def test_softmax_rows_matches_fp64(ctx, n, masked):
 
 # ----------------------------------------------------------------------------------------------- window attention
 def _nslots(heads, n_win):
-    return max(1, min(n_win, _sms() // (heads // 2)))
+    return max(1, min(n_win, sms() // (heads // 2)))
 
 
 def _ring(ns, B, nWh):
@@ -564,7 +521,7 @@ def _wattn_inputs(B, nWh, nWw, heads, shift, seed):
     gen = torch.Generator(device='cuda').manual_seed(seed)
     nW = B * nWh * nWw
     rows = nW * 49
-    buf, _ = _guarded(rows * 3 * C)            # NaN past the last row
+    buf, _ = guarded(rows * 3 * C)            # NaN past the last row
     qkv = buf.view(rows, 3 * C)
     qkv.copy_(torch.randn(rows, 3 * C, generator=gen, device='cuda'))
     qkv[:, :2 * C] *= 10 ** 0.5
@@ -596,12 +553,12 @@ def _wattn_tol(qkv, heads, B, nWh, nWw, scale=32 ** -0.5):
 def _run_wattn(ctx, qkv, tab, B, nWh, nWw, heads, shift, f32=True):
     rows, C = qkv.shape[0], heads * 32
     n = rows * C
-    out, ofull = _guarded(n)
+    out, ofull = guarded(n)
     (hi, hfull), (lo, lfull) = _planes(n)
     ctx.check(_op(ctx, 'alm_op_window_attention_ex', qkv.data_ptr(), tab.data_ptr(), out.data_ptr() if f32 else None,
                   hi.data_ptr(), lo.data_ptr(), B, nWh, nWw, C, heads, shift))
     for full, fill in ((ofull, NAN), (hfull, -1), (lfull, -1)):
-        _assert_guard(full, n, fill)
+        assert_guard(full, n, fill)
     if not f32:
         assert bool(torch.isnan(out).all()), 'fp32 output written without one'
     return out.view(rows, C), hi, lo
@@ -618,7 +575,7 @@ def _qkv_planes(qkv, C):
     h = x.to(torch.bfloat16)
     planes = []
     for p in (h, (x - h.float()).to(torch.bfloat16)):
-        buf, _ = _guarded(x.numel(), torch.int16, -1)
+        buf, _ = guarded(x.numel(), torch.int16, -1)
         buf.copy_(p.view(torch.int16).flatten())
         planes.append(buf)
     return planes
@@ -627,12 +584,12 @@ def _qkv_planes(qkv, C):
 def _run_wattn_planes(ctx, planes, tab, B, nWh, nWw, heads, shift, f32=True):
     rows, C = planes[0].numel() // (3 * heads * 32), heads * 32
     n = rows * C
-    out, ofull = _guarded(n)
+    out, ofull = guarded(n)
     (hi, hfull), (lo, lfull) = _planes(n)
     ctx.check(_op(ctx, 'alm_op_window_attention_planes', planes[0].data_ptr(), planes[1].data_ptr(), tab.data_ptr(),
                   out.data_ptr() if f32 else None, hi.data_ptr(), lo.data_ptr(), B, nWh, nWw, C, heads, shift))
     for full, fill in ((ofull, NAN), (hfull, -1), (lfull, -1)):
-        _assert_guard(full, n, fill)
+        assert_guard(full, n, fill)
     if not f32:
         assert bool(torch.isnan(out).all()), 'fp32 output written without one'
     return out.view(rows, C), hi, lo
@@ -675,7 +632,7 @@ def test_window_attention_ex_matches_fp64(ctx, name):
     if 'ring' in name:
         assert n_win >= 3 * ns and n_win % ns != 0, (n_win, ns)
     if 'below' in name:
-        assert n_win < _sms() // (heads // 2)
+        assert n_win < sms() // (heads // 2)
     _check_wattn(ctx, B, nWh, nWw, heads, shift, seed=n_win + heads)
 
 

@@ -20,6 +20,8 @@ checked on every call (hi == bf16_rn(f32), lo == bf16_rn(f32 - hi)).
 import pytest
 import torch
 
+from tests import support
+from tests.support import ctx, options
 from tests.test_gpu_gemm_operands import (GUARD, NAN_F32, Case, Opd, _call, _check, _epilogue, _launch_shape,
                                           _outputs, _r8, _run, _setup)
 
@@ -33,20 +35,11 @@ MAX_STAGES = 16
 WORST = {}  # (tile width, nsplit) -> worst err / bound
 
 
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 1024)
-    yield c
+@pytest.fixture(scope='module', autouse=True)
+def _report():
+    yield
     print('[gemm capped] worst err/bound: ' + ', '.join(
         f'{bn}-column tiles nsplit {ns}: {r:.3g}' for (bn, ns), r in sorted(WORST.items())))
-    c.close()
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def _stages(M, bn, nsplit):
@@ -87,30 +80,26 @@ def _assert_same(base, got, label):
 
 
 def _record(c, nsplit, worst):
-    bn = _launch_shape(c.M, c.N, c.nb0 * c.nb1, _sms())[0]
+    bn = _launch_shape(c.M, c.N, c.nb0 * c.nb1, support.sms())[0]
     WORST[(bn, nsplit)] = max(WORST.get((bn, nsplit), 0.0), worst)
 
 
 def _capped(ctx, name, c, nsplit, seed, caps=None):
     """c uncapped against fp64, then under every cap bit for bit against the uncapped outputs; returns the worst
     err / bound"""
-    sms = _sms()
+    sms = support.sms()
     tiles = _tiles(c.M, c.N, _launch_shape(c.M, c.N, c.nb0 * c.nb1, sms)[0], c.nb0 * c.nb1)
     assert tiles <= 2 * sms, f'{name}: {tiles} tiles, the cap applies to <= {2 * sms}'
     _setup(c, seed)
     if nsplit == 1:
         c.a.poison_lo()
         c.b.poison_lo()
-    try:
-        ctx.set_option('small_grid_cap', 0)
+    with options(ctx, small_grid_cap=0):
         base = _run(ctx, c, nsplit, 0)
-        worst = _check(c, base, nsplit, 0, f'{name} nsplit {nsplit} uncapped')
-        for cap in caps or _caps(tiles, sms):
-            ctx.set_option('small_grid_cap', cap)
+    worst = _check(c, base, nsplit, 0, f'{name} nsplit {nsplit} uncapped')
+    for cap in caps or _caps(tiles, sms):
+        with options(ctx, small_grid_cap=cap):
             _assert_same(base, _run(ctx, c, nsplit, 0), f'{name} nsplit {nsplit} small_grid_cap {cap}')
-    finally:
-        ctx.set_option('small_grid_cap', 0)
-        ctx.set_option('nsplit', 3)
     _record(c, nsplit, worst)
     return worst
 
@@ -137,7 +126,7 @@ SHAPES = {'narrow': _narrow_shape, 'wide': _wide_shape}
 def test_the_cases_reach_every_schedule_property():
     """odd and even tile counts per CTA, grids where some CTAs have one tile more, cooperative and ping-pong launches,
     and every residue of k_blocks mod the ring depth"""
-    sms = _sms()
+    sms = support.sms()
     for width, shape in SHAPES.items():
         M, N = shape(sms)
         bn = 32 if width == 'narrow' else 128
@@ -158,7 +147,7 @@ def test_the_cases_reach_every_schedule_property():
 def test_k_blocks_around_the_ring_depth(ctx, width, nsplit):
     """every residue of k_blocks mod the stage count: consumer 1's skip over the other consumer's tiles must land on
     the right stage and phase after many tiles"""
-    M, N = SHAPES[width](_sms())
+    M, N = SHAPES[width](support.sms())
     bn = 32 if width == 'narrow' else 128
     for kb in _kbs(_stages(M, bn, nsplit)):
         K = 64 * kb - (24 if kb % 2 == 0 else 0)  # K tails on the even counts
@@ -181,7 +170,7 @@ def test_decoder_token_shapes(ctx, name, nsplit):
     """M = 1 ... 130 rows: tails inside half 0, inside half 1, exactly 64 and 128, and a second row block.  Uncapped
     these run cooperatively (one tile per CTA); every cap runs them ping-pong."""
     N, K, extra = DECODER[name]
-    sms = _sms()
+    sms = support.sms()
     worst = 0.0
     for M in range(1, 131):
         e = dict(ldo=N, **{k: v for k, v in extra.items() if k != 'resid'})
@@ -219,7 +208,7 @@ EPILOGUES = list(_epilogue_cases(132))  # the names only: they do not depend on 
 @pytest.mark.parametrize('nsplit', [3, 1])
 @pytest.mark.parametrize('name', EPILOGUES)
 def test_epilogue_tables_refreshed_on_every_tile(ctx, name, nsplit):
-    c = _epilogue_cases(_sms())[name]()
+    c = _epilogue_cases(support.sms())[name]()
     worst = _capped(ctx, name, c, nsplit, seed=sum(map(ord, name)))
     print(f'[gemm capped] {name} nsplit {nsplit}: worst err/bound {worst:.3g}')
 
@@ -229,7 +218,7 @@ def test_epilogue_tables_refreshed_on_every_tile(ctx, name, nsplit):
 def test_row_maps_and_in_place_residual(ctx, width, nsplit):
     """Row maps (a permutation with dropped rows, residual rows read through their own map) and the in-place residual
     (out_f32 == resid): under every cap, bit for bit the plain call with the rows moved / the residual copied."""
-    sms = _sms()
+    sms = support.sms()
     M, N = SHAPES[width](sms)
     K, ld = 100, _r8(N)
     c = Case(Opd(M, K, _r8(K)), Opd(N, K, _r8(K)), dict(ldo=ld, bias='col', resid=(ld, 0, 0), act=1))
@@ -251,12 +240,11 @@ def test_row_maps_and_in_place_residual(ctx, width, nsplit):
     src = (rows[:, None] * ld + col).reshape(-1)
     dst = (out_map[keep].long()[:, None] * ld + col).reshape(-1)
     tiles = _tiles(M, N, 32 if width == 'narrow' else 128)
-    try:
-        ctx.set_option('small_grid_cap', 0)
+    with options(ctx, small_grid_cap=0):
         base = _run(ctx, c, nsplit, 0)
-        worst = _check(c, base, nsplit, 0, f'{width} plain')
-        for cap in [0] + _caps(tiles, sms):
-            ctx.set_option('small_grid_cap', cap)
+    worst = _check(c, base, nsplit, 0, f'{width} plain')
+    for cap in [0] + _caps(tiles, sms):
+        with options(ctx, nsplit=nsplit, small_grid_cap=cap):
             # row maps
             out = _outputs(c.written.numel())
             e = _epilogue(c, *out)
@@ -275,8 +263,5 @@ def test_row_maps_and_in_place_residual(ctx, width, nsplit):
             n = base[0].numel()
             assert bool((x[n:].view(torch.int32) == NAN_F32).all()), f'{width}: in-place write past the output'
             _assert_same(base, (x[:n], out[1], out[2]), f'{width} nsplit {nsplit} in-place residual, small_grid_cap {cap}')
-    finally:
-        ctx.set_option('small_grid_cap', 0)
-        ctx.set_option('nsplit', 3)
     _record(c, nsplit, worst)
     print(f'[gemm capped] {width} row maps / in place nsplit {nsplit}: worst err/bound {worst:.3g}')

@@ -14,30 +14,20 @@ batched problem.
 import pytest
 import torch
 
+from tests.support import ctx, options, sms
+
 torch.set_grad_enabled(False)
 
 GUARD = 67
+WORKSPACE_MB = 4096
 NAN_BF16 = 0x7fc0
 ALM_ERR_INVALID = -1
-
-
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 4096)
-    return c
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 # name: dict(M, N, K, batch, w_batch, act, alpha, bias ('none' | 'col' | 'row'), resid ('none' | 'plain' | 'map' |
 # 'inplace'), out_map, col_group, out ('f32' | 'split' | 'both'), ldo (None: N))
 def _cases():
-    s = _sms()
+    s = sms()
     return {
         # ping-pong, 128-column tiles, M tail in half 1, N a multiple of 8 only (last chunk partly past N)
         'pingpong_gelu_both': dict(M=(2 * s + 3) * 128 + 70, N=280, K=64, act=1, bias='col', out='both'),
@@ -157,10 +147,10 @@ def _run_case(ctx, c, nsplit):
     bias_d = bias.cuda() if bias is not None else None
     rmap_d = resid_map.cuda() if resid_map is not None else None
     omap_d = orow.to(torch.int32).cuda() if c.get('out_map') else None
-    ctx.set_option('nsplit', nsplit)
-    ctx.check(ctx.lib.alm_op_gemm(ctx.h, Ad.data_ptr(), Wd.data_ptr(), M, N, K, batch, w_batch, ptr(out_f32),
-                                  ptr(out_hi), ptr(out_lo), ldo, obs0, ptr(bias_d), bias_mode, bias_bs0, alpha, act,
-                                  ptr(resid_d), ldr, rbs0, ptr(rmap_d), ptr(omap_d), cg, cstride))
+    with options(ctx, nsplit=nsplit):
+        ctx.check(ctx.lib.alm_op_gemm(ctx.h, Ad.data_ptr(), Wd.data_ptr(), M, N, K, batch, w_batch, ptr(out_f32),
+                                      ptr(out_hi), ptr(out_lo), ldo, obs0, ptr(bias_d), bias_mode, bias_bs0, alpha, act,
+                                      ptr(resid_d), ldr, rbs0, ptr(rmap_d), ptr(omap_d), cg, cstride))
     ref = x[:, live, :]
     written = torch.zeros(size, dtype=torch.bool)
     written[idx_live.reshape(-1)] = True
@@ -189,17 +179,14 @@ def _run_case(ctx, c, nsplit):
 @pytest.mark.parametrize('name', CASES)
 def test_gemm_epilogue_matches_fp64(ctx, name):
     c = _cases()[name]
-    try:
-        for nsplit, tol in ((3, 2e-5), (1, 6e-3)):
-            ref, got = _run_case(ctx, c, nsplit)
-            for kind, v in got.items():
-                v = v.double()
-                assert torch.isfinite(v).all(), (nsplit, kind)
-                rows_err = ((v - ref).norm(dim=2) / (ref.norm(dim=2) + 1e-30)).amax(dim=0)
-                assert float(rows_err.max()) < 10 * tol, (nsplit, kind, int(rows_err.argmax()))
-                assert float((v - ref).norm() / ref.norm()) < tol, (nsplit, kind)
-    finally:
-        ctx.set_option('nsplit', 3)
+    for nsplit, tol in ((3, 2e-5), (1, 6e-3)):
+        ref, got = _run_case(ctx, c, nsplit)
+        for kind, v in got.items():
+            v = v.double()
+            assert torch.isfinite(v).all(), (nsplit, kind)
+            rows_err = ((v - ref).norm(dim=2) / (ref.norm(dim=2) + 1e-30)).amax(dim=0)
+            assert float(rows_err.max()) < 10 * tol, (nsplit, kind, int(rows_err.argmax()))
+            assert float((v - ref).norm() / ref.norm()) < tol, (nsplit, kind)
 
 
 @pytest.mark.gpu

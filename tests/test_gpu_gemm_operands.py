@@ -27,6 +27,9 @@ import random
 import pytest
 import torch
 
+from tests import support
+from tests.support import ctx, options
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
@@ -39,22 +42,8 @@ T, TP, NTOK, G = 257, 264, 27, 8  # MGP-STR: tokens, their padded row stride, A^
 RUNS = ((3, 0), (3, 1), (1, 0), (1, 1))  # (nsplit, gemm_impl)
 
 
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    yield c
-    c.set_option('nsplit', 3)
-    c.set_option('gemm_impl', 0)
-
-
 def _r8(x):
     return (x + 7) // 8 * 8
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def _launch_shape(M, N, nb, sms):
@@ -201,11 +190,10 @@ def _call(ctx, a, b, e):
 
 
 def _run(ctx, c, nsplit, impl):
-    ctx.set_option('nsplit', nsplit)
-    ctx.set_option('gemm_impl', impl)
-    out = _outputs(c.written.numel())
-    lo = not (nsplit == 1 and c.lo_null)
-    ctx.check(_call(ctx, c.a.desc(lo), c.b.desc(lo), _epilogue(c, *out)))
+    with options(ctx, nsplit=nsplit, gemm_impl=impl):
+        out = _outputs(c.written.numel())
+        lo = not (nsplit == 1 and c.lo_null)
+        ctx.check(_call(ctx, c.a.desc(lo), c.b.desc(lo), _epilogue(c, *out)))
     return out
 
 
@@ -281,16 +269,12 @@ def _check(c, out, nsplit, impl, label):
 def _run_case(ctx, name, c, seed):
     _setup(c, seed)
     worst = {}
-    try:
-        for nsplit, impl in RUNS:
-            if nsplit == 1:
-                c.a.poison_lo()
-                c.b.poison_lo()
-            label = f'{name} nsplit={nsplit} gemm_impl={impl}'
-            worst[(nsplit, impl)] = _check(c, _run(ctx, c, nsplit, impl), nsplit, impl, label)
-    finally:
-        ctx.set_option('nsplit', 3)
-        ctx.set_option('gemm_impl', 0)
+    for nsplit, impl in RUNS:
+        if nsplit == 1:
+            c.a.poison_lo()
+            c.b.poison_lo()
+        label = f'{name} nsplit={nsplit} gemm_impl={impl}'
+        worst[(nsplit, impl)] = _check(c, _run(ctx, c, nsplit, impl), nsplit, impl, label)
     print(f'[gemm operands] {name}: worst err/bound ' + ', '.join(
         f'nsplit {ns} impl {im}: {r:.3g}' for (ns, im), r in worst.items()))
     return worst
@@ -440,11 +424,11 @@ def _random_case(i, sms):
 
 @pytest.mark.parametrize('i', range(N_RANDOM))
 def test_random_geometry_matches_fp64(ctx, i):
-    _run_case(ctx, f'random_{i}', _random_case(i, _sms()), seed=1000 + i)
+    _run_case(ctx, f'random_{i}', _random_case(i, support.sms()), seed=1000 + i)
 
 
 def test_random_geometry_reaches_both_tile_widths_and_schedules():
-    sms = _sms()
+    sms = support.sms()
     seen = set()
     for i in range(N_RANDOM):
         c = _random_case(i, sms)
@@ -473,16 +457,16 @@ SLICES = {
 @pytest.mark.parametrize('name', list(SLICES))
 def test_slice_of_a_batched_launch_equals_the_unbatched_call(ctx, name):
     c = SLICES[name]()
-    sms = _sms()
+    sms = support.sms()
     assert _launch_shape(c.M, c.N, c.nb0 * c.nb1, sms)[0] == _launch_shape(c.M, c.N, 1, sms)[0], \
         'the case must give both launches the same tile width'
     _setup(c, seed=sum(map(ord, name)))
-    try:
-        for nsplit, impl in RUNS:
-            if nsplit == 1:
-                c.a.poison_lo()
-                c.b.poison_lo()
-            batched = _run(ctx, c, nsplit, impl)
+    for nsplit, impl in RUNS:
+        if nsplit == 1:
+            c.a.poison_lo()
+            c.b.poison_lo()
+        batched = _run(ctx, c, nsplit, impl)
+        with options(ctx, nsplit=nsplit, gemm_impl=impl):   # the unbatched calls run at the same settings
             for b0, b1 in {(0, 0), (c.nb0 - 1, c.nb1 - 1), (c.nb0 // 2, c.nb1 - 1)}:
                 idx = c.out_index(torch.tensor([b0], device='cuda'), torch.tensor([b1], device='cuda'))[0]
                 sub = Case(c.a, c.b, dict(c.e, obs0=0, obs1=0))
@@ -497,9 +481,6 @@ def test_slice_of_a_batched_launch_equals_the_unbatched_call(ctx, name):
                     yv = y[sidx].view(torch.int32) if k == 0 else y[sidx]
                     assert torch.equal(xv, yv), (f'nsplit {nsplit} gemm_impl {impl}: slice ({b0}, {b1}) output '
                                                  f'{("f32", "hi", "lo")[k]} differs from the unbatched call')
-    finally:
-        ctx.set_option('nsplit', 3)
-        ctx.set_option('gemm_impl', 0)
 
 
 # ------------------------------------------------------------------------------------------ argument checks
@@ -533,8 +514,7 @@ def test_rejects_operands_the_engine_cannot_address(ctx):
         'extents do not broadcast': (op(a, nb0=3), op(b)),
         'b1 extents do not broadcast': (op(a, nb1=2, bs1=8), op(b, nb1=3, bs1=8)),
     }
-    try:
-        ctx.set_option('nsplit', 3)
+    with options(ctx, nsplit=3):
         for what, (x, y) in bad.items():
             assert _call(ctx, x, y, _epilogue(c, *out)) == ALM_ERR_INVALID, what
         assert _call(ctx, op(a, lo=None), op(b), _epilogue(c, *out)) == ALM_ERR_INVALID, 'no lo plane at nsplit 3'
@@ -554,5 +534,3 @@ def test_rejects_operands_the_engine_cannot_address(ctx):
         c.b.poison_lo()
         c.lo_null = True  # nsplit 1 runs without lo planes
         _check(c, _run(ctx, c, 1, 0), 1, 0, 'nsplit 1 without lo planes')
-    finally:
-        ctx.set_option('nsplit', 3)

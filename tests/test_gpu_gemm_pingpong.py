@@ -12,17 +12,13 @@ alm_op_gemm_planes (test_gpu_gemm_operands.py).
 import pytest
 import torch
 
+from tests.support import ctx, options
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
 
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 4096)
-    return c
+WORKSPACE_MB = 4096
 
 
 def _shapes():
@@ -46,16 +42,13 @@ def test_gemm_schedules_match_fp64(ctx, case):
     ref = torch.einsum('bmk,bnk->bmn', A.double(), Wt.double()) + b.double()
     ref = torch.nn.functional.gelu(ref) if act == 1 else (torch.relu(ref) if act == 2 else ref)
     Ad, Wd, bd = A.cuda(), Wt.cuda(), b.cuda()
-    try:
-        for nsplit, tol in ((3, 2e-5), (1, 6e-3)):
-            ctx.set_option('nsplit', nsplit)
+    for nsplit, tol in ((3, 2e-5), (1, 6e-3)):
+        with options(ctx, nsplit=nsplit):
             out = torch.full((batch, M, N), float('nan'), device='cuda')
             ctx.check(ctx.lib.alm_op_linear(ctx.h, Ad.data_ptr(), Wd.data_ptr(), bd.data_ptr(), out.data_ptr(), M, N, K,
                                             act, batch))
             got = out.cpu().double()
-            rows_err = ((got - ref).norm(dim=2) / (ref.norm(dim=2) + 1e-30)).amax(dim=0)   # worst batch per row
-            assert torch.isfinite(got).all(), nsplit
-            assert float(rows_err.max()) < 10 * tol, (nsplit, int(rows_err.argmax()))
-            assert float((got - ref).norm() / ref.norm()) < tol, nsplit
-    finally:
-        ctx.set_option('nsplit', 3)
+        rows_err = ((got - ref).norm(dim=2) / (ref.norm(dim=2) + 1e-30)).amax(dim=0)   # worst batch per row
+        assert torch.isfinite(got).all(), nsplit
+        assert float(rows_err.max()) < 10 * tol, (nsplit, int(rows_err.argmax()))
+        assert float((got - ref).norm() / ref.norm()) < tol, nsplit

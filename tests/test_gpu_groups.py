@@ -3,15 +3,12 @@ OmniParserB200.group_lines).  The device must equal tests/golden/omni_groups.npz
 layouts) and the host build of the same bodies (tests/emu/group_emu.cpp) exactly, line polygons bit for bit; it must
 be reproducible run to run, take the same number of launches whatever the counts, refuse bad arguments before any
 device work, chain after spot_tiled without changing it, and hand its line polygons over to preprocess.curve_crops."""
-import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
-
 import numpy as np
 import pytest
 import torch
+
+from tests.support import assert_same, ctx, emu, golden
+from tests.test_groups_cpu import bind
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
@@ -22,35 +19,16 @@ NAMES = ['paragraph', 'paragraph_rot7', 'paragraph_rot30', 'columns_3h', 'column
          'interleave', 'mutual', 'overlap', 'ties', 'degenerate', 'single', 'empty', 'all', 'tiles']
 ALM_ERR_INVALID = -1
 
-_EMU = None
-
 
 @pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    c = _lib.Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope='module')
-def gold(golden_dir):
-    return np.load(os.path.join(golden_dir, 'omni_groups.npz'))
+def gold():
+    return golden('omni_groups.npz')
 
 
 def emu_group(polys, count, offset, **params):
     """alm_omni_group_lines' five launches as host code (tests/emu/group_emu.cpp) -> the dict group_lines returns."""
-    global _EMU
     from advancedliteratemachinery_b200.omniparser import check_group_args
-    if _EMU is None:
-        if shutil.which('g++') is None:
-            pytest.skip('g++ not available')
-        so = os.path.join(tempfile.mkdtemp(), 'group_emu.so')
-        subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                               os.path.join(os.path.dirname(os.path.abspath(__file__)), 'emu', 'group_emu.cpp'), '-o', so])
-        _EMU = C.CDLL(so)
-        _EMU.emu_group_lines.restype = C.c_long
-        _EMU.emu_group_lines.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_double] * 5 + [C.c_void_p] * 8
+    lib = emu('group_emu', bind)
     prm = check_group_args(**params)
     polys = np.ascontiguousarray(polys, np.float64).reshape(-1, 32)
     count, offset = np.ascontiguousarray(count, np.int32), np.ascontiguousarray(offset, np.int32)
@@ -58,22 +36,11 @@ def emu_group(polys, count, offset, **params):
     out = dict(n_lines=np.zeros(P, np.int32), line_offset=np.zeros(P, np.int32), line_first=np.zeros(N, np.int32),
                line_words=np.zeros(N, np.int32), order=np.zeros(N, np.int32), line_of=np.zeros(N, np.int32),
                rank_of=np.zeros(N, np.int32), line_polys=np.zeros((N, 32)))
-    K = _EMU.emu_group_lines(P, count.ctypes.data, offset.ctypes.data, polys.ctypes.data, *[prm[k] for k in PARAMS],
-                             *[out[k].ctypes.data for k in OUTPUTS])
+    K = lib.emu_group_lines(P, count.ctypes.data, offset.ctypes.data, polys.ctypes.data, *[prm[k] for k in PARAMS],
+                            *[out[k].ctypes.data for k in OUTPUTS])
     for k in ('line_first', 'line_words', 'line_polys'):
         out[k] = out[k][:K]
     return out
-
-
-def assert_same(a, b):
-    """Two groupings are equal, the line polygons bit for bit."""
-    assert a.keys() == b.keys()
-    for k in a:
-        x, y = np.asarray(a[k]), np.asarray(b[k])
-        assert x.shape == y.shape and x.dtype == y.dtype, k
-        if x.dtype.kind == 'f':
-            x, y = x.view(np.uint64), y.view(np.uint64)
-        assert np.array_equal(x, y), k
 
 
 def pages_call(pages):
@@ -164,14 +131,14 @@ def test_invalid_arguments_are_named_and_leave_the_context_usable(ctx, gold):
     assert call()[0] == 0
 
 
-def test_grouping_chains_after_spot_tiled_and_leaves_it_unchanged(golden_dir):
+def test_grouping_chains_after_spot_tiled_and_leaves_it_unchanged():
     """spot_tiled on the tiles fixture's page, then group_lines: the oracle applied to the same merged polygons; the
     spotting result is what it was, before and after."""
     from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
     from advancedliteratemachinery_b200.omniparser import group_lines
     from oracle import group_ref as R
     from tests.conftest import omni_sd
-    t = np.load(os.path.join(golden_dir, 'omni_tiles.npz'))
+    t = golden('omni_tiles.npz')
     m = OmniParserB200(omni_sd(int(t['wseed']), float(t['pt_eos_bias'])),
                        OmniVocab(pt_seq_length=int(t['pt_seq_length']), rec_length=int(t['rec_length'])), workspace_mb=4096)
     try:

@@ -26,9 +26,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests import support
+from tests.support import NAN, assert_guard, bits, close_models, ctx, guarded, omni_model, options, release_models
 from tests.test_gpu_coschedule import _assert_fixture_ids, _assert_same
-from tests.test_gpu_encoder_ops import (NAN, U32, _assert_guard, _assert_split, _bits, _guarded, _ln_tol, _op, _planes,
-                                        _ptr)
+from tests.test_gpu_encoder_ops import U32, _assert_split, _ln_tol, _op, _planes, _ptr
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
@@ -36,28 +37,7 @@ torch.set_grad_enabled(False)
 ERR_INVALID = -1
 D = 512
 V = 1104
-_MODELS = {}
-
-
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 1024)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
+WORKSPACE_MB = 1024
 
 
 # ----------------------------------------------------------------------------------------------- embed_ln
@@ -87,16 +67,16 @@ def _embed_tokens(n, t, tstride, seed):
 
 def _embed(ctx, tok, t, S, word, pos, g, b, S_half=0, tok2=None, pos2=None):
     """alm_op_embed_ln into NaN-guarded outputs -> (x [S, 512], qpos [512], qpos2 [512] or None)"""
-    x, xf = _guarded(S * D)
-    q, qf = _guarded(D)
-    q2, q2f = _guarded(D) if S_half else (None, None)
+    x, xf = guarded(S * D)
+    q, qf = guarded(D)
+    q2, q2f = guarded(D) if S_half else (None, None)
     ctx.check(_op(ctx, 'alm_op_embed_ln', tok.data_ptr(), tok.stride(0), t, S, S_half, _ptr(tok2),
                   tok2.stride(0) if tok2 is not None else 0, word.data_ptr(), V, pos.data_ptr(), _ptr(pos2),
                   g.data_ptr(), b.data_ptr(), x.data_ptr(), q.data_ptr(), _ptr(q2)))
-    _assert_guard(xf, S * D)
-    _assert_guard(qf, D)
+    assert_guard(xf, S * D)
+    assert_guard(qf, D)
     if S_half:
-        _assert_guard(q2f, D)
+        assert_guard(q2f, D)
     return x.view(S, D), q, q2
 
 
@@ -123,7 +103,7 @@ def test_embed_ln_single_against_fp64(ctx, S, t):
     x, q, _ = _embed(ctx, tok, t, S, word, pos, g, b)
     rows, ref = _embed_ref(tok, t, word, pos, g, b)
     worst = _check_embed_rows(x, rows, ref, g, 'x')
-    assert torch.equal(_bits(q), _bits(pos[t].contiguous())), 'qpos is not pos_emb[t]'
+    assert torch.equal(bits(q), bits(pos[t].contiguous())), 'qpos is not pos_emb[t]'
     print(f'[joint] embed_ln S={S} t={t}: worst error / bound {worst:.3f}')
 
 
@@ -141,13 +121,13 @@ def test_embed_ln_joint_against_fp64_and_two_single_launches(ctx, S_half, S, t):
     rows2, ref2 = _embed_ref(tok2, t, word, pos2, g, b)
     worst = max(_check_embed_rows(x[:S_half], rows1, ref1, g, 'first half'),
                 _check_embed_rows(x[S_half:], rows2, ref2, g, 'second half'))
-    assert torch.equal(_bits(q), _bits(pos[t].contiguous())), 'qpos is not pos_emb[t]'
-    assert torch.equal(_bits(q2), _bits(pos2[t].contiguous())), 'qpos2 is not pos_emb2[t]'
+    assert torch.equal(bits(q), bits(pos[t].contiguous())), 'qpos is not pos_emb[t]'
+    assert torch.equal(bits(q2), bits(pos2[t].contiguous())), 'qpos2 is not pos_emb2[t]'
     # what the decoder relies on: the joint launch is one single launch per half
     xa, qa, _ = _embed(ctx, tok, t, S_half, word, pos, g, b)
     xb, qb, _ = _embed(ctx, tok2, t, n2, word, pos2, g, b)
-    assert torch.equal(_bits(x[:S_half]), _bits(xa)) and torch.equal(_bits(x[S_half:]), _bits(xb))
-    assert torch.equal(_bits(q), _bits(qa)) and torch.equal(_bits(q2), _bits(qb))
+    assert torch.equal(bits(x[:S_half]), bits(xa)) and torch.equal(bits(x[S_half:]), bits(xb))
+    assert torch.equal(bits(q), bits(qa)) and torch.equal(bits(q2), bits(qb))
     print(f'[joint] embed_ln S_half={S_half} S={S} t={t}: worst error / bound {worst:.3f}')
 
 
@@ -162,7 +142,7 @@ def _gather(ctx, src, rows, outs, gamma, beta, add, rows_half=0, gamma2=None, be
     bufs = {}
     for k in outs:
         f32 = k.startswith('f32')
-        bufs[k] = _guarded(rows * D, torch.float32 if f32 else torch.int16, NAN if f32 else -1)
+        bufs[k] = guarded(rows * D, torch.float32 if f32 else torch.int16, NAN if f32 else -1)
 
     def p(k):
         return bufs[k][0].data_ptr() if k in bufs else None
@@ -174,7 +154,7 @@ def _gather(ctx, src, rows, outs, gamma, beta, add, rows_half=0, gamma2=None, be
         ctx.check(_op(ctx, 'alm_op_gather_ln', *args))
     res = {}
     for k, (buf, full) in bufs.items():
-        _assert_guard(full, buf.numel(), NAN if k.startswith('f32') else -1)
+        assert_guard(full, buf.numel(), NAN if k.startswith('f32') else -1)
         res[k] = buf.view(rows, D)
     return res
 
@@ -213,7 +193,7 @@ def test_gather_ln_joint_against_fp64_and_each_half_alone(ctx, S, form, mean):
         # bit for bit the single entry on this half alone with its own affine and query position (ld_add 0 too)
         alone = _gather(ctx, src[h * S:], S, FORMS[form] + twins, g, b, adds[h])
         for k in alone:
-            assert torch.equal(_bits(alone[k]), _bits(half[k])), (h, k, 'joint half differs from the single launch')
+            assert torch.equal(bits(alone[k]), bits(half[k])), (h, k, 'joint half differs from the single launch')
     # the form exactly as the decoder launches it (no f32 outputs) writes the same planes
     plain = _gather(ctx, src, rows, FORMS[form], g1, b1, adds[0], S, g2, b2, adds[1])
     for k in plain:
@@ -277,25 +257,8 @@ def test_argument_errors_leave_the_context_usable(ctx):
 
 
 # ----------------------------------------------------------------------------------------------- whole decodes
-DEFAULT = dict(joint_decode=1, use_graphs=1, xattn_impl=0)
-
-
-def _model(key, make_sd, vie=0):
-    """one resident OmniParserB200 at a time"""
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(make_sd(), OmniVocab(vie_categories=vie), workspace_mb=4096)
-    m = _MODELS[key]
-    for k, v in DEFAULT.items():
-        m.ctx.set_option(k, v)
-    return m
-
-
 def _spot_model(wseed, bias):
-    from tests.conftest import omni_sd
-    return _model(('spot', wseed, bias), lambda: omni_sd(wseed, bias))
+    return omni_model(dict(wseed=wseed, pt_eos_bias=bias))
 
 
 def _decode_launches(m, f):
@@ -308,22 +271,17 @@ def joint_ab(m, run, what):
     """run() -> (result, launches of its decodes) with joint_decode 1 and 0, with graphs on and off, at xattn_impl 0 and
     2: bit for bit the same result, and fewer launches with the joint pass (it ran).  Returns the default run's result."""
     base = None
-    try:
-        for graphs in (1, 0):
-            for xattn in (0, 2):
-                got = {}
-                for joint in (1, 0):
-                    for k, v in dict(joint_decode=joint, use_graphs=graphs, xattn_impl=xattn).items():
-                        m.ctx.set_option(k, v)
+    for graphs in (1, 0):
+        for xattn in (0, 2):
+            got = {}
+            for joint in (1, 0):
+                with options(m.ctx, joint_decode=joint, use_graphs=graphs, xattn_impl=xattn):
                     got[joint] = run()
-                label = f'{what}: use_graphs {graphs}, xattn_impl {xattn}'
-                _assert_same(got[0][0], got[1][0], label + ', joint pass against the single-decoder loops')
-                assert got[1][1] < got[0][1], (label, 'the joint pass did not run', got[1][1], got[0][1])
-                if base is None:
-                    base = got[1][0]
-    finally:
-        for k, v in DEFAULT.items():
-            m.ctx.set_option(k, v)
+            label = f'{what}: use_graphs {graphs}, xattn_impl {xattn}'
+            _assert_same(got[0][0], got[1][0], label + ', joint pass against the single-decoder loops')
+            assert got[1][1] < got[0][1], (label, 'the joint pass did not run', got[1][1], got[0][1])
+            if base is None:
+                base = got[1][0]
     print(f'[joint] {what}: joint pass bit-identical to the single-decoder loops in 4 settings')
     return base
 
@@ -389,7 +347,7 @@ def _regimes():
     """batches of the 'full' page (4 instances each) whose S = 4 B rows per decoder put the self-attention step in each
     regime of the joint pass's decoder step: both halves and the joint rows on the wide kernel (S <= SMs / 4), one launch per half
     (SMs / 4 < S <= SMs / 2), none on the wide kernel (S > SMs / 2)"""
-    sms = _sms()
+    sms = support.sms()
     return {'one_wide_launch': (sms // 4) // 4, 'per_half_launches': (sms // 2) // 4, 'one_launch': (sms // 2) // 4 + 1}
 
 
@@ -397,7 +355,7 @@ def _regimes():
 def test_self_attention_regimes_of_the_sm_count(regime, golden_dir):
     case, gold, img, mask = _case('full', golden_dir)
     B = _regimes()[regime]
-    S, sms = 4 * B, _sms()
+    S, sms = 4 * B, support.sms()
     assert {'one_wide_launch': S <= sms / 4, 'per_half_launches': sms / 4 < S <= sms / 2,
             'one_launch': S > sms / 2}[regime], (regime, S, sms)
     m = _spot_model(case['wseed'], case['pt_eos_bias'])
@@ -464,13 +422,10 @@ def test_window_prompts(golden_dir):
 
 def test_kie(golden_dir):
     from advancedliteratemachinery_b200 import NestedTensor
-    from advancedliteratemachinery_b200 import synthetic as W
     from oracle.gen_golden import KIE_CASES, omni_inputs
     case = KIE_CASES['kie']
     gold = np.load(os.path.join(golden_dir, 'omni_kie.npz'))
-    m = _model(('kie',), lambda: W.omniparser_state_dict(seed=case['wseed'], vie_categories=case['vie'],
-                                                         pt_eos_bias=case['pt_eos_bias']), vie=case['vie'])
-    _set_lengths(m, case['pt_seq_length'], case['rec_length'])
+    m = omni_model(case, kie=True)
     img, mask = omni_inputs(case)
     v = m.vocab
     seqs = [v.pt_prompt(), torch.tensor([[v.poly_sos_index]]), torch.tensor([[v.rec_sos_index]]),
@@ -530,9 +485,14 @@ def _perturbed_sd(kind):
 @pytest.mark.parametrize('kind', ['rec_norm', 'swapped_positions'])
 def test_checkpoints_whose_halves_differ(kind, golden_dir):
     case, gold, img, mask = _case('full', golden_dir)
-    m = _model(('perturbed', kind), lambda: _perturbed_sd(kind))
-    _set_lengths(m, case['pt_seq_length'], 40)
-    base = joint_ab(m, _spotting_run(m, img, mask), f'omni full, {kind}, rec_length 40')
+    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
+    close_models()   # one resident model at a time
+    m = OmniParserB200(_perturbed_sd(kind), OmniVocab(), workspace_mb=4096)
+    try:
+        _set_lengths(m, case['pt_seq_length'], 40)
+        base = joint_ab(m, _spotting_run(m, img, mask), f'omni full, {kind}, rec_length 40')
+    finally:
+        m.ctx.close()
     # the change reaches the decode: the probabilities are not the unchanged checkpoint's
     ref = _spot_model(0, -30.0)
     _set_lengths(ref, case['pt_seq_length'], 40)

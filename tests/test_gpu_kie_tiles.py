@@ -4,7 +4,6 @@ reference's per-tile outputs (tests/golden/omni_kie_tiles.npz); a one-tile page 
 turns must give the reading of np.rot90(page, k) mapped back; 'auto' must pick the reference probes' turn; the device
 merge must equal the host build of the same bodies (tests/emu/kie_tile_emu.cpp) bit for bit; and refused calls leave
 the context and every other decode unchanged."""
-import os
 
 import numpy as np
 import pytest
@@ -12,40 +11,11 @@ import torch
 
 from oracle import kie_tile_ref as K
 from oracle import page_turn_ref as PT
-from tests.test_kie_tiles_cpu import assert_same, emu_merge, fabricate
+from tests.support import assert_same, golden, kw, omni_model, release_models
+from tests.test_kie_tiles_cpu import emu_merge, fabricate
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
-
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def fixture(golden_dir):
-    return np.load(os.path.join(golden_dir, 'omni_kie_tiles.npz'))
-
-
-def model(g):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from advancedliteratemachinery_b200 import synthetic as W
-    if 'kie' not in _MODELS:
-        sd = W.omniparser_state_dict(seed=int(g['wseed']), vie_categories=int(g['vie']),
-                                     pt_eos_bias=float(g['pt_eos_bias']))
-        _MODELS['kie'] = OmniParserB200(sd, OmniVocab(vie_categories=int(g['vie']),
-                                                      pt_seq_length=int(g['pt_seq_length']),
-                                                      rec_length=int(g['rec_length'])), workspace_mb=4096)
-    return _MODELS['kie']
-
-
-def kw(g):
-    return dict(tile=int(g['tile']), overlap=int(g['overlap']), test_min_size=int(g['test_min_size']),
-                test_max_size=int(g['test_max_size']))
 
 
 def ref_tiles(g):
@@ -68,11 +38,11 @@ def same_entities(a, b, rtol=0.0):
         assert [e[2] for e in a] == [e[2] for e in b]
 
 
-def test_fixture_page_equals_reference_merge(golden_dir):
+def test_fixture_page_equals_reference_merge():
     """Texts, classes and rects bit for bit, probabilities within the decoder's tolerance; every tile's token ids are
     the reference's; the device merge of the device's own tile decodes equals the host build bit for bit."""
-    g = fixture(golden_dir)
-    m = model(g)
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     page = g['page']
     got = m.kie_tiled([page], **kw(g))
     ref = K.merge([page.shape[:2]], int(g['tile']), int(g['overlap']), ref_tiles(g))
@@ -90,11 +60,11 @@ def test_fixture_page_equals_reference_merge(golden_dir):
     assert [tuple(s) for s in t['merged']['source'].tolist()] == ref['source'][0]
 
 
-def test_one_tile_page_is_decode_kie(golden_dir):
+def test_one_tile_page_is_decode_kie():
     """A page that fits in one tile gives exactly decode_kie's list from forward_pages on the whole page."""
     from advancedliteratemachinery_b200 import preprocess as P
-    g = fixture(golden_dir)
-    m = model(g)
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     page = np.ascontiguousarray(g['page'][:100, :90])
     got = m.kie_tiled([page], **kw(g))
     v = m.vocab
@@ -105,11 +75,11 @@ def test_one_tile_page_is_decode_kie(golden_dir):
     assert exp and got[0] == exp
 
 
-def test_turns_map_back(golden_dir):
+def test_turns_map_back():
     """Explicit turns k = 1..3 give kie_tiled(np.rot90(page, k)) with every rect and vertex mapped back; 'upright' and
     all-zero turns give the same result."""
-    g = fixture(golden_dir)
-    m = model(g)
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     page = g['page']
     H, W = page.shape[:2]
     up = m.kie_tiled([page], **kw(g))
@@ -136,10 +106,10 @@ def test_turns_map_back(golden_dir):
         assert np.array_equal(t['merged']['poly'], pv)
 
 
-def test_auto_picks_the_reference_turn(golden_dir):
+def test_auto_picks_the_reference_turn():
     """'auto' chooses the turn of the reference's probes with their scores, and reads the page at that turn."""
-    g = fixture(golden_dir)
-    m = model(g)
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     page = g['page']
     got = m.kie_tiled([page], orientation='auto', **kw(g))
     t = m.last_tiles
@@ -149,9 +119,9 @@ def test_auto_picks_the_reference_turn(golden_dir):
     assert got == m.kie_tiled([page], orientation=g['probe_turn'].tolist(), **kw(g))
 
 
-def test_max_batch_gives_the_same_entities(golden_dir):
-    g = fixture(golden_dir)
-    m = model(g)
+def test_max_batch_gives_the_same_entities():
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     pages = [g['page'], np.ascontiguousarray(g['page'][:100, :90]), np.ascontiguousarray(g['page'][:, :150])]
     ref = m.kie_tiled(pages, max_batch=1, **kw(g))
     n = len(m.last_tiles['plan'])
@@ -159,12 +129,12 @@ def test_max_batch_gives_the_same_entities(golden_dir):
         assert m.kie_tiled(pages, max_batch=b, **kw(g)) == ref
 
 
-def test_merge_at_scale_equals_host_build(golden_dir):
+def test_merge_at_scale_equals_host_build():
     """16 A4 pages at 300 dpi x 12 tiles of fabricated entities (1..8 words, wordless ones, some turned): the device
     merge equals the host build of the same bodies bit for bit."""
     from advancedliteratemachinery_b200.omniparser import merge_kie_tiles
-    g = fixture(golden_dir)
-    m = model(g)
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     rng = np.random.default_rng(11)
     sizes = [(3508, 2480)] * 16
     turns = [0] * 8 + [1, 2, 3, 0, 1, 2, 3, 0]
@@ -184,7 +154,7 @@ def test_merge_at_scale_equals_host_build(golden_dir):
         assert 0 < int(dev['count'].sum()) and (dev['word_count'] > 1).any()
 
 
-def test_errors_leave_everything_usable(golden_dir):
+def test_errors_leave_everything_usable():
     """A spotting checkpoint, a bad layout, a bad turn, a mismatched inst_pos and a too-small capacity are refused;
     afterwards decode_kie / forward_pages, kie_tiled and spot_tiled give what they gave before."""
     import ctypes as C
@@ -193,8 +163,8 @@ def test_errors_leave_everything_usable(golden_dir):
     from advancedliteratemachinery_b200 import preprocess as P
     from advancedliteratemachinery_b200.omniparser import merge_kie_tiles
     from tests.conftest import omni_sd
-    g = fixture(golden_dir)
-    m = model(g)
+    g = golden('omni_kie_tiles.npz')
+    m = omni_model(g, kie=True)
     page = g['page']
     v = m.vocab
     small = np.ascontiguousarray(page[:100, :90])
@@ -248,13 +218,12 @@ def test_errors_leave_everything_usable(golden_dir):
     assert fwd() == before
     assert m.kie_tiled([page], **kw(g)) == tiled
     # a spotting checkpoint is refused; its context keeps working
-    tg = np.load(os.path.join(golden_dir, 'omni_tiles.npz'))
+    tg = golden('omni_tiles.npz')
     s = OmniParserB200(omni_sd(int(tg['wseed']), float(tg['pt_eos_bias'])),
                        OmniVocab(pt_seq_length=int(tg['pt_seq_length']), rec_length=int(tg['rec_length'])),
                        workspace_mb=4096)
     try:
-        tkw = dict(tile=int(tg['tile']), overlap=int(tg['overlap']), test_min_size=int(tg['test_min_size']),
-                   test_max_size=int(tg['test_max_size']))
+        tkw = kw(tg)
         spot = s.spot_tiled([tg['page']], **tkw)
         with pytest.raises(ValueError):
             s.kie_tiled([tg['page']], **tkw)

@@ -3,13 +3,13 @@ MGPSTRB200.recognize_lines).  Bar: window crops equal tests/golden/pre_lines.npz
 counts, boxes and centres equal oracle/line_ref.py bit for bit when it is fed the device's own per-window maps (read
 back through forward(is_eval=True) on the same window crops); a one-window line is what recognize_regions /
 recognize_polygons give for its crop."""
-
 import numpy as np
 import pytest
 import torch
 
+from tests.support import emu, mgp_model, options, release_models
 from tests.test_curve_crops_cpu import curve_fixture, curve_regions
-from tests.test_lines_cpu import build_emu, emu_line_stitch, line_fixture
+from tests.test_lines_cpu import bind, emu_line_stitch, line_fixture
 from tests.test_quad_crops_cpu import quad_fixture, text_regions
 
 pytestmark = pytest.mark.gpu
@@ -19,11 +19,7 @@ CODE = {'quad': 1, 'curve': 2}
 
 @pytest.fixture(scope='module')
 def model():
-    from advancedliteratemachinery_b200 import MGPSTRB200
-    from tests.conftest import mgp_sd
-    m = MGPSTRB200(mgp_sd(0))
-    yield m
-    m.ctx.close()
+    return mgp_model()
 
 
 def chunks(n, max_batch):
@@ -100,8 +96,7 @@ def test_stitch_equals_oracle_on_device_maps(model, nsplit):
     """recognize_lines on the fixture's quads (chunks of at most 16 windows) and curves: every stitched id, probability,
     count, box and centre equals the oracle's on the device's own maps, ids and probabilities."""
     m = model
-    m.ctx.set_option('nsplit', nsplit)
-    try:
+    with options(m.ctx, nsplit=nsplit):
         z, pages = line_fixture()
         dev = [torch.from_numpy(p).cuda() for p in pages]
         for kind, regions, pidx, mb in (('quad', z['quads'], z['quad_page_index'], 16),
@@ -111,8 +106,6 @@ def test_stitch_equals_oracle_on_device_maps(model, nsplit):
             assert np.array_equal(out[5].numpy(), plan['n'])
             assert_lines_oracle(out, maps, ids, probs, plan, kind)
             assert (out[2] > 26).any() or kind == 'curve'
-    finally:
-        m.ctx.set_option('nsplit', 3)
 
 
 def fuse(ids, probs):
@@ -186,7 +179,7 @@ def test_chunking_empty_and_a_thousand_lines(model):
     out = m.recognize_lines(pages, np.zeros((0, 16, 2)), [], kind='curve')
     assert out[0].shape == (3, 0, 210)
 
-    lib = build_emu()
+    lib = emu('line_emu', bind)
     for kind, (pg, regions, pidx) in (('quad', text_regions(seed=11)), ('curve', curve_regions(seed=12))):
         dev = [torch.from_numpy(p).cuda() for p in pg]
         out = m.recognize_lines(dev, regions, pidx, kind=kind)

@@ -16,54 +16,19 @@ Every output buffer is followed by a guard region that must come back bit for bi
 call must not read holds NaN: pad columns, rows after the last crop or row, and the whole lo plane at nsplit 1, where
 the model's producers never write it.  Split outputs must be hi = bf16_rn(x), lo = bf16_rn(x - hi) of the fp32 value.
 """
-import contextlib
-
 import pytest
 import torch
+
+from tests.support import NAN, assert_guard, bits, ctx, guarded, options
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
-GUARD = 1024
-NAN = float('nan')
+WORKSPACE_MB = 2048
 ERR_INVALID, ERR_UNSUPPORTED = -1, -5
 U32 = 2.0 ** -24        # fp32 unit roundoff
 UBF = 2.0 ** -8         # bf16 unit roundoff
 NAN16 = -1              # 0xffff: a bf16 NaN
-
-
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    c.set_option('workspace_mb', 2048)
-    yield c
-    c.close()
-
-
-@contextlib.contextmanager
-def nsplit(ctx, n):
-    try:
-        ctx.set_option('nsplit', n)
-        yield
-    finally:
-        ctx.set_option('nsplit', 3)
-
-
-def _guarded(n, dtype=torch.float32, fill=NAN, guard=GUARD):
-    """(first n elements, whole buffer) of a device buffer with `guard` elements of `fill` after it"""
-    full = torch.full((n + guard,), fill, dtype=dtype, device='cuda')
-    return full[:n], full
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _assert_guard(full, n, fill=NAN):
-    g = full[n:]
-    assert torch.equal(_bits(g), _bits(torch.full_like(g, fill))), 'write past the end of the output'
 
 
 def _ptr(t):
@@ -189,8 +154,8 @@ def _run_attn(ctx, hi, lo, B, T, H, ldo, f32=True, with_lo=True):
     block long, so rows of the last block past T that were written would land in it."""
     D, R = H * 64, B * T
     n, guard = R * ldo, 64 * ldo
-    out, ofull = _guarded(n, guard=guard) if f32 else (None, None)
-    (oh, hfull), (ol, lfull) = (_guarded(n, torch.int16, NAN16, guard) for _ in range(2))
+    out, ofull = guarded(n, guard=guard) if f32 else (None, None)
+    (oh, hfull), (ol, lfull) = (guarded(n, torch.int16, NAN16, guard) for _ in range(2))
     ctx.check(_op(ctx, 'alm_op_attention_ex', hi.data_ptr(), lo.data_ptr() if with_lo else None, hi.stride(0), B, T, H,
                   _ptr(out), oh.data_ptr(), ol.data_ptr(), ldo))
     res = []
@@ -198,10 +163,10 @@ def _run_attn(ctx, hi, lo, B, T, H, ldo, f32=True, with_lo=True):
         if buf is None:
             res.append(None)
             continue
-        _assert_guard(full, n, fill)
+        assert_guard(full, n, fill)
         v = buf.view(R, ldo)
         gap = v[:, D:]
-        assert torch.equal(_bits(gap), _bits(torch.full_like(gap, fill))), 'wrote past the row width'
+        assert torch.equal(bits(gap), bits(torch.full_like(gap, fill))), 'wrote past the row width'
         res.append(v[:, :D].contiguous())
     return tuple(res)
 
@@ -214,7 +179,7 @@ def _check_attention(ctx, x, B, T, H, ld, ldo, ref=None, alone=True):
     D = H * 64
     ref = ref or _attn_ref(x, B, T, H)
     for ns in (3, 1):
-        with nsplit(ctx, ns):
+        with options(ctx, nsplit=ns):
             hi, lo = _planes(x, ld, lo_nan=ns == 1)
             out, oh, ol = _run_attn(ctx, hi, lo, B, T, H, ldo)
             assert torch.isfinite(out).all(), ns
@@ -235,7 +200,7 @@ def _check_attention(ctx, x, B, T, H, ld, ldo, ref=None, alone=True):
             if alone and B > 1:   # the last crop alone (followed by the NaN rows) == the same crop inside the batch
                 rows = slice((B - 1) * T, B * T)
                 got, _, _ = _run_attn(ctx, hi[rows], lo[rows], 1, T, H, D)
-                assert torch.equal(_bits(got), _bits(out[rows])), ns
+                assert torch.equal(bits(got), bits(out[rows])), ns
 
 
 # T at every edge of the 64-row query blocks, 16-row warp bands, 64-key blocks and 8-key column pairs, odd and even
@@ -275,17 +240,17 @@ def test_attention_fp32_entry_matches_fp64(ctx, B, T, H):
     x[:, :D] *= 1.5     # sharper softmax than unit-variance scores
     ref = _attn_ref(x, B, T, H)
     for ns, rel in ((3, 3e-5), (1, 2e-2)):
-        with nsplit(ctx, ns):
-            out, ofull = _guarded(B * T * D, guard=64 * D)
+        with options(ctx, nsplit=ns):
+            out, ofull = guarded(B * T * D, guard=64 * D)
             ctx.check(_op(ctx, 'alm_op_attention', x.data_ptr(), out.data_ptr(), B, T, H))
-            _assert_guard(ofull, B * T * D)
+            assert_guard(ofull, B * T * D)
             out = out.view(B * T, D)
             err = (out.double() - ref['o']).abs()
             assert bool((err <= _attn_tol(ref, ns)).all()), (ns, float(err.max()))
             assert float(err.max() / ref['o'].abs().max()) < rel, ns     # and within rel of the largest output
             hi, lo = _planes(x, 3 * D, lo_nan=False)
             ex, _, _ = _run_attn(ctx, hi, lo, B, T, H, D)
-            assert torch.equal(_bits(ex), _bits(out)), ns
+            assert torch.equal(bits(ex), bits(out)), ns
 
 
 # ----------------------------------------------------------------------------------------------- row selection
@@ -349,11 +314,11 @@ def _logits(rows, n, ld, gen, special):
 def _run_select(ctx, x, n, k):
     rows, ld = x.shape[0], x.stride(0)
     per = max(k, 1)
-    ids, ifull = _guarded(rows * per, torch.int32, -7)
-    probs, pfull = _guarded(rows * per)
+    ids, ifull = guarded(rows * per, torch.int32, -7)
+    probs, pfull = guarded(rows * per)
     ctx.check(_op(ctx, 'alm_op_row_select', x.data_ptr(), ld, rows, n, k, ids.data_ptr(), probs.data_ptr()))
-    _assert_guard(ifull, rows * per, -7)
-    _assert_guard(pfull, rows * per)
+    assert_guard(ifull, rows * per, -7)
+    assert_guard(pfull, rows * per)
     return ids.view(rows, per), probs.view(rows, per)
 
 
@@ -381,11 +346,11 @@ def _check_select(ctx, x, n):
         ids, probs = _run_select(ctx, x, n, k)
         kk = min(k, n)
         assert torch.equal(ids[:, :kk].long(), order[:, :kk]), ('ids', k)
-        assert bool((ids[:, kk:] == -1).all()) and not bool(_bits(probs[:, kk:]).any()), ('past n', k)
-        assert torch.equal(ids[:, :1], id0) and torch.equal(_bits(probs[:, :1]), _bits(pr0)), ('candidate 0', k)
+        assert bool((ids[:, kk:] == -1).all()) and not bool(bits(probs[:, kk:]).any()), ('past n', k)
+        assert torch.equal(ids[:, :1], id0) and torch.equal(bits(probs[:, :1]), bits(pr0)), ('candidate 0', k)
         close(ids[:, :kk], probs[:, :kk], k)
         tied = v.gather(1, ids[:, :kk].long()) == top
-        assert torch.equal(_bits(probs[:, :kk])[tied], _bits(pr0.expand(-1, kk))[tied]), ('tied probability', k)
+        assert torch.equal(bits(probs[:, :kk])[tied], bits(pr0.expand(-1, kk))[tied]), ('tied probability', k)
         assert bool((probs[:, 1:kk] <= probs[:, :kk - 1]).all()), ('not non-increasing', k)
 
 
@@ -429,7 +394,7 @@ def test_argument_errors_leave_the_context_usable(ctx):
     assert attn(l=None) == ERR_INVALID                       # nsplit 3 needs the lo plane
     assert attn(T=273) == ERR_UNSUPPORTED
     assert bool(torch.isnan(out).all()), 'written before the error'
-    with nsplit(ctx, 1):
+    with options(ctx, nsplit=1):
         assert attn(l=None) == 0                             # nsplit 1 reads the hi plane only
 
     logits = torch.randn(4, 40, device='cuda')

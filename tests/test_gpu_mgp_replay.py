@@ -31,6 +31,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.support import options
 from tests.test_gpu_mgp_ops import _attn_ref, _attn_tol, _check_select
 
 pytestmark = pytest.mark.gpu
@@ -574,16 +575,6 @@ def _assert_same_bits(got, want, label):
                                      f'model {float(w[tuple(first)])!r}')
 
 
-def _opts(ctx, ns, impl):
-    ctx.set_option('nsplit', ns)
-    ctx.set_option('attn_impl', impl)
-
-
-def _reset(ctx):
-    ctx.set_option('nsplit', 3)
-    ctx.set_option('attn_impl', 0)
-
-
 CASES = ['depth1', 'depth2', 'base-B1', 'base-B3', 'base-B512', 'tiny', 'small', 'large', 'charstr']
 RUNS = [(3, 0), (3, 1), (1, 0), (1, 1)]   # (nsplit, attn_impl)
 
@@ -597,8 +588,7 @@ def test_replay_is_the_forward_bit_for_bit(case, ns, impl):
     ctx = m.ctx
     img = _image(B, seed=len(case) * 100 + B)
     label = f'{case} nsplit {ns} attn_impl {impl}'
-    try:
-        _opts(ctx, ns, impl)
+    with options(ctx, nsplit=ns, attn_impl=impl):
         want, launches = _forward(m, img)
         chk = _Checker(ns, crops if crops is not None else list(range(B)), label)
         ctx.launch_count(reset=True)
@@ -616,8 +606,6 @@ def test_replay_is_the_forward_bit_for_bit(case, ns, impl):
             sel = torch.full((len(rows), Vpad), float('nan'), device='cuda')
             sel[:, :V] = lg.reshape(-1, V)[rows]
             _check_select(ctx, sel, V)
-    finally:
-        _reset(ctx)
 
 
 def test_single_pass_forward_leaves_the_context_splitting():
@@ -628,15 +616,12 @@ def test_single_pass_forward_leaves_the_context_splitting():
     m, w, B, _ = _model('base-B3')
     ctx = m.ctx
     img = _image(B, seed=11)
-    try:
-        _opts(ctx, 1, 0)
+    with options(ctx, nsplit=1, attn_impl=0):
         single, _ = _forward(m, img)
         got1 = _replay(ctx, w, img, 1, 0)
         _assert_same_bits(got1, single, 'nsplit 1, model form')
-        _opts(ctx, 3, 0)
+    with options(ctx, nsplit=3, attn_impl=0):
         got3 = _replay(ctx, w, img, 3, 0)
         split, _ = _forward(m, img)
         _assert_same_bits(got3, split, 'nsplit 3 after a forward at nsplit 1')
         assert not torch.equal(got3['logits'][0], got1['logits'][0]), 'nsplit 3 and 1 must differ'
-    finally:
-        _reset(ctx)

@@ -6,17 +6,15 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import mgp_model, options, release_models
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
 
 @pytest.fixture(scope='module')
 def model():
-    from advancedliteratemachinery_b200 import MGPSTRB200
-    from tests.conftest import mgp_sd
-    m = MGPSTRB200(mgp_sd(0))
-    yield m
-    m.ctx.close()
+    return mgp_model()
 
 
 def _maxrel(a, b):
@@ -123,14 +121,11 @@ def test_config3_batch_512_rows_equal_small_batches_and_the_oracle(model):
     out = model(img[sel].contiguous(), is_eval=True)
     for a, b in zip(out[1:], ref[1:]):
         assert _maxrel(a, b) < 1e-3
-    model.ctx.set_option('nsplit', 1)
-    try:
+    with options(model.ctx, nsplit=1):
         model.forward(img.cuda(), is_eval=True, want_logits=False)
         flips = float((model.last_ids != ids_big).float().mean())
         print(f'single-pass bf16 at B=512: {flips * 100:.2f} % of the 3 x 512 x 27 ids differ from the split (fp32-class) mode')
         assert flips < 0.25
-    finally:
-        model.ctx.set_option('nsplit', 3)
 
 
 def test_fused_attention_model_path_matches_fixture_and_unfused_path(golden_dir):

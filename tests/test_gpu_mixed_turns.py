@@ -3,14 +3,12 @@ orientation='mixed'); DESIGN 4.15).  The device merge must equal the host build 
 in three launches; each of the four readings must be the explicit-turn reading; the merged result must equal
 oracle/turn_merge_ref.py on tests/golden/omni_page_turns.npz (the reference's four readings of one page) and on the
 device's own readings; and no other orientation may change."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import turn_merge_ref as R
-from tests.test_tiles_cpu import assert_same
+from tests.support import assert_same, golden, kw, omni_model, release_models, same
 from tests.test_turn_merge_cpu import EOS, PAD, emu_merge, fixture_rows
 
 pytestmark = pytest.mark.gpu
@@ -18,45 +16,12 @@ torch.set_grad_enabled(False)
 
 ERR_INVALID = -1  # include/alm_ocr.h ALM_ERR_INVALID
 
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def fixture(golden_dir):
-    return np.load(os.path.join(golden_dir, 'omni_page_turns.npz'))
-
-
-def model(gold):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed']), float(gold['pt_eos_bias'])),
-                                         OmniVocab(pt_seq_length=int(gold['pt_seq_length']),
-                                                   rec_length=int(gold['rec_length'])), workspace_mb=4096)
-    return _MODELS['spot']
-
-
-def kw(gold, **extra):
-    return dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-                test_max_size=int(gold['test_max_size']), **extra)
-
 
 def pages(gold):
     """The fixture page (larger than T), a page of 2 x 3 tiles and one smaller than a tile."""
     rng = np.random.default_rng(21)
     return [gold['page'], rng.integers(0, 256, (230, 301, 3), dtype=np.uint8),
             rng.integers(0, 256, (97, 120, 3), dtype=np.uint8)]
-
-
-def same(a, b):
-    """Two spot_tiled results are equal, floats bit for bit."""
-    assert [[list(d.items()) for d in r] for r in a] == [[list(d.items()) for d in r] for r in b]
 
 
 def large_rows(rng, P=16, n=4096, L=25):
@@ -81,11 +46,11 @@ def large_rows(rng, P=16, n=4096, L=25):
     return count, offset, pts, polys, rec, prob
 
 
-def test_device_merge_equals_the_emulation(golden_dir):
+def test_device_merge_equals_the_emulation():
     """The fixture's four readings and 16 pages x 4 readings x 4 096 fabricated rows: every output field of the
     device merge equals the host build fed the same inputs, bit for bit, in three launches."""
     from advancedliteratemachinery_b200.omniparser import merge_turns
-    m = model(fixture(golden_dir))
+    m = omni_model(golden('omni_page_turns.npz'))
     args, pad, eos = fixture_rows()
     m.ctx.launch_count(reset=True)
     got = merge_turns(m.ctx, *args, pad, eos)
@@ -101,13 +66,13 @@ def test_device_merge_equals_the_emulation(golden_dir):
         assert 0 < int(got['count'].sum()) < len(big[2])
 
 
-def test_mixed_on_the_fixture(golden_dir):
+def test_mixed_on_the_fixture():
     """The fixture page at tile 128: the four readings are the explicit-turn readings (and the reference's); the
     result is turn_merge_ref of the fixture's merged_* rows, with 'turns' / 'tile' / 'instance' from the oracle's
     sources, and turn_merge_ref of the device's own readings bit for bit."""
     from advancedliteratemachinery_b200 import postprocess
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     v = m.vocab
     page = gold['page']
     got = m.spot_tiled([page], orientation='mixed', **kw(gold))[0]
@@ -141,10 +106,10 @@ def test_mixed_on_the_fixture(golden_dir):
         assert d['pts'] == [pts.tolist()] and d['polys'] == poly.reshape(-1, 2).tolist() and d['rec'] == txt
 
 
-def test_single_tile_pages_read_the_auto_probes(golden_dir):
+def test_single_tile_pages_read_the_auto_probes():
     """Pages no larger than T: the four tiled readings are 'auto''s probe readings, array for array."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = [gold['page'], pages(gold)[2]]
     args = dict(kw(gold), tile=256, overlap=32)
     m.spot_tiled(pg, orientation='auto', **args)
@@ -156,13 +121,13 @@ def test_single_tile_pages_read_the_auto_probes(golden_dir):
         assert np.array_equal(t[k], a), k
 
 
-def test_mixed_agrees_across_chunks_page_kinds_and_sizes(golden_dir):
+def test_mixed_agrees_across_chunks_page_kinds_and_sizes():
     """max_batch 1 / 5 / 16, host and CUDA pages, every page alone and with the others (pages smaller and larger
     than T): the same result.  In chunks of 16 tiles the decoder's probabilities differ from those of smaller chunks
     in the last bits (its ids and coordinates do not; so do the upright and explicit-turn paths), so there the words,
     their turns, tiles, coordinates and texts are compared exactly and the scores to 1e-5."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = pages(gold)
     base = m.spot_tiled(pg, max_batch=5, orientation='mixed', **kw(gold))
     assert all(len(r) > 0 for r in base)
@@ -177,9 +142,9 @@ def test_mixed_agrees_across_chunks_page_kinds_and_sizes(golden_dir):
                                rtol=1e-5, atol=0)
 
 
-def test_group_lines_takes_the_result_as_it_is(golden_dir):
-    gold = fixture(golden_dir)
-    m = model(gold)
+def test_group_lines_takes_the_result_as_it_is():
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     res = m.spot_tiled(pages(gold), orientation='mixed', **kw(gold))
     lines = m.group_lines(res)
     assert len(lines) == len(res)
@@ -188,9 +153,9 @@ def test_group_lines_takes_the_result_as_it_is(golden_dir):
         assert words == list(range(len(r)))
 
 
-def test_other_orientations_are_unchanged_by_a_mixed_call(golden_dir):
-    gold = fixture(golden_dir)
-    m = model(gold)
+def test_other_orientations_are_unchanged_by_a_mixed_call():
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = pages(gold)
     modes = ('upright', [1, 3, 2], 'auto')
     before = [m.spot_tiled(pg, orientation=o, **kw(gold)) for o in modes]
@@ -199,14 +164,14 @@ def test_other_orientations_are_unchanged_by_a_mixed_call(golden_dir):
         same(m.spot_tiled(pg, orientation=o, **kw(gold)), b)
 
 
-def test_error_paths_leave_the_context_usable(golden_dir):
+def test_error_paths_leave_the_context_usable():
     """The C entry refuses bad pages / lengths, null buffers, negative counts, offsets that are not the counts'
     prefix sum, a bad iou and a small cap before any device work; the Python entries refuse bad orientations and a
     KIE checkpoint; the context merges correctly afterwards."""
     from advancedliteratemachinery_b200 import OmniParserB200
     from advancedliteratemachinery_b200.omniparser import merge_turns
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     lib, h = m.ctx.lib, m.ctx.h
     args, pad, eos = fixture_rows()
     count, offset = (np.ascontiguousarray(a, np.int32) for a in args[:2])

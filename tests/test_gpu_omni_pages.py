@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import close_models, omni_model, options, release_models
 from tests.test_pages_cpu import pages_case, pages_page
 
 pytestmark = pytest.mark.gpu
@@ -18,27 +19,9 @@ ERR_INVALID, ERR_STATE, ERR_UNSUPPORTED = -1, -4, -5
 ORDER = [0, 3, 1, 4, 2]   # fixture pages in a batch order that interleaves the sizes (page 0 and 4 share one)
 PROB_RTOL = 1e-5
 
-_MODELS = {}
 
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def spot_model(gold, workspace_mb=4096):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed'][0]), float(gold['pt_eos_bias'][0])), OmniVocab(),
-                                         workspace_mb=workspace_mb)
-    m = _MODELS['spot']
-    m.vocab.pt_seq_length = int(gold['pt_seq_length'][0])
-    m.vocab.rec_length = int(gold['rec_length'][0])
-    m.ctx.set_option('xattn_impl', 0)
-    return m
+def spot_model(gold):
+    return omni_model({k: gold[k][0] for k in ('wseed', 'pt_eos_bias', 'pt_seq_length', 'rec_length')})
 
 
 def canvas(pages):
@@ -78,9 +61,9 @@ def test_mixed_batch_matches_the_reference_fixture(golden_dir, impl):
     from advancedliteratemachinery_b200 import NestedTensor
     gold = pages_case(golden_dir)
     m = spot_model(gold)
-    m.ctx.set_option('xattn_impl', impl)   # before the encode: xattn_impl 1 needs its V_c^T
-    pages, (t, mask) = fixture_batch(gold)
-    outs = m.forward_pages(NestedTensor(t.cuda(), mask.cuda()))
+    with options(m.ctx, xattn_impl=impl):   # before the encode: xattn_impl 1 needs its V_c^T
+        pages, (t, mask) = fixture_batch(gold)
+        outs = m.forward_pages(NestedTensor(t.cuda(), mask.cuda()))
     assert len(outs) == len(ORDER)
     shapes = m.page_shapes()
     mem, pos = m.memory(0), m.memory(1)
@@ -209,8 +192,7 @@ def test_config2_page_inside_a_batch_of_page_sizes(golden_dir):
     from oracle.gen_golden import CONFIG2_CASE, config2_page
     from tests.conftest import omni_sd
     from tests.test_gpu_omniparser import MAX_NEAR_TIE_FLIPS, _judge_flips
-    for key in list(_MODELS):
-        _MODELS.pop(key).ctx.close()
+    close_models()
     case = CONFIG2_CASE
     gold = np.load(os.path.join(golden_dir, 'omni_config2_page0.npz'))
     sd = omni_sd(case['wseed'], case['pt_eos_bias'])

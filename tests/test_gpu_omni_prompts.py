@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import close_models, omni_model, options, release_models
 from tests.test_prompts_cpu import prompt_case, prompt_page
 
 pytestmark = pytest.mark.gpu
@@ -15,7 +16,6 @@ torch.set_grad_enabled(False)
 LOGIT_REL_TOL = 1e-3
 ALM_ERR_INVALID, ALM_ERR_OOM, ALM_ERR_STATE = -1, -3, -4
 
-_MODEL = {}
 
 
 def _maxrel(a, b):
@@ -25,22 +25,8 @@ def _maxrel(a, b):
 
 def fixture_model(gold, workspace_mb=8192):
     """One resident OmniParserB200 on the fixture's checkpoint, decode lengths of the fixture."""
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'm' not in _MODEL:
-        _MODEL['m'] = OmniParserB200(omni_sd(int(gold['wseed'][0]), float(gold['pt_eos_bias'][0])), OmniVocab(),
-                                     workspace_mb=workspace_mb)
-    m = _MODEL['m']
-    m.vocab.pt_seq_length = int(gold['pt_seq_length'][0])
-    m.vocab.rec_length = int(gold['rec_length'][0])
-    return m
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_model():
-    yield
-    if 'm' in _MODEL:
-        _MODEL.pop('m').ctx.close()
+    return omni_model({k: gold[k][0] for k in ('wseed', 'pt_eos_bias', 'pt_seq_length', 'rec_length')},
+                      workspace_mb=workspace_mb)
 
 
 def fixture_pages(gold):
@@ -152,12 +138,9 @@ def test_window_prompts_under_the_other_cross_attention_kernels(impl, golden_dir
     gold = prompt_case(golden_dir)
     m = fixture_model(gold)
     imgs, masks = fixture_pages(gold)
-    try:
-        m.ctx.set_option('xattn_impl', impl)
+    with options(m.ctx, xattn_impl=impl):
         m.encode(imgs.cuda(), masks.cuda())   # xattn_impl 1 needs its V_c^T built by the encode
         check_against_fixture(m, gold, m.decode_prompts(torch.from_numpy(gold['prompts'])))
-    finally:
-        m.ctx.set_option('xattn_impl', 0)
 
 
 def _raw_decode_prompts(m, prompts, P, n_prompt, max_instances=None):
@@ -178,8 +161,6 @@ def test_error_paths(golden_dir):
     from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
     from advancedliteratemachinery_b200 import synthetic as W
     gold = prompt_case(golden_dir)
-    if 'm' in _MODEL:
-        _MODEL.pop('m').ctx.close()
     m = fixture_model(gold, workspace_mb=1024)
     v = m.vocab
     glob = v.pt_prompt()
@@ -205,14 +186,11 @@ def test_error_paths(golden_dir):
         v.pt_seq_length = int(gold['pt_seq_length'][0])
         m.encode(imgs.cuda(), masks.cuda())
         assert _raw_decode_prompts(m, two, 1, 7) == 0                             # the context stays usable
-        m.ctx.set_option('kv_decoders', 1)
-        try:
+        with options(m.ctx, kv_decoders=1):
             m.encode(imgs.cuda(), masks.cuda())
             assert _raw_decode_prompts(m, two, 1, 7) == ALM_ERR_STATE
-        finally:
-            m.ctx.set_option('kv_decoders', 3)
     finally:
-        _MODEL.pop('m').ctx.close()
+        close_models()
     kv = OmniVocab(vie_categories=4, pt_seq_length=9)
     k = OmniParserB200(W.omniparser_state_dict(seed=2, vie_categories=4, pt_eos_bias=-30.0), kv, workspace_mb=1024)
     try:

@@ -31,6 +31,7 @@ import ctypes
 import pytest
 import torch
 
+from tests.support import options
 from tests.test_gpu_encoder_ops import _fpn_err_tol, _joined, _stage_grids, _wattn_tol
 from tests.test_gpu_mgp_replay import _Checker, _epi, _Lin, _opd, _Pool
 from tests.test_gpu_omniparser import window_attention_ref64
@@ -456,15 +457,10 @@ def test_replay_is_the_encoder_bit_for_bit(case, ns, impl):
     img, mask, sizes = _case(case)
     label = f'{case} nsplit {ns} wattn_impl {impl}'
     chk = _EncChecker(ns, label, border=case == 'page')
-    try:
-        ctx.set_option('nsplit', ns)
-        ctx.set_option('wattn_impl', impl)
+    with options(ctx, nsplit=ns, wattn_impl=impl):
         rp = _Replay(ctx, w, ns, chk)
         if sizes is None:
             _run_single(m, rp, img, mask, label)
         else:
             _run_pages(m, rp, img, sizes, label)
         chk.report()
-    finally:
-        ctx.set_option('nsplit', 3)
-        ctx.set_option('wattn_impl', 3)

@@ -13,10 +13,15 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import close_models, ctx, omni_model, options, release_models
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
 LOGIT_REL_TOL = 1e-3
+# the op tests need little; the library default (24 GB), held for the whole module, would leave no room for the three
+# 20 GB contexts of the config-2 test on an 80 GB card
+WORKSPACE_MB = 4096
 
 
 def _rel(a, b):
@@ -29,30 +34,9 @@ def _maxrel(a, b):
     return float((a - b).abs().max() / (b.abs().max() + 1e-30))
 
 
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    # the op tests need little; the library default (24 GB), held for the whole module, would leave no room for the
-    # three 20 GB contexts of the config-2 test on an 80 GB card
-    c.set_option('workspace_mb', 4096)
-    return c
-
-
-_MODELS = {}
-
-
 def model_for(wseed, pt_eos_bias):
     """One resident OmniParserB200 per synthetic checkpoint (weights are 0.9 GB on the device)."""
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    key = (wseed, pt_eos_bias)
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(omni_sd(wseed, pt_eos_bias), OmniVocab(), workspace_mb=8192)
-    return _MODELS[key]
+    return omni_model(dict(wseed=wseed, pt_eos_bias=pt_eos_bias), workspace_mb=8192)
 
 
 # ----------------------------------------------------------------------------------------------- ops
@@ -67,15 +51,12 @@ def test_linear_tcgen05_matches_fp64(ctx, M, N, K, act, batch):
     ref = torch.nn.functional.gelu(ref) if act == 1 else (torch.relu(ref) if act == 2 else ref)
     Ad, Wd, bd = A.cuda(), Wt.cuda(), b.cuda()
     for nsplit, tol in ((3, 2e-5), (1, 6e-3)):
-        ctx.set_option('nsplit', nsplit)
         for impl in (0, 1):  # tensor-core kernel and the SIMT debug kernel must agree with fp64
-            ctx.set_option('gemm_impl', impl)
-            out = torch.full((batch, M, N), float('nan'), device='cuda')
-            ctx.check(ctx.lib.alm_op_linear(ctx.h, Ad.data_ptr(), Wd.data_ptr(), bd.data_ptr(), out.data_ptr(), M, N, K,
-                                            act, batch))
-            assert _rel(out.cpu(), ref) < tol, (nsplit, impl)
-    ctx.set_option('nsplit', 3)
-    ctx.set_option('gemm_impl', 0)
+            with options(ctx, nsplit=nsplit, gemm_impl=impl):
+                out = torch.full((batch, M, N), float('nan'), device='cuda')
+                ctx.check(ctx.lib.alm_op_linear(ctx.h, Ad.data_ptr(), Wd.data_ptr(), bd.data_ptr(), out.data_ptr(), M,
+                                                N, K, act, batch))
+                assert _rel(out.cpu(), ref) < tol, (nsplit, impl)
 
 
 # Swin stages and merges (128 .. 2048), MGP-STR tiny / small / base / large (192 is its own gather_ln_kernel<2, 192>
@@ -128,12 +109,11 @@ def test_window_attention_core(ctx, B, nWh, nWw, heads, shift):
     qd, td = qkv.cuda(), tab.cuda()
     # mma.sync kernel, fp32 SIMT debug kernel, persistent TMA-fed mma.sync kernel over head pairs
     for impl, tol in ((0, 5e-5), (1, 5e-6), (3, 5e-5)):
-        ctx.set_option('wattn_impl', impl)
-        out = torch.full((rows, C), float('nan'), device='cuda')
-        ctx.check(ctx.lib.alm_op_window_attention(ctx.h, qd.data_ptr(), td.data_ptr(), out.data_ptr(), B, nWh, nWw, C,
-                                                  heads, shift))
-        assert float((out.cpu() - ref).abs().max()) < tol, impl
-    ctx.set_option('wattn_impl', 3)   # back to the default
+        with options(ctx, wattn_impl=impl):
+            out = torch.full((rows, C), float('nan'), device='cuda')
+            ctx.check(ctx.lib.alm_op_window_attention(ctx.h, qd.data_ptr(), td.data_ptr(), out.data_ptr(), B, nWh, nWw,
+                                                      C, heads, shift))
+            assert float((out.cpu() - ref).abs().max()) < tol, impl
 
 
 # ----------------------------------------------------------------------------------------------- model
@@ -272,14 +252,11 @@ def test_single_pass_bf16_mode_is_close_but_not_the_parity_mode(golden_dir):
     case = OMNI_CASES['full']
     gold = np.load(os.path.join(golden_dir, 'omni_full.npz'))
     m = model_for(case['wseed'], case['pt_eos_bias'])
-    m.ctx.set_option('nsplit', 1)
-    try:
+    with options(m.ctx, nsplit=1):
         img, mask = omni_inputs(case)
         m.encode(img, mask)
         r = _rel(m.memory(0)[0], torch.from_numpy(gold['memory']))
         assert 1e-4 < r < 5e-2, r
-    finally:
-        m.ctx.set_option('nsplit', 3)
 
 
 def test_error_paths():
@@ -302,8 +279,7 @@ def test_kie_decode_matches_reference_fixture(golden_dir):
     from oracle.gen_golden import KIE_CASES, omni_inputs
     case = KIE_CASES['kie']
     gold = np.load(os.path.join(golden_dir, 'omni_kie.npz'))
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
+    close_models()
     sd = W.omniparser_state_dict(seed=case['wseed'], vie_categories=case['vie'], pt_eos_bias=case['pt_eos_bias'])
     v = OmniVocab(vie_categories=case['vie'], pt_seq_length=case['pt_seq_length'], rec_length=case['rec_length'])
     m = OmniParserB200(sd, v, workspace_mb=8192)
@@ -365,14 +341,11 @@ def test_fused_cross_attention_matches_gemm_path_and_oracle():
     assert bool(kpm_o[0].any()) and not bool(kpm_o[0].all())
     ref = O.decode_logits(seq[:8], mem_o[0], kpm_o[0], pos_o[0], sd, 'rec')
     lg = {0: {}, 1: {}}
-    try:
-        for impl in (1, 0):  # the unfused path needs its feature-major V_c^T built by the encode
-            m.ctx.set_option('xattn_impl', impl)
+    for impl in (1, 0):  # the unfused path needs its feature-major V_c^T built by the encode
+        with options(m.ctx, xattn_impl=impl):
             m.encode(img, mask)
             for n in (70, 10, 1):
                 lg[impl][n] = m.decode_logits(0, 'rec', seq[:n])
-    finally:
-        m.ctx.set_option('xattn_impl', 0)
     for n in (70, 10, 1):
         assert torch.isfinite(lg[0][n]).all()
         assert _maxrel(lg[0][n], lg[1][n]) < 2e-5, (n, _maxrel(lg[0][n], lg[1][n]))
@@ -381,13 +354,8 @@ def test_fused_cross_attention_matches_gemm_path_and_oracle():
         assert _rel(lg[0][n][:k], ref[:k]) < 1e-4
         # the two self-attention step kernels (CTA per (sequence, head) for few sequences / warp per pair) and the
         # fused kernel's 2 vs 3 CTAs per SM schedules agree as well
-        try:
-            m.ctx.set_option('sattn_wide', 0)
-            m.ctx.set_option('xattn_ctas_per_sm', 3)
+        with options(m.ctx, sattn_wide=0, xattn_ctas_per_sm=3):
             alt = m.decode_logits(0, 'rec', seq[:n])
-        finally:
-            m.ctx.set_option('sattn_wide', 1)
-            m.ctx.set_option('xattn_ctas_per_sm', 2)
         assert _maxrel(lg[0][n], alt) < 2e-5, (n, _maxrel(lg[0][n], alt))
 
 
@@ -408,11 +376,8 @@ def test_fused_cross_attention_8warp_variant_matches():
     for image in (0, 1):
         for n in (70, 33):
             ref = m.decode_logits(image, 'rec', seq[:n])
-            try:
-                m.ctx.set_option('xattn_wg', 2)
+            with options(m.ctx, xattn_wg=2):
                 alt = m.decode_logits(image, 'rec', seq[:n])
-            finally:
-                m.ctx.set_option('xattn_wg', 1)
             assert torch.isfinite(alt).all()
             assert _maxrel(alt, ref) < 2e-5, (image, n, _maxrel(alt, ref))
 
@@ -454,27 +419,24 @@ def test_tma_cross_attention_variant_matches_the_default_kernel(impl):
     seq = torch.cat([torch.randint(0, v.num_bins, (70, 2), generator=g), torch.full((70, 1), v.rec_sos_index),
                      torch.randint(v.num_bins, v.recog_pad_index, (70, 2), generator=g)], 1)
     m.encode(img, mask)
-    try:
-        for image in (0, 1):
-            for n in (70, 33, 10, 1):
-                m.ctx.set_option('xattn_impl', 0)
+    for image in (0, 1):
+        for n in (70, 33, 10, 1):
+            with options(m.ctx, xattn_impl=0):
                 ref = m.decode_logits(image, 'rec', seq[:n])
-                m.ctx.set_option('xattn_impl', impl)
+            with options(m.ctx, xattn_impl=impl):
                 alt = m.decode_logits(image, 'rec', seq[:n])
-                assert torch.isfinite(alt).all()
-                assert _maxrel(alt, ref) < 2e-5, (image, n, _maxrel(alt, ref))
-        m.vocab.pt_seq_length = 6
-        m.ctx.set_option('xattn_impl', 0)
+            assert torch.isfinite(alt).all()
+            assert _maxrel(alt, ref) < 2e-5, (image, n, _maxrel(alt, ref))
+    m.vocab.pt_seq_length = 6
+    with options(m.ctx, xattn_impl=0):
         a = m.forward_batch(NestedTensor(img.cuda(), mask.cuda()))
-        m.ctx.set_option('xattn_impl', impl)
+    with options(m.ctx, xattn_impl=impl):
         b = m.forward_batch(NestedTensor(img.cuda(), mask.cuda()))
-        for x, y in zip(a, b):
-            assert (x is None) == (y is None)
-            if x is not None:
-                for p, q in zip(x[0], y[0]):
-                    assert torch.equal(p, q)
-    finally:
-        m.ctx.set_option('xattn_impl', 0)
+    for x, y in zip(a, b):
+        assert (x is None) == (y is None)
+        if x is not None:
+            for p, q in zip(x[0], y[0]):
+                assert torch.equal(p, q)
 
 
 def test_config5_geometry_largest_page_and_long_point_sequence():
@@ -549,8 +511,7 @@ def test_config2_scale_decode_matches_the_reference(golden_dir):
     case = CONFIG2_CASE
     gold = np.load(os.path.join(golden_dir, 'omni_config2_page0.npz'))
     sd = omni_sd(case['wseed'], case['pt_eos_bias'])
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
+    close_models()
     v = OmniVocab(pt_seq_length=case['pt_seq_length'], rec_length=case['rec_length'])
     m = OmniParserB200(sd, v, workspace_mb=20480)
     img, mask = config2_page(case['seed'])
@@ -664,8 +625,7 @@ def test_shared_weights_contexts_and_stream_ordered_device_inputs():
     the call are ordered by alm_stream_wait inside the adapter."""
     from advancedliteratemachinery_b200 import NestedTensor, OmniParserB200, OmniVocab
     from tests.conftest import omni_sd
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
+    close_models()
     free0 = torch.cuda.mem_get_info()[0]
     v = OmniVocab(pt_seq_length=6)
     owner = OmniParserB200(omni_sd(0, 0.45), v, workspace_mb=4096)
@@ -756,13 +716,10 @@ def test_ln_fused_gemv_point_loop_is_bit_identical():
     imgs = torch.randn(3, 3, 128, 160, generator=g)
     seq = torch.cat([m.vocab.pt_prompt(), torch.randint(0, 1000, (1, 9), generator=g)], 1)
     res = {}
-    try:
-        for f in (0, 1):
-            m.ctx.set_option('fuse_ln_gemv', f)
+    for f in (0, 1):
+        with options(m.ctx, fuse_ln_gemv=f):
             outs = m.forward_batch(NestedTensor(imgs, None))
             res[f] = (outs, m.decode_logits(1, 'pt', seq))
-    finally:
-        m.ctx.set_option('fuse_ln_gemv', 1)
     assert torch.equal(res[0][1], res[1][1])
     for a, b in zip(res[0][0], res[1][0]):
         assert (a is None) == (b is None)

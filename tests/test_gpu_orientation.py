@@ -6,8 +6,10 @@ import numpy as np
 import pytest
 import torch
 
+from tests import support
+from tests.support import mgp_model, release_models
 from tests.test_curve_crops_cpu import curve_fixture, random_polygons
-from tests.test_orientation_cpu import CHAR_TABLE, emu_turned_crops
+from tests.test_orientation_cpu import CHAR_TABLE, bind, emu_turned_crops
 from tests.test_quad_crops_cpu import quad_fixture, random_quads
 
 pytestmark = pytest.mark.gpu
@@ -18,17 +20,12 @@ WP = [f'w{i}' for i in range(102)] + ['[SEP]'] + [f'w{i}' for i in range(103, 30
 
 @pytest.fixture(scope='module')
 def model():
-    from advancedliteratemachinery_b200 import MGPSTRB200
-    from tests.conftest import mgp_sd
-    m = MGPSTRB200(mgp_sd(0))
-    yield m
-    m.ctx.close()
+    return mgp_model()
 
 
 @pytest.fixture(scope='module')
 def emu():
-    from tests.test_orientation_cpu import build_emu
-    return build_emu()
+    return support.emu('orient_emu', bind)
 
 
 def bits(a, b):

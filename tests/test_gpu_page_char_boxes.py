@@ -4,14 +4,13 @@ of the same bodies (tests/emu/rec_box_emu.cpp) in every field, bit for bit, on t
 tests/test_page_char_boxes_cpu.py and at 16 pages x 4 096 words in one launch; a page read turned must give the boxes
 of np.rot90(page, k) read upright, mapped by the rule, bit for bit; locations must change nothing else; every word's
 boxes must come from the reading the merges kept; and rec_locations=False must be today's path."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import rec_box_ref as R
 from oracle.whole_page_ref import map_back
+from tests.support import ctx, golden, kw, omni_model, release_models
 from tests.test_page_char_boxes_cpu import (EOS, KEYS, PAD, assert_same, emu_boxes, fabricate, frames_to_tiles,
                                            hand_made_words)
 
@@ -20,54 +19,18 @@ torch.set_grad_enabled(False)
 
 ERR_INVALID = -1  # include/alm_ocr.h ALM_ERR_INVALID
 
-_MODELS = {}
 
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        m = _MODELS.pop(k)
-        (m if k == 'ctx' else m.ctx).close()
-
-
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    if 'ctx' not in _MODELS:
-        _MODELS['ctx'] = _lib.Context(0)
-    return _MODELS['ctx']
-
-
-def device(polys, rec, loc, fi, frames):
+def device(ctx, polys, rec, loc, fi, frames):
     from advancedliteratemachinery_b200.omniparser import char_boxes
     sizes, tiles, turns = frames_to_tiles(frames)
-    return char_boxes(ctx(), sizes, tiles, polys, rec, loc, fi, PAD, EOS, turns=turns)
+    return char_boxes(ctx, sizes, tiles, polys, rec, loc, fi, PAD, EOS, turns=turns)
 
 
-def gold_of(golden_dir, name):
-    return np.load(os.path.join(golden_dir, name))
-
-
-def model(gold):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed']), float(gold['pt_eos_bias'])),
-                                         OmniVocab(pt_seq_length=int(gold['pt_seq_length']),
-                                                   rec_length=int(gold['rec_length'])), workspace_mb=4096)
-    return _MODELS['spot']
-
-
-def kw(gold, **extra):
-    return dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-                test_max_size=int(gold['test_max_size']), **extra)
-
-
-def pages(golden_dir):
+def pages():
     """The fixture pages of omni_tiles.npz (2 x 3 tiles) and omni_page_turns.npz (two tiles upright, two turned), a page
     of one tile and one of 2 x 3 tiles of noise."""
     rng = np.random.default_rng(5)
-    return [gold_of(golden_dir, 'omni_tiles.npz')['page'], gold_of(golden_dir, 'omni_page_turns.npz')['page'],
+    return [golden('omni_tiles.npz')['page'], golden('omni_page_turns.npz')['page'],
             rng.integers(0, 256, (97, 120, 3), dtype=np.uint8), rng.integers(0, 256, (230, 301, 3), dtype=np.uint8)]
 
 
@@ -96,43 +59,44 @@ def oracle_chars(m, sizes, plan, turns, polys, rec, loc, tile_index):
 
 # ---- the entry against the host build
 
+
 @pytest.mark.parametrize('seed', range(3))
-def test_device_equals_the_emulation_on_fabricated_words(seed):
+def test_device_equals_the_emulation_on_fabricated_words(ctx, seed):
     args = fabricate(seed)
-    n0 = ctx().launch_count()
-    assert_same(device(*args), emu_boxes(*args))
-    assert ctx().launch_count() == n0 + 1
+    n0 = ctx.launch_count()
+    assert_same(device(ctx, *args), emu_boxes(*args))
+    assert ctx.launch_count() == n0 + 1
 
 
 @pytest.mark.parametrize('L', [1, 1021])
-def test_device_equals_the_emulation_at_the_rec_length_bounds(L):
+def test_device_equals_the_emulation_at_the_rec_length_bounds(ctx, L):
     args = fabricate(10 + L, N=24 if L > 1 else 200, L=L)
-    assert_same(device(*args), emu_boxes(*args))
+    assert_same(device(ctx, *args), emu_boxes(*args))
 
 
-def test_device_equals_the_emulation_on_hand_made_words():
+def test_device_equals_the_emulation_on_hand_made_words(ctx):
     args = hand_made_words()
-    assert_same(device(*args), emu_boxes(*args))
+    assert_same(device(ctx, *args), emu_boxes(*args))
 
 
-def test_device_equals_the_emulation_at_16_pages_x_4096_words_in_one_launch():
+def test_device_equals_the_emulation_at_16_pages_x_4096_words_in_one_launch(ctx):
     polys, rec, loc, fi, frames = fabricate(99, N=16 * 4096, F=16 * 12, nan=0.001)
-    n0 = ctx().launch_count()
-    got = device(polys, rec, loc, fi, frames)
-    assert ctx().launch_count() == n0 + 1
+    n0 = ctx.launch_count()
+    got = device(ctx, polys, rec, loc, fi, frames)
+    assert ctx.launch_count() == n0 + 1
     assert_same(got, emu_boxes(polys, rec, loc, fi, frames))
     assert int(got['n_chars'].sum()) > 16 * 4096 * 5
 
 
-def test_no_words_no_launch():
+def test_no_words_no_launch(ctx):
     args = fabricate(1, N=0)
-    n0 = ctx().launch_count()
-    got = device(*args)
-    assert ctx().launch_count() == n0 and got['n_chars'].shape == (0,)
+    n0 = ctx.launch_count()
+    got = device(ctx, *args)
+    assert ctx.launch_count() == n0 and got['n_chars'].shape == (0,)
 
 
-def test_refusals_return_invalid_and_leave_the_context_usable():
-    c = ctx()
+def test_refusals_return_invalid_and_leave_the_context_usable(ctx):
+    c = ctx
     polys, rec, loc, fi, frames = fabricate(4, N=8)
     frames = np.ascontiguousarray(frames, np.int32)
     N, L = rec.shape
@@ -170,12 +134,13 @@ def test_refusals_return_invalid_and_leave_the_context_usable():
 
 # ---- spot_tiled and read_regions
 
-def test_turned_pages_give_the_boxes_of_the_turned_page_read_upright(golden_dir):
+
+def test_turned_pages_give_the_boxes_of_the_turned_page_read_upright():
     """Turn k of the two fixture pages: the words' 'chars' equal the rule applied to np.rot90(page, k) read upright
     (its polygons mapped to the page, its ids and locations), bit for bit: the turned tiles are pixel permutations."""
-    gold = gold_of(golden_dir, 'omni_page_turns.npz')
-    m = model(gold)
-    for page in pages(golden_dir)[:2]:
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
+    for page in pages()[:2]:
         H, W = page.shape[:2]
         for k in range(4):
             got = m.spot_tiled([page], orientation=[k], rec_locations=True, **kw(gold))[0]
@@ -192,10 +157,10 @@ def test_turned_pages_give_the_boxes_of_the_turned_page_read_upright(golden_dir)
                 same_chars(d['chars'], w_)
 
 
-def test_locations_change_nothing_else(golden_dir):
-    gold = gold_of(golden_dir, 'omni_page_turns.npz')
-    m = model(gold)
-    pg = pages(golden_dir)
+def test_locations_change_nothing_else():
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
+    pg = pages()
     for orientation in ['upright', [1, 0, 3, 2], 'auto', 'mixed']:
         off = m.spot_tiled(pg, orientation=orientation, **kw(gold))
         on = m.spot_tiled(pg, orientation=orientation, rec_locations=True, **kw(gold))
@@ -205,12 +170,12 @@ def test_locations_change_nothing_else(golden_dir):
 
 
 @pytest.mark.parametrize('orientation', ['auto', 'mixed', 'upright'])
-def test_chars_come_from_the_kept_reading(golden_dir, orientation):
+def test_chars_come_from_the_kept_reading(orientation):
     """Each word's 'chars' are the rule applied to the locations of the tile instance its 'tile' / 'instance' (and,
     for 'mixed', 'turns') name; 'auto' reads the one-tile page from its probe.  max_batch 1 / 5 / 16 agree."""
-    gold = gold_of(golden_dir, 'omni_page_turns.npz')
-    m = model(gold)
-    pg = pages(golden_dir)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
+    pg = pages()
     sizes = [p.shape[:2] for p in pg]
     res = m.spot_tiled(pg, orientation=orientation, max_batch=5, rec_locations=True, **kw(gold))
     t = m.last_tiles
@@ -245,12 +210,12 @@ def test_chars_come_from_the_kept_reading(golden_dir, orientation):
                     assert np.abs(ca['box'] - cb['box']).max() <= 0.1
 
 
-def test_read_regions_at_decode_points_gives_spot_tiled_chars(golden_dir):
+def test_read_regions_at_decode_points_gives_spot_tiled_chars():
     """On a page of one tile, read_regions at the words' own points reproduces the decode (read_at), so its 'chars'
     equal spot_tiled's bit for bit; on the larger pages each region's chars follow the rule in its own frame."""
-    gold = gold_of(golden_dir, 'omni_page_turns.npz')
-    m = model(gold)
-    pg = pages(golden_dir)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
+    pg = pages()
     res = m.spot_tiled([pg[2]], rec_locations=True, **kw(gold))[0]
     assert res
     pts = np.array([d['pts'][0] for d in res])
@@ -282,12 +247,12 @@ def test_read_regions_at_decode_points_gives_spot_tiled_chars(golden_dir):
         same_chars(d['chars'], w_)
 
 
-def test_off_by_default_and_refusals(golden_dir):
+def test_off_by_default_and_refusals():
     """rec_locations=False is the default: the same words and launches; with locations on, launches are added, and a
     later call without them is back to the default's words and launches."""
-    gold = gold_of(golden_dir, 'omni_page_turns.npz')
-    m = model(gold)
-    pg = pages(golden_dir)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
+    pg = pages()
 
     def run(**extra):
         n0 = m.ctx.launch_count()

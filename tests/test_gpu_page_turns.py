@@ -4,46 +4,17 @@ bit for bit; a page read at turn k must equal spot_tiled of np.rot90(page, k) wi
 oracle/page_turn_ref.py; 'upright' and all-zero turns must be today's result; 'auto' must choose what the oracle
 chooses from the device's own probe readings and then equal the explicit reading at that turn; and
 tests/golden/omni_page_turns.npz (the unmodified reference on np.rot90 of a page) must be reproduced."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import page_turn_ref as R
+from tests.support import assert_same, golden, kw, omni_model, release_models, same
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
 ERR_INVALID = -1  # include/alm_ocr.h ALM_ERR_INVALID
-
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def fixture(golden_dir):
-    return np.load(os.path.join(golden_dir, 'omni_page_turns.npz'))
-
-
-def model(gold):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed']), float(gold['pt_eos_bias'])),
-                                         OmniVocab(pt_seq_length=int(gold['pt_seq_length']),
-                                                   rec_length=int(gold['rec_length'])), workspace_mb=4096)
-    return _MODELS['spot']
-
-
-def kw(gold, **extra):
-    return dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-                test_max_size=int(gold['test_max_size']), **extra)
 
 
 def pages(gold):
@@ -64,11 +35,6 @@ def mapped(res, k, H, W):
         e['turns'] = k
         out.append(e)
     return out
-
-
-def same(a, b):
-    """Two spot_tiled results are equal, floats bit for bit (== on Python floats, with the keys in order)."""
-    assert [[list(d.items()) for d in r] for r in a] == [[list(d.items()) for d in r] for r in b]
 
 
 def test_turned_tile_inputs_equal_omni_tiles_of_turned_pages():
@@ -93,11 +59,11 @@ def test_turned_tile_inputs_equal_omni_tiles_of_turned_pages():
         ctx.close()
 
 
-def test_explicit_turns_equal_the_rotated_pages_mapped_back(golden_dir):
+def test_explicit_turns_equal_the_rotated_pages_mapped_back():
     """Every page at every turn: spot_tiled(orientation=turns) equals spot_tiled of np.rot90(page, k) with the rows
     mapped back by the oracle, in every field (vertex j maps to vertex j: the order is kept)."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = pages(gold)
     for turns in ([1, 2, 3], [3, 0, 2], [2, 3, 1]):
         got = m.spot_tiled(pg, max_batch=1, orientation=np.array(turns), **kw(gold))
@@ -111,14 +77,13 @@ def test_explicit_turns_equal_the_rotated_pages_mapped_back(golden_dir):
          m.spot_tiled(pg, max_batch=1, orientation=[1, 2, 3], **kw(gold)))
 
 
-def test_the_fixture_at_every_turn(golden_dir):
+def test_the_fixture_at_every_turn():
     """The fixture page read at turns 0..3 as four pages: tile decodes equal the reference's (ids exact,
     probabilities close), the merge equals the oracle's (coordinates exact), and the device merge equals the host build
     fed the device's own tile outputs."""
     from tests.test_page_turns_cpu import emu_merge_turned
-    from tests.test_tiles_cpu import assert_same
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     page = gold['page']
     m.spot_tiled([page] * 4, orientation=[0, 1, 2, 3], **kw(gold))
     t = m.last_tiles
@@ -133,10 +98,10 @@ def test_the_fixture_at_every_turn(golden_dir):
                                               t['prob'], m.vocab.num_bins))
 
 
-def test_upright_and_zero_turns_are_todays_result(golden_dir):
+def test_upright_and_zero_turns_are_todays_result():
     """'upright' is the default path (no new keys, same last_tiles); all-zero turns give the same rows bit for bit."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = pages(gold)
     base = m.spot_tiled(pg, **kw(gold))
     t0 = m.last_tiles
@@ -148,14 +113,14 @@ def test_upright_and_zero_turns_are_todays_result(golden_dir):
     same(zero, [[dict(d, turns=0) for d in r] for r in base])
 
 
-def test_auto_chooses_what_the_oracle_chooses_and_reads_at_that_turn(golden_dir):
+def test_auto_chooses_what_the_oracle_chooses_and_reads_at_that_turn():
     """'auto': the probe readings are the reference's on the fixture page; turns and page_scores equal the oracle's
     choice from the device's own probe readings; the result equals explicit-turn spot_tiled at the chosen turns (a
     page of several tiles read again in tiles, the others kept from their probe); only P turns and P x 4 scores come
     back from the one-launch selection."""
     from advancedliteratemachinery_b200.omniparser import orient_select
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     v = m.vocab
     pg = pages(gold)
     P = len(pg)
@@ -181,11 +146,11 @@ def test_auto_chooses_what_the_oracle_chooses_and_reads_at_that_turn(golden_dir)
     assert np.array_equal(turns, t['turns']) and np.array_equal(scores, t['page_scores'])
 
 
-def test_auto_on_many_pages_and_chunks(golden_dir):
+def test_auto_on_many_pages_and_chunks():
     """'auto' over several chunks equals 'auto' one page at a time, and the selection at scale equals the oracle."""
     from advancedliteratemachinery_b200.omniparser import orient_select
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = pages(gold)
     same(m.spot_tiled(pg, max_batch=3, orientation='auto', **kw(gold)),
          [m.spot_tiled([p], max_batch=3, orientation='auto', **kw(gold))[0] for p in pg])
@@ -200,14 +165,14 @@ def test_auto_on_many_pages_and_chunks(golden_dir):
     assert np.array_equal(turns, want_t) and np.array_equal(scores.view(np.uint64), want_s.view(np.uint64))
 
 
-def test_error_paths_leave_the_context_usable(golden_dir):
+def test_error_paths_leave_the_context_usable():
     """Unknown orientation strings, turns of the wrong length or outside 0..3 and a KIE checkpoint raise ValueError;
     the C entries refuse bad turns and bad counts before any device work; the context reads correctly afterwards."""
     import ctypes as C
     from advancedliteratemachinery_b200 import OmniParserB200, _lib, preprocess as Pre
     from advancedliteratemachinery_b200.omniparser import merge_tiles
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_page_turns.npz')
+    m = omni_model(gold)
     pg = pages(gold)
     for bad in ('sideways', 'Auto', [0, 1], [0, 1, 4], [0, -1, 0], np.zeros(3)):
         with pytest.raises(ValueError):

@@ -14,6 +14,8 @@ import ctypes
 import pytest
 import torch
 
+from tests.support import ctx, options
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
@@ -32,15 +34,6 @@ SHAPES = [
     (40, 512, 512, ACT_NONE, True, False),
     (300, 2048, 512, ACT_RELU, False, True),
 ]
-
-
-@pytest.fixture(scope='module')
-def ctx():
-    from advancedliteratemachinery_b200 import _lib
-    assert torch.cuda.is_available(), 'GPU tests need an H100; there is no CPU fallback to test'
-    c = _lib.Context(0)
-    yield c
-    c.set_option('nsplit', 3)
 
 
 def _planes(x):
@@ -71,7 +64,6 @@ def _call(ctx, a, b, e):
 def test_joint_linear_is_two_single_linears(ctx, shape, nsplit):
     from advancedliteratemachinery_b200 import _lib
     S, N, K, act, resid, split = shape
-    ctx.set_option('nsplit', nsplit)
     g = torch.Generator().manual_seed(S * 7 + N * 3 + K)
     A = _planes(torch.randn(2 * S, K, generator=g)).cuda()
     W = _planes(torch.randn(2 * N, K, generator=g) * K ** -0.5).cuda()
@@ -103,8 +95,9 @@ def test_joint_linear_is_two_single_linears(ctx, shape, nsplit):
         torch.cuda.synchronize()
         return out, planes
 
-    joint, joint_planes = run(True)
-    single, single_planes = run(False)
+    with options(ctx, nsplit=nsplit):
+        joint, joint_planes = run(True)
+        single, single_planes = run(False)
     assert not torch.isnan(single).any()
     assert torch.equal(joint.view(torch.int32), single.view(torch.int32)), 'joint GEMM differs from the two single GEMMs'
     if split:

@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_quad_crops_cpu import build_emu, emu_quad_crops, quad_fixture, text_regions
+from tests.support import emu
+from tests.test_quad_crops_cpu import bind, emu_quad_crops, quad_fixture, text_regions
 
 pytestmark = pytest.mark.gpu
 ALM_ERR_INVALID = -1
@@ -26,7 +27,7 @@ def test_thousand_regions_equal_host_emulation():
     """16 pages of 1024 x 1024, 64 regions each: every output bit equals the host run of the kernel bodies."""
     from advancedliteratemachinery_b200 import _lib, preprocess as P
     pages, quads, pidx = text_regions(seed=7)
-    _, _, ref = emu_quad_crops(build_emu(), pages, quads, pidx)
+    _, _, ref = emu_quad_crops(emu('quad_emu', bind), pages, quads, pidx)
     ctx = _lib.Context(0)
     got = P.quad_crops(ctx, [torch.from_numpy(p).cuda() for p in pages], quads, pidx)
     assert np.array_equal(got.cpu().numpy().view(np.uint32), ref.view(np.uint32))

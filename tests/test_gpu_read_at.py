@@ -13,33 +13,15 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import golden, kw, omni_model, options, release_models
 from tests.test_read_at_cpu import brute_route
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
 ERR_INVALID, ERR_STATE = -1, -4
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
 def spot_model(wseed=0, pt_eos_bias=-30.0, pt_seq_length=8, rec_length=25):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    key = (wseed, pt_eos_bias)
-    if key not in _MODELS:
-        for k in [k for k in _MODELS if k != 'kie']:
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(omni_sd(wseed, pt_eos_bias), OmniVocab(), workspace_mb=4096)
-    m = _MODELS[key]
-    m.vocab.pt_seq_length, m.vocab.rec_length = pt_seq_length, rec_length
-    return m
+    return omni_model(dict(wseed=wseed, pt_eos_bias=pt_eos_bias, pt_seq_length=pt_seq_length, rec_length=rec_length))
 
 
 def case(name, golden_dir):
@@ -97,7 +79,6 @@ def test_decode_fixtures_read_at_their_own_points(name, golden_dir):
 EXTRAS = [dict(), dict(rec_candidates=5), dict(rec_beams=1), dict(rec_beams=4, length_penalty=0.5),
           dict(rec_locations=True)]
 SETTINGS = [dict(joint_decode=1), dict(joint_decode=0), dict(decode_streams=1), dict(use_graphs=0)]
-DEFAULTS = dict(joint_decode=1, decode_streams=2, use_graphs=1)
 
 
 def round_trip(m, encode):
@@ -122,13 +103,8 @@ def test_decode_then_read_at_its_points_is_decode(setting, golden_dir):
     _, _, img1, mask1 = case('masked', golden_dir)
     img, mask = torch.cat([img0, img1, img0]), torch.cat([mask0, mask1, mask0])
     m = spot_model(0, -30.0, 8, 25)
-    try:
-        for k, v in setting.items():
-            m.ctx.set_option(k, v)
+    with options(m.ctx, **setting):
         round_trip(m, lambda: m.encode(img, mask))
-    finally:
-        for k, v in DEFAULTS.items():
-            m.ctx.set_option(k, v)
 
 
 def test_decode_then_read_at_on_pages_of_different_sizes():
@@ -220,12 +196,9 @@ def test_refusals_leave_the_context_usable(golden_dir):
         rc = _decode_at(m, *args, **kw)
         assert rc == ERR_INVALID, (what, rc)
         assert_same(m._read_at_arrays([pts]), want, f'after refusing {what}')
-    m.ctx.set_option('kv_decoders', 1)
-    try:
+    with options(m.ctx, kv_decoders=1):
         m.encode(img, mask)
         assert _decode_at(m, good, [4], 4) == ERR_STATE, 'kv_decoders < 3'
-    finally:
-        m.ctx.set_option('kv_decoders', 3)
     m.encode(img, mask)
     assert_same(m._read_at_arrays([pts]), want, 'after refusing kv_decoders < 3')
     # candidates together with beams: refused by the setters, in Python and in the library
@@ -274,12 +247,9 @@ def test_kie_checkpoint_is_refused():
 
 
 # ----------------------------------------------------------------------------------------------- read_regions
-def tiles_fixture(golden_dir):
-    gold = np.load(os.path.join(golden_dir, 'omni_tiles.npz'))
-    m = spot_model(int(gold['wseed']), float(gold['pt_eos_bias']), int(gold['pt_seq_length']), int(gold['rec_length']))
-    kw = dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-              test_max_size=int(gold['test_max_size']))
-    return gold, m, kw
+def tiles_fixture():
+    gold = golden('omni_tiles.npz')
+    return gold, omni_model(gold), kw(gold)
 
 
 def check_regions(m, pages, regions, pi, kind, kw, max_batch=16):
@@ -328,9 +298,9 @@ def check_regions(m, pages, regions, pi, kind, kw, max_batch=16):
     return res
 
 
-def test_read_regions_on_the_tiled_page(golden_dir):
+def test_read_regions_on_the_tiled_page():
     from advancedliteratemachinery_b200.omniparser import tile_to_page
-    gold, m, kw = tiles_fixture(golden_dir)
+    gold, m, kw = tiles_fixture()
     page = gold['page']
     words = m.spot_tiled([page], **kw)[0]
     mg, plan = m.last_tiles['merged'], m.last_tiles['plan']
@@ -357,7 +327,7 @@ def test_read_regions_on_the_tiled_page(golden_dir):
     check_regions(m, [page], polys, np.zeros(len(polys), int), 'polygon', kw)
 
 
-def test_read_regions_on_an_a4_page_with_candidates_and_beams(golden_dir):
+def test_read_regions_on_an_a4_page_with_candidates_and_beams():
     m = spot_model(0, -30.0, 12, 25)
     rng = np.random.default_rng(9)
     a4 = rng.integers(0, 256, (3508, 2480, 3), dtype=np.uint8)

@@ -10,6 +10,8 @@ import numpy as np
 import pytest
 import torch
 
+from tests.support import omni_model, options, release_models
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
@@ -65,11 +67,7 @@ def _op(m, q, k, kpm, key_len, mw, q_split):
 
 @pytest.fixture(scope='module')
 def spot():
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    m = OmniParserB200(omni_sd(0, -30.0), OmniVocab(), workspace_mb=8192)
-    yield m
-    m.ctx.close()
+    return omni_model(dict(wseed=0, pt_eos_bias=-30.0), workspace_mb=8192)
 
 
 @pytest.mark.parametrize('nsplit', [3, 1])
@@ -87,12 +85,9 @@ def test_op_against_fp64_moments(spot, nsplit, Ncap, q_split):
     kpm[1, 5] = 1
     key_len = [200, 137, 1, 195]
     mw = [20, 20, 20, 13]
-    spot.ctx.set_option('nsplit', nsplit)
-    try:
+    with options(spot.ctx, nsplit=nsplit):
         got = _op(spot, q, k, kpm, key_len, mw, q_split)
         got2 = _op(spot, q, k, kpm, key_len, mw, q_split)
-    finally:
-        spot.ctx.set_option('nsplit', 3)
     assert np.array_equal(got.view(np.uint32), got2.view(np.uint32)), 'not bit-reproducible'
     ref = _ref_moments(q, k, kpm, key_len, mw, nsplit)
     s = torch.einsum('nhd,mhd->hnm', q[3].view(Ncap, 8, 64).double(), k[3].view(M, 8, 64).double()) / 8
@@ -155,11 +150,8 @@ def test_spotting_locations_match_the_reference_maps(spot, name, maps_fixture, g
     n = ref.shape[0]
     report, runs = {}, []
     for graphs in (1, 0):
-        spot.ctx.set_option('use_graphs', graphs)
-        try:
+        with options(spot.ctx, use_graphs=graphs):
             out = spot(NestedTensor(img, mask), _seqs(v, case['canvas']), rec_locations=True)
-        finally:
-            spot.ctx.set_option('use_graphs', 1)
         (pt, poly, rec), _ = out
         assert np.array_equal(rec.numpy()[0], maps_fixture[f'{name}_rec']), name
         loc = spot.last_rec_locations

@@ -8,48 +8,25 @@ alm_pre_omni_tiles_at_turned, alm_omni_select_regions).
 * candidates, beams and character boxes follow the kept reading;
 * the new C entries against the emulation and the range entry, their refusals, and the Python refusals.
 """
-import os
-
 import numpy as np
 import pytest
 import torch
 
+from tests.support import golden, kw, omni_model, release_models
 from tests.test_region_turns_cpu import EOS, NB, PAD, emu_select, fabricate
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
 ERR_INVALID = -1
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
 def spot_model(wseed=0, pt_eos_bias=-30.0, pt_seq_length=8, rec_length=25):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    key = (wseed, pt_eos_bias)
-    if key not in _MODELS:
-        for k in list(_MODELS):
-            _MODELS.pop(k).ctx.close()
-        _MODELS[key] = OmniParserB200(omni_sd(wseed, pt_eos_bias), OmniVocab(), workspace_mb=4096)
-    m = _MODELS[key]
-    m.vocab.pt_seq_length, m.vocab.rec_length = pt_seq_length, rec_length
-    return m
+    return omni_model(dict(wseed=wseed, pt_eos_bias=pt_eos_bias, pt_seq_length=pt_seq_length, rec_length=rec_length))
 
 
-def tiles_fixture(golden_dir):
+def tiles_fixture():
     """the omni_tiles.npz model and page (300 x 220, read in 128-pixel tiles), and spot_tiled's words on it"""
-    gold = np.load(os.path.join(golden_dir, 'omni_tiles.npz'))
-    m = spot_model(int(gold['wseed']), float(gold['pt_eos_bias']), int(gold['pt_seq_length']), int(gold['rec_length']))
-    kw = dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-              test_max_size=int(gold['test_max_size']))
-    return gold, m, kw
+    gold = golden('omni_tiles.npz')
+    return gold, omni_model(gold), kw(gold)
 
 
 def fixture_regions(m, page, kw):
@@ -114,8 +91,8 @@ def a4_boxes(seed=10, R=30):
 
 
 # ------------------------------------------------------------------------------------------------ turn 0
-def test_turn_zero_is_upright_bit_for_bit(golden_dir):
-    gold, m, kw = tiles_fixture(golden_dir)
+def test_turn_zero_is_upright_bit_for_bit():
+    gold, m, kw = tiles_fixture()
     page = gold['page']
     for kind, regions in fixture_regions(m, page, kw).items():
         R = len(regions)
@@ -174,8 +151,8 @@ def check_turned(m, page, regions, kind, k, kw, max_batch):
 
 
 @pytest.mark.parametrize('k', [1, 2, 3])
-def test_a_turn_is_a_turned_page(k, golden_dir):
-    gold, m, kw = tiles_fixture(golden_dir)
+def test_a_turn_is_a_turned_page(k):
+    gold, m, kw = tiles_fixture()
     regions = fixture_regions(m, gold['page'], kw)
     for kind in ('point', 'box'):
         check_turned(m, gold['page'], regions[kind], kind, k, kw, max_batch=3)
@@ -191,8 +168,8 @@ def test_a_turn_on_an_a4_page():
 
 
 # ------------------------------------------------------------------------------------------------ mixed turns
-def test_mixed_turns_agree_with_single_turn_calls(golden_dir):
-    gold, m, kw = tiles_fixture(golden_dir)
+def test_mixed_turns_agree_with_single_turn_calls():
+    gold, m, kw = tiles_fixture()
     page = gold['page']
     other = np.ascontiguousarray(np.rot90(page, 1)[40:, :250])
     boxes = fixture_regions(m, page, kw)['box']
@@ -246,8 +223,8 @@ def check_auto(m, pages, regions, pi, kind, kw, max_batch, **extra):
     return got, kept
 
 
-def test_auto_keeps_the_better_reading(golden_dir):
-    gold, m, kw = tiles_fixture(golden_dir)
+def test_auto_keeps_the_better_reading():
+    gold, m, kw = tiles_fixture()
     page = gold['page']
     regions = fixture_regions(m, page, kw)
     tall = np.array([[20, 20, 40, 120], [150, 30, 170, 200]], np.float64)   # 2 h >= 3 w: turns 1 and 3
@@ -279,9 +256,9 @@ def test_auto_on_an_a4_page():
 
 
 # ------------------------------------------------------------------------------------------------ lists
-def test_candidates_beams_and_chars_follow_the_kept_reading(golden_dir):
+def test_candidates_beams_and_chars_follow_the_kept_reading():
     from advancedliteratemachinery_b200.omniparser import char_boxes, char_dicts
-    gold, m, kw = tiles_fixture(golden_dir)
+    gold, m, kw = tiles_fixture()
     page = gold['page']
     boxes = fixture_regions(m, page, kw)['box']
     R = len(boxes)
@@ -381,9 +358,9 @@ def test_select_regions_equals_the_emulation():
         ctx.close()
 
 
-def test_select_regions_refusals_leave_the_context_usable(golden_dir):
+def test_select_regions_refusals_leave_the_context_usable():
     from advancedliteratemachinery_b200.omniparser import select_regions
-    gold, m, kw = tiles_fixture(golden_dir)
+    gold, m, kw = tiles_fixture()
     frames, fidx, pt, poly, rec, prob = fabricate(9, R=12)
     ok = select_regions(m.ctx, frames, fidx, pt, poly, rec, prob, NB, PAD, EOS)
     lib, h = m.lib, m.ctx.h
@@ -421,11 +398,11 @@ def test_select_regions_refusals_leave_the_context_usable(golden_dir):
 
 
 # ------------------------------------------------------------------------------------------------ Python refusals
-def test_python_refusals_come_before_any_device_work(golden_dir):
+def test_python_refusals_come_before_any_device_work():
     from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
     from advancedliteratemachinery_b200 import synthetic as W
     from oracle.gen_golden import KIE_CASES
-    gold, m, kw = tiles_fixture(golden_dir)
+    gold, m, kw = tiles_fixture()
     page = gold['page']
     pts = np.array([[50, 50], [100, 200]])
     m.read_regions([page], pts, [0, 0], kind='point', orientation=[1, 3], **kw)

@@ -12,55 +12,26 @@ rec_candidates=, rec_beams=, length_penalty=); DESIGN 4.11, 4.14, 4.15).
 * refusals come before any device work, and a later plain call is spot_tiled() with the lists reset;
 * max_batch 1 / 5 / 16 give the same lists.
 """
-import os
-
 import numpy as np
 import pytest
 import torch
 
+from tests.support import golden, kw, omni_model, release_models, same
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
-_MODELS = {}
+
+def setup():
+    gold = golden('omni_tiles.npz')
+    return gold, omni_model(gold)
 
 
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def gold_of(golden_dir, name):
-    return np.load(os.path.join(golden_dir, name))
-
-
-def model(gold):
-    """omni_tiles.npz and omni_page_turns.npz share the checkpoint and the vocabulary"""
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed']), float(gold['pt_eos_bias'])),
-                                         OmniVocab(pt_seq_length=int(gold['pt_seq_length']),
-                                                   rec_length=int(gold['rec_length'])), workspace_mb=4096)
-    return _MODELS['spot']
-
-
-def kw(gold, **extra):
-    return dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-                test_max_size=int(gold['test_max_size']), **extra)
-
-
-def setup(golden_dir):
-    gold = gold_of(golden_dir, 'omni_tiles.npz')
-    return gold, model(gold)
-
-
-def pages(golden_dir):
+def pages():
     """The fixture pages of omni_tiles.npz (2 x 3 tiles) and omni_page_turns.npz (two tiles upright, two turned), a page
     of one tile and one of 2 x 3 tiles of noise."""
     rng = np.random.default_rng(5)
-    return [gold_of(golden_dir, 'omni_tiles.npz')['page'], gold_of(golden_dir, 'omni_page_turns.npz')['page'],
+    return [golden('omni_tiles.npz')['page'], golden('omni_page_turns.npz')['page'],
             rng.integers(0, 256, (97, 120, 3), dtype=np.uint8), rng.integers(0, 256, (230, 301, 3), dtype=np.uint8)]
 
 
@@ -70,11 +41,6 @@ def one_tile_page():
 
 def sliced(pages, plan):
     return [np.ascontiguousarray(pages[p][y:y + h, x:x + w]) for p, y, x, h, w in plan.tolist()]
-
-
-def same(a, b):
-    """Two spot_tiled results are equal, floats bit for bit (== on Python floats, with the keys in order)."""
-    assert [[list(d.items()) for d in r] for r in a] == [[list(d.items()) for d in r] for r in b]
 
 
 def same_arrays(a, b, tag=''):
@@ -116,10 +82,10 @@ def terminal_end(v, row):
 
 # ------------------------------------------------------------------------------------------------ candidates
 @pytest.mark.parametrize('k', [1, 3, 8])
-def test_candidates_are_free_and_are_the_tiles_decode(k, golden_dir):
+def test_candidates_are_free_and_are_the_tiles_decode(k):
     from advancedliteratemachinery_b200 import preprocess as P
     from advancedliteratemachinery_b200.omniparser import slot_candidates
-    gold, m = setup(golden_dir)
+    gold, m = setup()
     page = gold['page']
     base = m.spot_tiled([page], **kw(gold))
     got = m.spot_tiled([page], rec_candidates=k, **kw(gold))
@@ -145,10 +111,10 @@ def test_candidates_are_free_and_are_the_tiles_decode(k, golden_dir):
             same_arrays(w, (t['candidates'][0][j, :n], t['candidates'][1][j, :n]), f'tile {j}')
 
 
-def test_one_tile_page_gets_decodes_candidates_and_beams(golden_dir):
+def test_one_tile_page_gets_decodes_candidates_and_beams():
     from advancedliteratemachinery_b200 import preprocess as P
     from advancedliteratemachinery_b200.omniparser import slot_beams, slot_candidates
-    gold, m = setup(golden_dir)
+    gold, m = setup()
     page = one_tile_page()
     nt = P.omni_pages(m.ctx, [page], int(gold['test_min_size']), int(gold['test_max_size']))
     for extra in (dict(rec_candidates=3), dict(rec_beams=4), dict(rec_beams=3, length_penalty=0.5)):
@@ -165,10 +131,10 @@ def test_one_tile_page_gets_decodes_candidates_and_beams(golden_dir):
 
 
 # ------------------------------------------------------------------------------------------------ beams
-def test_width_one_is_spot_tiled_up_to_the_first_terminal_token(golden_dir):
-    gold, m = setup(golden_dir)
+def test_width_one_is_spot_tiled_up_to_the_first_terminal_token():
+    gold, m = setup()
     v = m.vocab
-    pg = pages(golden_dir)
+    pg = pages()
     for orientation in ('upright', [1, 0, 3, 2], 'mixed'):
         base = m.spot_tiled(pg, orientation=orientation, **kw(gold))
         mg = m.last_tiles['turn_merge' if orientation == 'mixed' else 'merged']
@@ -183,15 +149,15 @@ def test_width_one_is_spot_tiled_up_to_the_first_terminal_token(golden_dir):
             assert (ids[i, 0, e:] == v.recog_pad_index).all() and (probs[i, 0, e:] == 0).all(), (orientation, i)
 
 
-def test_beams_keep_the_greedy_geometry_and_are_the_tiles_decode(golden_dir):
+def test_beams_keep_the_greedy_geometry_and_are_the_tiles_decode():
     """W = 4: points, polygons, 'tile', 'instance' (and 'turns') as spot_tiled(), 'rec' / 'score' hypothesis 0's; every
     word's n-best list is its tile instance's, and those of the fixture page's tiles are decode(rec_beams=4) of
     forward_pages on the host-sliced tiles."""
     from advancedliteratemachinery_b200 import postprocess, preprocess as P
     from advancedliteratemachinery_b200.omniparser import slot_beams
-    gold, m = setup(golden_dir)
+    gold, m = setup()
     v = m.vocab
-    pg = pages(golden_dir)
+    pg = pages()
     for orientation in ('upright', [1, 0, 3, 2], [2, 2, 2, 2], [3, 1, 1, 3]):
         base = m.spot_tiled(pg, orientation=orientation, **kw(gold))
         got = m.spot_tiled(pg, orientation=orientation, rec_beams=4, length_penalty=0.7, **kw(gold))
@@ -218,11 +184,11 @@ def test_beams_keep_the_greedy_geometry_and_are_the_tiles_decode(golden_dir):
             same_arrays(w, tuple(a[j, :n] for a in t['beams']), f'tile {j}')
 
 
-def test_turned_lists_equal_the_turned_page_read_upright(golden_dir):
+def test_turned_lists_equal_the_turned_page_read_upright():
     """Turn k reads the tiles of np.rot90(page, k) bit for bit, so its tiles' lists are those of that page read
     upright."""
-    gold, m = setup(golden_dir)
-    page = pages(golden_dir)[1]
+    gold, m = setup()
+    page = pages()[1]
     for extra in (dict(rec_candidates=5), dict(rec_beams=4)):
         name = 'candidates' if 'rec_candidates' in extra else 'beams'
         for k in range(4):
@@ -234,9 +200,9 @@ def test_turned_lists_equal_the_turned_page_read_upright(golden_dir):
 
 # ------------------------------------------------------------------------------------------------ orientation
 @pytest.mark.parametrize('orientation', ['upright', 'turns', 'auto', 'mixed'])
-def test_rows_follow_each_word_back_to_its_tile_instance(orientation, golden_dir):
-    gold, m = setup(golden_dir)
-    pg = pages(golden_dir)
+def test_rows_follow_each_word_back_to_its_tile_instance(orientation):
+    gold, m = setup()
+    pg = pages()
     o = [1, 0, 3, 2] if orientation == 'turns' else orientation
     base = m.spot_tiled(pg, orientation=o, max_batch=5, **kw(gold))
     got = m.spot_tiled(pg, orientation=o, max_batch=5, rec_candidates=4, **kw(gold))
@@ -261,10 +227,10 @@ def test_rows_follow_each_word_back_to_its_tile_instance(orientation, golden_dir
         assert len(t['probe']) == 8
 
 
-def test_candidates_with_locations_keep_the_chars(golden_dir):
+def test_candidates_with_locations_keep_the_chars():
     from tests.test_gpu_page_char_boxes import same_chars
-    gold, m = setup(golden_dir)
-    pg = pages(golden_dir)
+    gold, m = setup()
+    pg = pages()
     for orientation in ('upright', 'auto', 'mixed'):
         alone = m.spot_tiled(pg, orientation=orientation, rec_locations=True, **kw(gold))
         loc = m.last_tiles['loc']
@@ -280,9 +246,9 @@ def test_candidates_with_locations_keep_the_chars(golden_dir):
 
 
 # ------------------------------------------------------------------------------------------------ refusals and reset
-def test_refusals_come_before_any_device_work_and_a_plain_call_resets(golden_dir, monkeypatch):
-    gold, m = setup(golden_dir)
-    pg = pages(golden_dir)
+def test_refusals_come_before_any_device_work_and_a_plain_call_resets(monkeypatch):
+    gold, m = setup()
+    pg = pages()
     base = m.spot_tiled(pg, **kw(gold))
     for extra in (dict(rec_candidates=3), dict(rec_beams=2)):   # a plain call after one with lists
         m.spot_tiled(pg, **kw(gold, **extra))
@@ -309,12 +275,12 @@ def test_refusals_come_before_any_device_work_and_a_plain_call_resets(golden_dir
 
 
 # ------------------------------------------------------------------------------------------------ chunks
-def test_chunk_sizes_give_the_same_lists(golden_dir):
+def test_chunk_sizes_give_the_same_lists():
     """max_batch 1 / 5 / 16 over two pages of different sizes (chunks through encode and encode_pages): the same words
     and candidates bit for bit.  Beams with W > 1 run the tensor-core decoder path, whose probabilities move in the
     last bits with the batch shape (DESIGN 4.4, as test_gpu_beams checks for decode): the same words and hypothesis
     ids, probabilities and scores within 5e-5 relative."""
-    gold, m = setup(golden_dir)
+    gold, m = setup()
     pg = [gold['page'], one_tile_page()]
     runs, lists = [], []
     for mb in (1, 5, 16):

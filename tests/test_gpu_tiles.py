@@ -3,44 +3,15 @@ Tile inputs must equal omni_pages of the host-sliced tiles bit for bit; every ti
 spot_tiled on the fixture page must equal tests/golden/omni_tiles.npz (the unmodified reference run on every tile and
 merged by oracle/tile_ref.py); and the device merge must equal the host build of the same bodies (tests/emu/tile_emu.cpp)
 bit for bit, on the device's own tile outputs and on 16 pages x 12 tiles x 512 fabricated instances."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
-from tests.test_tiles_cpu import assert_same, emu_merge, fabricate
+from tests.support import assert_same, golden, kw, omni_model, release_models
+from tests.test_tiles_cpu import emu_merge, fabricate
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
-
-_MODELS = {}
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def fixture(golden_dir):
-    return np.load(os.path.join(golden_dir, 'omni_tiles.npz'))
-
-
-def model(gold):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed']), float(gold['pt_eos_bias'])),
-                                         OmniVocab(pt_seq_length=int(gold['pt_seq_length']),
-                                                   rec_length=int(gold['rec_length'])), workspace_mb=4096)
-    return _MODELS['spot']
-
-
-def kw(gold):
-    return dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-                test_max_size=int(gold['test_max_size']))
 
 
 def sliced(pages, plan):
@@ -72,12 +43,12 @@ def test_tile_inputs_equal_omni_pages_of_sliced_tiles():
         ctx.close()
 
 
-def test_spot_tiled_equals_the_fixture(golden_dir):
+def test_spot_tiled_equals_the_fixture():
     """ids exact, coordinates exact (page and tile frame), probabilities close; every tile's decode equals
     forward_pages on the sliced tiles bit for bit; the merge equals the emulation fed the device's own tile outputs."""
     from advancedliteratemachinery_b200 import preprocess as P
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_tiles.npz')
+    m = omni_model(gold)
     page = gold['page']
     res = m.spot_tiled([page], **kw(gold))
     t = m.last_tiles
@@ -110,11 +81,11 @@ def test_spot_tiled_equals_the_fixture(golden_dir):
         assert (d['tile'], d['instance']) == tuple(gold['merged_source'][r])
 
 
-def test_single_tile_page_equals_decode_pred_seq(golden_dir):
+def test_single_tile_page_equals_decode_pred_seq():
     """A page no larger than one tile: exactly decode_pred_seq of forward_pages on that page."""
     from advancedliteratemachinery_b200 import postprocess as Post, preprocess as P
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_tiles.npz')
+    m = omni_model(gold)
     page = second_page()
     res = m.spot_tiled([page], **kw(gold))[0]
     out = m.forward_pages(P.omni_pages(m.ctx, [page], int(gold['test_min_size']), int(gold['test_max_size'])))[0]
@@ -125,14 +96,14 @@ def test_single_tile_page_equals_decode_pred_seq(golden_dir):
     assert [(d['tile'], d['instance']) for d in res] == [(0, i) for i in range(len(want))]
 
 
-def test_chunk_sizes_agree_and_other_outputs_are_unchanged(golden_dir):
+def test_chunk_sizes_agree_and_other_outputs_are_unchanged():
     """max_batch 1 / 5 / 16 over two pages of different sizes (chunks through encode and encode_pages) give one
     result; decode / forward_pages on other inputs are the same before and after a tiled call; the merge is three
     launches."""
     from advancedliteratemachinery_b200 import NestedTensor, OmniParserB200, preprocess as P
     from advancedliteratemachinery_b200.omniparser import merge_tiles
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_tiles.npz')
+    m = omni_model(gold)
     pages = [gold['page'], second_page()]
     probe = P.omni_pages(m.ctx, [second_page(), gold['page'][:120, :150]], 128, 256)
     before = m.forward_pages(probe)
@@ -176,13 +147,13 @@ def test_merge_at_scale_equals_the_emulation():
         ctx.close()
 
 
-def test_error_paths_leave_the_context_usable(golden_dir):
+def test_error_paths_leave_the_context_usable():
     """Bad tile / overlap / margin / band / iou, a page index out of range, tiles that are not the plan's, n_inst out
     of range and a short capacity are refused before any device work; the context merges correctly afterwards."""
     from advancedliteratemachinery_b200 import _lib, preprocess as P
     from advancedliteratemachinery_b200.omniparser import merge_tiles
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = golden('omni_tiles.npz')
+    m = omni_model(gold)
     sizes = [gold['page'].shape[:2]]
     T, ov = int(gold['tile']), int(gold['overlap'])
     plan = gold['plan']

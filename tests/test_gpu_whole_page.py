@@ -4,15 +4,14 @@ OmniParserB200.spot_tiled(whole_page=True)).  On the fixture page spot_tiled equ
 oracle/whole_page_ref.py); the device merge equals the host build of the same bodies (tests/emu/whole_page_emu.cpp) bit
 for bit, on the device's own readings and on 16 pages x 12 tiles of fabricated rows; every orientation mode, chunk size
 and page kind agrees with the rule."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import turn_merge_ref as TM
 from oracle import whole_page_ref as WP
-from tests.test_tiles_cpu import assert_same
+from tests import support
+from tests.support import assert_same, golden, omni_model, release_models, same
 from tests.test_whole_page_cpu import band_poly, emu_merge
 
 pytestmark = pytest.mark.gpu
@@ -20,38 +19,18 @@ torch.set_grad_enabled(False)
 
 ERR_INVALID = -1  # include/alm_ocr.h ALM_ERR_INVALID
 
-_MODELS = {}
 
-
-@pytest.fixture(scope='module', autouse=True)
-def _release_models():
-    yield
-    for k in list(_MODELS):
-        _MODELS.pop(k).ctx.close()
-
-
-def fixture(golden_dir):
+def fixture():
     """The fixture, with its page: omni_tiles.npz's (the same page seed)."""
-    g = dict(np.load(os.path.join(golden_dir, 'omni_whole_page.npz')))
-    t = np.load(os.path.join(golden_dir, 'omni_tiles.npz'))
+    g = dict(golden('omni_whole_page.npz'))
+    t = golden('omni_tiles.npz')
     assert int(g['seed']) == int(t['seed'])
     g['page'] = t['page']
     return g
 
 
-def model(gold):
-    from advancedliteratemachinery_b200 import OmniParserB200, OmniVocab
-    from tests.conftest import omni_sd
-    if 'spot' not in _MODELS:
-        _MODELS['spot'] = OmniParserB200(omni_sd(int(gold['wseed']), float(gold['pt_eos_bias'])),
-                                         OmniVocab(pt_seq_length=int(gold['pt_seq_length']),
-                                                   rec_length=int(gold['rec_length'])), workspace_mb=4096)
-    return _MODELS['spot']
-
-
 def kw(gold, **extra):
-    return dict(tile=int(gold['tile']), overlap=int(gold['overlap']), test_min_size=int(gold['test_min_size']),
-                test_max_size=int(gold['test_max_size']), margin=float(gold['margin']), **extra)
+    return support.kw(gold, margin=float(gold['margin']), **extra)
 
 
 def pages(gold):
@@ -59,11 +38,6 @@ def pages(gold):
     rng = np.random.default_rng(21)
     return [gold['page'], rng.integers(0, 256, (230, 301, 3), dtype=np.uint8),
             rng.integers(0, 256, (97, 120, 3), dtype=np.uint8)]
-
-
-def same(a, b):
-    """Two spot_tiled results are equal, floats bit for bit."""
-    assert [[list(d.items()) for d in r] for r in a] == [[list(d.items()) for d in r] for r in b]
 
 
 def emu_of(m, sizes, turns, gold, tiles, whole):
@@ -76,11 +50,11 @@ def oracle_of(m, sizes, turns, gold, tiles, whole):
                     tiles, *whole)
 
 
-def test_spot_tiled_equals_the_fixture(golden_dir):
+def test_spot_tiled_equals_the_fixture():
     """ids exact, coordinates exact, probabilities close; the merge equals the emulation fed the device's own
     readings in every field."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = fixture()
+    m = omni_model(gold)
     page = gold['page']
     size = page.shape[:2]
     got = m.spot_tiled([page], whole_page=True, **kw(gold))[0]
@@ -129,10 +103,10 @@ def large_input(rng, P=16, n=4096, w=509, L=25, num_bins=1000):
     return sizes, turns, tiles, whole
 
 
-def test_device_merge_equals_the_emulation_at_16_pages_x_12_tiles(golden_dir):
+def test_device_merge_equals_the_emulation_at_16_pages_x_12_tiles():
     from advancedliteratemachinery_b200.omniparser import merge_whole_page
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = fixture()
+    m = omni_model(gold)
     sizes, turns, tiles, whole = large_input(np.random.default_rng(7))
     m.ctx.launch_count(reset=True)
     got = merge_whole_page(m.ctx, sizes, 1200, 256, tiles, *whole, 1000, 4.0, turns=turns)
@@ -143,9 +117,9 @@ def test_device_merge_equals_the_emulation_at_16_pages_x_12_tiles(golden_dir):
     assert 0 < kept_whole < int(whole[0].sum()) and int(got['count'].sum()) - kept_whole < int(tiles['count'].sum())
 
 
-def test_single_tile_pages_are_not_read_again(golden_dir):
-    gold = fixture(golden_dir)
-    m = model(gold)
+def test_single_tile_pages_are_not_read_again():
+    gold = fixture()
+    m = omni_model(gold)
     pg = [pages(gold)[2], gold['page'][:100, :110]]
     m.ctx.launch_count(reset=True)
     want = m.spot_tiled(pg, **kw(gold))
@@ -156,10 +130,10 @@ def test_single_tile_pages_are_not_read_again(golden_dir):
     assert 'whole' not in m.last_tiles
 
 
-def test_auto_reuses_its_probe(golden_dir):
+def test_auto_reuses_its_probe():
     """'auto': the whole-page reading is the probe at the chosen turn; only the merge's three launches are added."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = fixture()
+    m = omni_model(gold)
     pg = pages(gold)
     m.ctx.launch_count(reset=True)
     m.spot_tiled(pg, orientation='auto', **kw(gold))
@@ -178,11 +152,11 @@ def test_auto_reuses_its_probe(golden_dir):
 
 
 @pytest.mark.parametrize('k', [1, 2, 3])
-def test_explicit_turns_read_the_fixture(golden_dir, k):
+def test_explicit_turns_read_the_fixture(k):
     """The page np.rot90(page, -k) read at turn k is the fixture page: the whole-page reading is the reference's, and
     the merge is the oracle's on the device's readings, in the turned page's pixels."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = fixture()
+    m = omni_model(gold)
     page = np.ascontiguousarray(np.rot90(gold['page'], -k))
     m.spot_tiled([page], orientation=[k], whole_page=True, **kw(gold))
     t = m.last_tiles
@@ -195,11 +169,11 @@ def test_explicit_turns_read_the_fixture(golden_dir, k):
     assert_same(t['whole_merge'], oracle_of(m, [page.shape[:2]], [k], gold, t['merged'], t['whole']))
 
 
-def test_mixed_on_the_fixture(golden_dir):
+def test_mixed_on_the_fixture():
     """Each of the four readings is merged with its own whole-page partner (reading 0 is the fixture's), then
     merge_turns runs on the result."""
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = fixture()
+    m = omni_model(gold)
     v = m.vocab
     page = gold['page']
     got = m.spot_tiled([page], orientation='mixed', whole_page=True, **kw(gold))[0]
@@ -216,9 +190,9 @@ def test_mixed_on_the_fixture(golden_dir):
     assert len(got) == int(t['turn_merge']['count'][0])
 
 
-def test_a_saturated_whole_page_does_not_raise(golden_dir):
-    gold = fixture(golden_dir)
-    m = model(gold)
+def test_a_saturated_whole_page_does_not_raise():
+    gold = fixture()
+    m = omni_model(gold)
     keep = m.vocab.pt_seq_length
     m.vocab.pt_seq_length = 2
     try:
@@ -228,9 +202,9 @@ def test_a_saturated_whole_page_does_not_raise(golden_dir):
         m.vocab.pt_seq_length = keep
 
 
-def test_chunk_sizes_agree_and_later_calls_are_unchanged(golden_dir):
-    gold = fixture(golden_dir)
-    m = model(gold)
+def test_chunk_sizes_agree_and_later_calls_are_unchanged():
+    gold = fixture()
+    m = omni_model(gold)
     pg = pages(gold)
     before = [m.spot_tiled(pg, **kw(gold)), m.spot_tiled(pg, orientation=[1, 0, 3], **kw(gold))]
     m.encode_pages(*_encoded(m, pg[1]))
@@ -261,18 +235,18 @@ def _encoded(m, page):
     return nt.tensors, P.omni_plan([page.shape[:2]], 128, 256)[0]
 
 
-def test_group_lines_takes_the_result_as_it_is(golden_dir):
-    gold = fixture(golden_dir)
-    m = model(gold)
+def test_group_lines_takes_the_result_as_it_is():
+    gold = fixture()
+    m = omni_model(gold)
     res = m.spot_tiled(pages(gold), whole_page=True, **kw(gold))
     for r, ls in zip(res, m.group_lines(res)):
         assert sorted(w for line in ls for w in line['words']) == list(range(len(r)))
 
 
-def test_error_paths_leave_the_context_usable(golden_dir):
+def test_error_paths_leave_the_context_usable():
     from advancedliteratemachinery_b200.omniparser import merge_whole_page
-    gold = fixture(golden_dir)
-    m = model(gold)
+    gold = fixture()
+    m = omni_model(gold)
     lib, h = m.ctx.lib, m.ctx.h
     sizes, turns, tiles, whole = large_input(np.random.default_rng(3), P=2, n=200, w=30)
     hs = np.array([s[0] for s in sizes], np.int32)

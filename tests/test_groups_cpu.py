@@ -5,42 +5,27 @@ structural properties of any grouping; and the host-side Python (line_results, a
 import ctypes as C
 import math
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
+
+from tests.support import assert_same, emu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 OUTPUTS = ('n_lines', 'line_offset', 'line_first', 'line_words', 'order', 'line_of', 'rank_of', 'line_polys')
 PARAMS = ('cos_tol', 'height_ratio', 'max_offset', 'max_overlap', 'max_gap')
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/group_emu.cpp (host compile of the grouping kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'group_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'group_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/group_emu.cpp (host compile of the grouping kernels' bodies)."""
     lib.emu_group_lines.restype = C.c_long
     lib.emu_group_lines.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_double] * 5 + [C.c_void_p] * 8
-    _EMU = lib
-    return lib
 
 
 def emu_group(polys, count, offset, **params):
     """alm_omni_group_lines' five launches on the host -> the dict group_lines / group_ref.group_lines return."""
     from oracle import group_ref as R
-    lib = build_emu()
+    lib = emu('group_emu', bind)
     prm = dict(R.DEFAULTS, **params)
     polys = np.ascontiguousarray(polys, np.float64).reshape(-1, 32)
     count, offset = np.ascontiguousarray(count, np.int32), np.ascontiguousarray(offset, np.int32)
@@ -53,17 +38,6 @@ def emu_group(polys, count, offset, **params):
     for k in ('line_first', 'line_words', 'line_polys'):
         out[k] = out[k][:K]
     return out
-
-
-def assert_same(a, b):
-    """Two groupings are equal, the line polygons bit for bit."""
-    assert a.keys() == b.keys()
-    for k in a:
-        x, y = np.asarray(a[k]), np.asarray(b[k])
-        assert x.shape == y.shape and x.dtype == y.dtype, k
-        if x.dtype.kind == 'f':
-            x, y = x.view(np.uint64), y.view(np.uint64)
-        assert np.array_equal(x, y), k
 
 
 def gold():

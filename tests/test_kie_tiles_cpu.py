@@ -5,9 +5,6 @@ a page by oracle/gen_golden_kie_tiles.py).  Also: the shared entity walk still g
 import ctypes as C
 import json
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -15,36 +12,23 @@ import pytest
 from oracle import kie_tile_ref as K
 from oracle import tile_ref as R
 from oracle import page_turn_ref as PT
+from tests.support import emu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 NB, BASE, NCLS = 1000, 1104, 4   # num_bins, class_base (padding_index + 1), SROIE classes
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/kie_tile_emu.cpp (host compile of the kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'kie_tile_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'kie_tile_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/kie_tile_emu.cpp (host compile of the kernels' bodies)."""
     lib.emu_merge_kie_tiles.restype = C.c_long
     lib.emu_merge_kie_tiles.argtypes = ([C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p] * 3 + [C.c_int] +
                                         [C.c_void_p] * 3 + [C.c_int] * 4 + [C.c_double] * 3 + [C.c_void_p] * 11)
-    _EMU = lib
-    return lib
 
 
 def emu_merge(sizes, T, ov, raw, margin=4.0, band=None, iou=0.5, turns=None, num_bins=NB, class_base=BASE,
               n_classes=NCLS):
     """alm_omni_merge_kie_tiles' launches on the host -> the dict merge_kie_tiles returns (None: a walk failed)."""
-    lib = build_emu()
+    lib = emu('kie_tile_emu', bind)
     band = ov / 4 if band is None else band
     hs = np.ascontiguousarray([s[0] for s in sizes], np.int32)
     ws = np.ascontiguousarray([s[1] for s in sizes], np.int32)
@@ -73,17 +57,6 @@ def emu_merge(sizes, T, ov, raw, margin=4.0, band=None, iou=0.5, turns=None, num
     for k in ('rect', 'poly', 'word_source'):
         out[k] = out[k][:nw.value]
     return out
-
-
-def assert_same(a, b):
-    """Two merge results are equal, floats bit for bit."""
-    assert a.keys() == b.keys()
-    for k in a:
-        x, y = np.asarray(a[k]), np.asarray(b[k])
-        assert x.shape == y.shape and x.dtype == y.dtype, k
-        if x.dtype.kind == 'f':
-            x, y = x.view(np.uint64 if x.itemsize == 8 else np.uint32), y.view(np.uint64 if y.itemsize == 8 else np.uint32)
-        assert np.array_equal(x, y), k
 
 
 def oracle_of(sizes, T, ov, raw, turns=None, **kw):

@@ -2,15 +2,14 @@
 point), of the kernels' bodies run on the host against tests/golden/pre_lines.npz (window crops cut from the
 unmodified reference crops by oracle/gen_golden_lines.py) and of the stitch against oracle/line_ref.py, bit for bit."""
 import ctypes as C
+import functools
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
+from tests.support import emu
 from tests.test_char_boxes_cpu import random_maps
 from tests.test_curve_crops_cpu import random_polygons
 
@@ -23,22 +22,18 @@ def line_fixture():
     return z, pages
 
 
-def build_emu():
-    """Build tests/emu/line_emu.cpp (host compile of the line kernels' bodies) and bind it."""
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'line_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'line_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/line_emu.cpp (host compile of the line kernels' bodies)."""
     lib.emu_line_windows.restype = None
     lib.emu_line_windows.argtypes = [C.c_int] + [C.c_void_p] * 4
     lib.emu_line_crops.restype = None
     lib.emu_line_crops.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_void_p]
     lib.emu_line_stitch.restype = None
     lib.emu_line_stitch.argtypes = [C.c_int] * 4 + [C.c_void_p] * 10
-    return lib
+
+
+# the emulation under the name tools/bench_lines.py loads it by
+build_emu = functools.partial(emu, 'line_emu', bind)
 
 
 def i32(v):
@@ -129,7 +124,7 @@ def test_host_entry_point_equals_rule():
     from oracle import line_ref as L
     sizes = random_sizes(np.random.default_rng(1), 3000)
     n, x0, wn = P.line_windows(sizes)
-    lib = build_emu()
+    lib = emu('line_emu', bind)
     en, ex0, ewn = np.zeros_like(n), np.zeros_like(x0), np.zeros_like(wn)
     lib.emu_line_windows(len(sizes), i32(sizes).ctypes.data, en.ctypes.data, ex0.ctypes.data, ewn.ctypes.data)
     assert np.array_equal(n, en) and np.array_equal(x0, ex0) and np.array_equal(wn, ewn)
@@ -164,7 +159,7 @@ def test_kernel_bodies_on_the_host_equal_fixture(kind):
     are the fixture's."""
     z, pages = line_fixture()
     regions, pidx = (z['quads'], z['quad_page_index']) if kind == 'quad' else (z['polys'], z['curve_page_index'])
-    got, plan = emu_line_crops(build_emu(), pages, regions, pidx, kind)
+    got, plan = emu_line_crops(emu('line_emu', bind), pages, regions, pidx, kind)
     assert np.array_equal(plan['sizes'], z[f'{kind}_sizes']) and np.array_equal(plan['n'], z[f'{kind}_n'])
     want = torch.from_numpy(z[f'{kind}_out_u8']).to(torch.float32).div(255).numpy()
     assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
@@ -213,7 +208,7 @@ def test_stitch_on_the_host_equals_oracle(kind):
     plan = line_plans(rng, 40)[kind == 'curve']
     B = int(plan['n'].sum())
     maps, probs = random_maps(rng, B), random_probs(rng, B)
-    lib = build_emu()
+    lib = emu('line_emu', bind)
     code = 1 if kind == 'quad' else 2
     for head in (0, 1, 2):
         ids = line_ids(rng, B, head)
@@ -238,7 +233,7 @@ def test_seams_overlap_and_missing_ends():
     lies exactly on a seam goes to the right window, a window without an end token contributes all 26 tokens, and a
     last window without an end token ends the line with probability 0.  Host bodies and oracle agree on each."""
     from oracle import line_ref as L
-    lib = build_emu()
+    lib = emu('line_emu', bind)
     geom = np.eye(3).reshape(1, 9)
 
     def both(maps, ids, probs, cw):
@@ -304,7 +299,7 @@ def test_single_window_lines_equal_char_boxes():
     sizes, geom = q['sizes'][rows], q['geom'][rows]
     B = len(rows)
     maps, probs = random_maps(rng, B), random_probs(rng, B)
-    lib = build_emu()
+    lib = emu('line_emu', bind)
     for head in (1, 2):
         ids = line_ids(rng, B, head)
         got = emu_line_stitch(lib, maps, ids, probs, head, 1, sizes, geom)

@@ -4,13 +4,11 @@ the upright crops and against the oracle crops + np.rot90 + Pillow's resize, and
 the selection kernel against alm_post_mgp_fuse.  Bar: bit-exact everywhere."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+from tests import support
 from tests.test_curve_crops_cpu import curve_fixture, random_polygons
 from tests.test_quad_crops_cpu import quad_fixture, random_quads
 
@@ -20,25 +18,17 @@ CHAR_TABLE = ['[GO]', '[s]'] + list('0123456789abcdefghijklmnopqrstuvwxyz')
 
 @pytest.fixture(scope='module')
 def emu():
-    return build_emu()
+    return support.emu('orient_emu', bind)
 
 
-def build_emu():
-    """Build tests/emu/orient_emu.cpp (host compile of the kernels' bodies) and bind it."""
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'orient_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'orient_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/orient_emu.cpp (host compile of the kernels' bodies)."""
     for f in ('emu_unturn', 'emu_turn_px', 'emu_turned_crops', 'emu_head_conf', 'emu_select'):
         getattr(lib, f).restype = None
     lib.emu_unturn.argtypes = lib.emu_turn_px.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     lib.emu_turned_crops.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 12 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.emu_head_conf.argtypes = [C.c_int] * 4 + [C.c_void_p] * 3
     lib.emu_select.argtypes = [C.c_int] * 4 + [C.c_void_p] * 2 + [C.c_int] + [C.c_void_p] * 4
-    return lib
 
 
 def i32(v):

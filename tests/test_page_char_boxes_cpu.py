@@ -3,48 +3,31 @@ host (tests/emu/rec_box_emu.cpp) against oracle/rec_box_ref.py, bit for bit, on 
 the identity frame against ``postprocess.rec_char_boxes``; the turn commuting with the boxes; and the refusals of
 ``omniparser.char_boxes``."""
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import rec_box_ref as R
 from oracle.whole_page_ref import map_back
+from tests.support import emu
 
 NB = 1000
 PAD, EOS = 1096, 1099   # OmniVocab's recog_pad_index / rec_eos_index (unknown = PAD - 1)
 KEYS = ('n_chars', 'step', 'centre', 'cov', 'box')
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/rec_box_emu.cpp (host compile of the kernel's bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'rec_box_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'rec_box_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/rec_box_emu.cpp (host compile of the kernel's bodies)."""
     lib.emu_char_boxes.restype = None
     lib.emu_char_boxes.argtypes = ([C.c_long, C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_int64, C.c_int64] +
                                    [C.c_void_p] * 5)
     lib.emu_valid_frame.restype = C.c_int
     lib.emu_valid_frame.argtypes = [C.c_void_p]
-    _EMU = lib
-    return lib
 
 
 def emu_boxes(polys, rec, loc, frame_index, frames, pad=PAD, eos=EOS):
     """alm_omni_char_boxes' launch on the host -> the dict omniparser.char_boxes / rec_box_ref.char_boxes return."""
-    lib = build_emu()
+    lib = emu('rec_box_emu', bind)
     polys = np.ascontiguousarray(polys, np.float64).reshape(-1, 32)
     rec = np.ascontiguousarray(rec, np.int64)
     N, L = rec.shape
@@ -122,7 +105,7 @@ def fabricate(seed, N=200, L=25, F=12, nan=0.02):
 def both(*args):
     """The frames are valid and the emulation equals the oracle bit for bit; returns the result."""
     frames = np.ascontiguousarray(args[4], np.int32).reshape(-1, 7)
-    assert all(build_emu().emu_valid_frame(f.ctypes.data) for f in frames)
+    assert all(emu('rec_box_emu', bind).emu_valid_frame(f.ctypes.data) for f in frames)
     got = emu_boxes(*args)
     assert_same(got, R.char_boxes(*args, PAD, EOS))
     return got
@@ -260,7 +243,7 @@ def test_wrapper_refuses_bad_shapes_and_frames():
 def test_wrapper_frame_check_is_the_kernels():
     """omniparser.char_boxes refuses exactly the frames rec_box_core::valid_frame refuses."""
     from advancedliteratemachinery_b200.omniparser import char_boxes
-    lib = build_emu()
+    lib = emu('rec_box_emu', bind)
     rng = np.random.default_rng(11)
     seen = set()
     for _ in range(1000):   # turns outside 0..3 are check_turns' (test above)

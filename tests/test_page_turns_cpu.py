@@ -4,34 +4,20 @@ oracle/page_turn_ref.py, bit for bit: on np.rot90 itself, on fabricated tile out
 tests/golden/omni_page_turns.npz (the reference run on np.rot90 of a page by oracle/gen_golden_page_turns.py)."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import page_turn_ref as R
 from oracle import tile_ref
-from tests.test_tiles_cpu import assert_same, emu_merge, fabricate
+from tests.support import assert_same, emu
+from tests.test_tiles_cpu import emu_merge, fabricate
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/page_turn_emu.cpp (host compile of the kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'page_turn_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'page_turn_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/page_turn_emu.cpp (host compile of the kernels' bodies)."""
     lib.emu_turned_tiles.restype = C.c_long
     lib.emu_turned_tiles.argtypes = [C.c_void_p] + [C.c_int] * 5 + [C.c_void_p, C.c_long]
     lib.emu_map_back.restype = None
@@ -41,13 +27,11 @@ def build_emu():
                                            [C.c_double] * 3 + [C.c_void_p] * 7)
     lib.emu_orient_select.restype = None
     lib.emu_orient_select.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_int64] * 2 + [C.c_void_p] * 2
-    _EMU = lib
-    return lib
 
 
 def emu_tiles(page, k, T, ov):
     """tile_gather_kernel on every tile of page read at turn k -> the tiles' bytes, concatenated."""
-    lib = build_emu()
+    lib = emu('page_turn_emu', bind)
     page = np.ascontiguousarray(page, np.uint8)
     H, W = page.shape[:2]
     cap = 4 * (H + T) * (W + T) * 3
@@ -59,7 +43,7 @@ def emu_tiles(page, k, T, ov):
 
 def emu_merge_turned(sizes, turns, T, ov, n_inst, pt, poly, rec, prob, num_bins, margin=4.0, band=None, iou=0.5):
     """alm_omni_merge_tiles_turned's launches on the host -> the dict merge_tiles / page_turn_ref.merge return."""
-    lib = build_emu()
+    lib = emu('page_turn_emu', bind)
     band = ov / 4 if band is None else band
     hs = np.ascontiguousarray([s[0] for s in sizes], np.int32)
     ws = np.ascontiguousarray([s[1] for s in sizes], np.int32)
@@ -84,7 +68,7 @@ def emu_merge_turned(sizes, turns, T, ov, n_inst, pt, poly, rec, prob, num_bins,
 
 def emu_select(n_inst, rec, prob, pad, eos):
     """orient_select_kernel on the host -> (turns int32 [P], scores f64 [P, 4])."""
-    lib = build_emu()
+    lib = emu('page_turn_emu', bind)
     n_inst = np.ascontiguousarray(n_inst, np.int32).reshape(-1, 4)
     rec = np.ascontiguousarray(rec, np.int64)
     prob = np.ascontiguousarray(prob, np.float32)
@@ -131,7 +115,7 @@ def test_gather_equals_rot90(k):
 def test_map_back_takes_pixel_centres_to_their_source(k):
     """The centre of every turned pixel maps by rule 3 (device body and oracle) to the centre of the page pixel
     np.rot90 took it from."""
-    lib = build_emu()
+    lib = emu('page_turn_emu', bind)
     for H, W in ((7, 5), (4, 9), (1, 3)):
         idx = np.rot90(np.arange(H * W).reshape(H, W), k)
         x, y = C.c_double(), C.c_double()

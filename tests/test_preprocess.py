@@ -7,8 +7,9 @@ import numpy as np
 import pytest
 import torch
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+from tests.support import emu
 
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 
 
 def _omni():
@@ -57,19 +58,14 @@ def test_kernel_weights_equal_the_pinned_oracle():
             assert np.array_equal(bounds, ob) and np.array_equal(coefs, ok), (in_size, out_size, name)
 
 
-def _emu():
-    """Build tests/emu/preproc_emu.cpp (host compile of the kernels' per-pixel bodies) and bind it."""
+def bind(lib):
+    """Bind tests/emu/preproc_emu.cpp (host compile of the kernels' per-pixel bodies)."""
     import ctypes as C
-    import shutil
-    import subprocess
-    import tempfile
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'preproc_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'preproc_emu.cpp'), '-o', so])
-    return C.CDLL(so)
+    for f in (lib.emu_resize_norm, lib.emu_pad_mask):
+        f.restype = None
+    lib.emu_resize_norm.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_int, C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    lib.emu_pad_mask.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
 
 
 def _emu_batch(lib, images, sizes, canvas, filter_name, normalize):
@@ -96,14 +92,8 @@ def _emu_batch(lib, images, sizes, canvas, filter_name, normalize):
 def test_kernel_bodies_on_the_host_equal_reference_fixtures():
     """The per-pixel functions the CUDA kernels execute (csrc/preproc_core.h), compiled for the host and driven in the
     kernels' launch order with the library's own size plan and weights, reproduce the reference outputs bit for bit."""
-    import ctypes as C
     from advancedliteratemachinery_b200 import preprocess as P
-    lib = _emu()
-    for f in (lib.emu_resize_norm, lib.emu_pad_mask):
-        f.restype = None
-    lib.emu_resize_norm.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
-                                    C.c_void_p, C.c_int, C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
-    lib.emu_pad_mask.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    lib = emu('preproc_emu', bind)
     z, pages = _omni()
     sizes, canvas = P.omni_plan([p.shape[:2] for p in pages], int(z['min_size']), int(z['max_size']))
     out, mask = _emu_batch(lib, pages, sizes, canvas, 'bilinear', True)

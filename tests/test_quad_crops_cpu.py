@@ -5,13 +5,12 @@ oracle/gen_golden_quads.py).  Bar: bit-exact everywhere; the inverse maps equal 
 itself uses) bit for bit."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
+
+from tests.support import emu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 REF_MODULES = '/root/reference/Applications/DocXChain/modules'
@@ -59,18 +58,10 @@ def text_regions(seed, n_pages=16, per_page=64, size=1024):
     return pages, q, np.repeat(np.arange(n_pages, dtype=np.int32), per_page)
 
 
-def build_emu():
-    """Build tests/emu/quad_emu.cpp (host compile of the kernels' per-pixel bodies) and bind it."""
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'quad_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'quad_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/quad_emu.cpp (host compile of the kernels' per-pixel bodies)."""
     lib.emu_quad_crops.restype = None
     lib.emu_quad_crops.argtypes = [C.c_int] + [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-    return lib
 
 
 def emu_quad_crops(lib, pages, quads, page_index, imgH=32, imgW=128):
@@ -190,7 +181,7 @@ def test_kernel_bodies_on_the_host_equal_fixture():
     run over every launch's grid with the library's plan and weights, reproduce every reference crop and the final
     tensor bit for bit."""
     z, pages, crops, out = quad_fixture()
-    warped, sizes, got = emu_quad_crops(build_emu(), pages, z['quads'], z['page_index'])
+    warped, sizes, got = emu_quad_crops(emu('quad_emu', bind), pages, z['quads'], z['page_index'])
     assert np.array_equal(sizes, z['sizes'])
     off = 0
     for r, crop in enumerate(crops):

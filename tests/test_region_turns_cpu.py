@@ -3,10 +3,6 @@ host (tests/emu/region_turn_emu.cpp) against a numpy restatement -- the score, t
 four turns, turn 0 against ``tile_to_page`` -- and of the host helpers: the forward turn of points and boxes, the tall
 rule and the routing in the turned frame."""
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -14,36 +10,23 @@ import pytest
 from advancedliteratemachinery_b200 import preprocess as Pre
 from advancedliteratemachinery_b200.omniparser import (plan_region_turns, region_boxes, region_turn_candidates,
                                                        tile_to_page, turn_boxes, turn_points)
+from tests.support import emu
 from tests.test_read_at_cpu import brute_route
 
 NB = 1000
 PAD, EOS = 1096, 1099   # OmniVocab's recog_pad_index / rec_eos_index (unknown = PAD - 1)
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/region_turn_emu.cpp (host compile of the kernel's bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'region_turn_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'region_turn_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/region_turn_emu.cpp (host compile of the kernel's bodies)."""
     lib.emu_select_regions.restype = None
     lib.emu_select_regions.argtypes = ([C.c_long, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 5 +
                                        [C.c_int, C.c_int, C.c_int64, C.c_int64] + [C.c_void_p] * 4)
-    _EMU = lib
-    return lib
 
 
 def emu_select(frames, fidx, pt, poly, rec, prob):
     """alm_omni_select_regions' launch on the host -> (kept, scores, pts, polys)"""
-    lib = build_emu()
+    lib = emu('region_turn_emu', bind)
     fidx = np.ascontiguousarray(fidx, np.int32)
     R, Cn = fidx.shape
     frames = np.ascontiguousarray(frames, np.int32).reshape(-1, 7)

@@ -5,42 +5,27 @@ and on tests/golden/omni_tiles.npz (the reference run on every tile of a page by
 import ctypes as C
 import json
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+from tests.support import emu
+
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/tile_emu.cpp (host compile of the merge kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'tile_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'tile_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/tile_emu.cpp (host compile of the merge kernels' bodies)."""
     lib.emu_tile_axis.restype = C.c_int
     lib.emu_tile_axis.argtypes = [C.c_int] * 3 + [C.c_void_p, C.c_int]
     lib.emu_merge_tiles.restype = C.c_long
     lib.emu_merge_tiles.argtypes = ([C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5 +
                                     [C.c_int] * 3 + [C.c_double] * 3 + [C.c_void_p] * 7)
-    _EMU = lib
-    return lib
 
 
 def emu_merge(sizes, T, ov, n_inst, pt, poly, rec, prob, num_bins, margin=4.0, band=None, iou=0.5):
     """alm_omni_merge_tiles' three launches on the host -> the dict merge_tiles / tile_ref.merge return."""
-    lib = build_emu()
+    lib = emu('tile_emu', bind)
     band = ov / 4 if band is None else band
     hs = np.ascontiguousarray([s[0] for s in sizes], np.int32)
     ws = np.ascontiguousarray([s[1] for s in sizes], np.int32)
@@ -87,7 +72,7 @@ def test_layout_properties():
     entry point and the emulation equal the oracle."""
     from advancedliteratemachinery_b200 import preprocess as P
     from oracle import tile_ref as R
-    lib = build_emu()
+    lib = emu('tile_emu', bind)
     buf = np.zeros(1 << 16, np.int32)
     for H, W, T, ov in random_layouts(np.random.default_rng(0), 5000).tolist():
         for L in (H, W):

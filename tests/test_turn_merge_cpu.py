@@ -3,9 +3,6 @@
 page (tests/golden/omni_page_turns.npz, merged_*), on fabricated readings and on hand-made cases."""
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -13,38 +10,24 @@ import pytest
 from oracle import page_turn_ref as PT
 from oracle import tile_ref
 from oracle import turn_merge_ref as R
-from tests.test_tiles_cpu import assert_same
+from tests.support import assert_same, emu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 PAD, EOS = 1096, 1099
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/turn_merge_emu.cpp (host compile of the kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'turn_merge_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'turn_merge_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/turn_merge_emu.cpp (host compile of the kernels' bodies)."""
     lib.emu_merge_turns.restype = C.c_long
     lib.emu_merge_turns.argtypes = ([C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int64, C.c_int64, C.c_double] +
                                     [C.c_void_p] * 7)
     lib.emu_map_row.restype = None
     lib.emu_map_row.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
-    _EMU = lib
-    return lib
 
 
 def emu_merge(count, offset, pts, polys, rec, prob, pad=PAD, eos=EOS, iou=0.5):
     """alm_omni_merge_turns' three launches on the host -> the dict merge_turns / turn_merge_ref.merge return."""
-    lib = build_emu()
+    lib = emu('turn_merge_emu', bind)
     count = np.ascontiguousarray(count, np.int32)
     offset = np.ascontiguousarray(offset, np.int32)
     pts = np.ascontiguousarray(pts, np.float64).reshape(-1, 2)
@@ -232,8 +215,9 @@ def test_non_finite_rows_are_kept_and_drop_nothing():
     assert pages == [[[0, 0], [1, 0]], [[0, 0], [3, 0]], [[0, 0], [2, 0]]]
     assert np.isnan(R.box(polys[1])).all() and np.isnan(R.box(polys[5])).all()
     box, score = np.zeros(4), np.zeros(1)
-    build_emu().emu_map_row(polys[1].ctypes.data, rec[1].ctypes.data, prob[1].ctypes.data, rec.shape[1], PAD, EOS,
-                            box.ctypes.data, score.ctypes.data)
+    lib = emu('turn_merge_emu', bind)
+    lib.emu_map_row(polys[1].ctypes.data, rec[1].ctypes.data, prob[1].ctypes.data, rec.shape[1], PAD, EOS,
+                    box.ctypes.data, score.ctypes.data)
     assert np.isnan(box).all() and score[0] == PT.spot_score(rec[1], prob[1], PAD, EOS)
 
 

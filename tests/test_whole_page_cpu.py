@@ -5,49 +5,32 @@ stated properties."""
 import ctypes as C
 import math
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import tile_ref
 from oracle import whole_page_ref as R
-from tests.test_tiles_cpu import assert_same
+from tests.support import assert_same, emu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 NB = 1000
 A4 = (3508, 2480)
 
-_EMU = None
 
-
-def build_emu():
-    """Build tests/emu/whole_page_emu.cpp (host compile of the kernels' bodies) and bind it."""
-    global _EMU
-    if _EMU is not None:
-        return _EMU
-    if shutil.which('g++') is None:
-        pytest.skip('g++ not available')
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = os.path.join(tempfile.mkdtemp(), 'whole_page_emu.so')
-    subprocess.check_call(['g++', '-O1', '-ffp-contract=off', '-shared', '-fPIC', '-std=c++17',
-                           os.path.join(here, 'emu', 'whole_page_emu.cpp'), '-o', so])
-    lib = C.CDLL(so)
+def bind(lib):
+    """Bind tests/emu/whole_page_emu.cpp (host compile of the kernels' bodies)."""
     lib.emu_merge_whole_page.restype = C.c_long
     lib.emu_merge_whole_page.argtypes = ([C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.c_double, C.c_int] +
                                          [C.c_void_p] * 12 + [C.c_int, C.c_int] + [C.c_void_p] * 7)
     lib.emu_inside.restype = C.c_int
     lib.emu_inside.argtypes = [C.c_double, C.c_double, C.c_void_p]
-    _EMU = lib
-    return lib
 
 
 def emu_merge(sizes, turns, T, ov, margin, num_bins, tiles, n_inst, pt, poly, rec, prob):
     """alm_omni_merge_whole_page's three launches on the host -> the dict merge_whole_page / whole_page_ref.merge
     return."""
-    lib = build_emu()
+    lib = emu('whole_page_emu', bind)
     P = len(sizes)
     hs = np.ascontiguousarray([s[0] for s in sizes], np.int32)
     ws = np.ascontiguousarray([s[1] for s in sizes], np.int32)
@@ -85,6 +68,7 @@ def both(*args):
 
 
 # ---- fabrication -------------------------------------------------------------------------------------------------
+
 
 def band_poly(x0, y0, x1, y1, slant=0.0):
     """16 vertices of a word from (x0, y0) to (x1, y1) (top-left, bottom-right of the upright box), the bottom edge
@@ -188,6 +172,7 @@ def test_fabrication_exercises_both_decisions():
 
 # ---- the reference fixture ---------------------------------------------------------------------------------------
 
+
 def gold():
     """The fixture, with its page: omni_tiles.npz's (the same page seed)."""
     g = dict(np.load(os.path.join(GOLD, 'omni_whole_page.npz')))
@@ -216,6 +201,7 @@ def test_fixture_merge_equals_the_emulation_and_the_oracle():
 
 
 # ---- hand-made cases ---------------------------------------------------------------------------------------------
+
 
 def a4_tile_decode(words, T=1200, ov=256, max_inst=4, L=3):
     """Tile decodes of an A4 page from page-frame words [(x0, y0, x1, y1)]: every tile reads the part of each word it
@@ -312,7 +298,7 @@ def test_single_tile_pages_keep_no_whole_row():
 
 
 def test_nan_coordinates_are_never_inside():
-    lib = build_emu()
+    lib = emu('whole_page_emu', bind)
     sq = np.ascontiguousarray(band_poly(0, 0, 10, 10))
     assert lib.emu_inside(5.0, 5.0, sq.ctypes.data) and R.inside(5.0, 5.0, sq)
     for x, y in ((math.nan, 5.0), (5.0, math.nan), (math.nan, math.nan)):
@@ -339,6 +325,7 @@ def test_empty_pages_and_readings():
 
 
 # ---- properties ------------------------------------------------------------------------------------------------
+
 
 @pytest.mark.parametrize('seed', range(4))
 def test_narrow_whole_rows_are_never_kept(seed):
