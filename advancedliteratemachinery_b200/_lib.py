@@ -268,6 +268,14 @@ SIGNATURES = {
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_long]),
+    # ctx, heights, widths, n_pages, turns, tile, overlap, margin, num_bins, class_base, n_classes, count, offset,
+    # ent_class, ent_prob, word_offset, word_count, ent_source, word_rect, word_poly, word_source, n_tok, tokens,
+    # tok_prob, max_tok, n_inst, inst_pos, poly, max_inst, page_count, page_offset, ent_class_out, ent_prob_out,
+    # word_offset_out, word_count_out, ent_source_out, cap_ent, word_rect_out, word_poly_out, word_source_out, cap_words
+    'alm_omni_merge_kie_whole_page': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                                C.c_int, C.c_double, C.c_int, C.c_int, C.c_int] +
+                                      [C.c_void_p] * 13 + [C.c_int] + [C.c_void_p] * 3 + [C.c_int] +
+                                      [C.c_void_p] * 7 + [C.c_long] + [C.c_void_p] * 3 + [C.c_long]),
     # ctx, n_words, rec_length, polys, rec, loc, frame_index, n_frames, frames, recog_pad_index, rec_eos_index, n_chars,
     # step, centre, cov, box
     'alm_omni_char_boxes': (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -1120,6 +1120,62 @@ int alm_omni_select_regions(alm_ctx* h, long n_regions, int n_cand, const int32_
   });
 }
 
+namespace {
+
+// The entity table of n KIE readings (alm_omni_merge_kie_tiles: one per tile; alm_omni_merge_kie_whole_page: one per
+// page): max_ent slots per reading, n_ent used, and the totals of entities and of their words
+struct EntityTable {
+  std::vector<kie_tile_core::Entity> table;
+  std::vector<int> n_ent;
+  int max_ent = 1;
+  long ents = 0, words = 0;
+};
+
+// The walk of every reading's token stream: the checks (the refusals name each reading `what` and its index), and the
+// entity table of the merge
+EntityTable walk_readings(const char* fn, const char* what, int n, const int32_t* n_tok, const int64_t* tokens,
+                          const float* tok_prob, int max_tok, const int32_t* n_inst, const int32_t* inst_pos,
+                          int max_inst, int num_bins, int class_base, int n_classes) {
+  EntityTable t;
+  std::vector<std::vector<kie_tile_core::Entity>> per(static_cast<size_t>(n));
+  t.n_ent.resize(static_cast<size_t>(n));
+  for (int k = 0; k < n; ++k) {
+    const std::string at = std::string(fn) + ": " + what + " " + std::to_string(k);
+    ALM_REQUIRE(n_tok[k] >= 0 && n_tok[k] <= max_tok, ALM_ERR_INVALID, at + ": n_tok outside [0, max_tok]");
+    ALM_REQUIRE(n_inst[k] >= 0 && n_inst[k] <= max_inst, ALM_ERR_INVALID, at + ": n_inst outside [0, max_inst]");
+    const long o = static_cast<long>(k) * max_tok;
+    int pairs = 0;
+    const int st = kie_tile_core::walk(tokens + o, tok_prob + o, n_tok[k], inst_pos + static_cast<long>(k) * max_inst,
+                                       n_inst[k], num_bins, class_base, n_classes, &per[static_cast<size_t>(k)], &pairs);
+    ALM_REQUIRE(st != kie_tile_core::kWalkBadClass, ALM_ERR_INVALID, at + ": a token is neither a bin nor an entity class");
+    ALM_REQUIRE(st == kie_tile_core::kWalkOk && pairs == n_inst[k], ALM_ERR_INVALID,
+                at + ": inst_pos does not match the (x, y) pairs of the token stream");
+    t.n_ent[static_cast<size_t>(k)] = static_cast<int>(per[static_cast<size_t>(k)].size());
+    t.max_ent = std::max(t.max_ent, t.n_ent[static_cast<size_t>(k)]);
+    t.ents += t.n_ent[static_cast<size_t>(k)];
+    for (const kie_tile_core::Entity& e : per[static_cast<size_t>(k)]) t.words += e.words;
+  }
+  t.table.assign(static_cast<size_t>(n) * t.max_ent, kie_tile_core::Entity{0, 0.f, 0, 0});
+  for (int k = 0; k < n; ++k)
+    std::copy(per[static_cast<size_t>(k)].begin(), per[static_cast<size_t>(k)].end(),
+              t.table.begin() + static_cast<long>(k) * t.max_ent);
+  return t;
+}
+
+// The output capacities and buffers of a KIE merge that may keep `ents` entities with `words` words
+void require_kie_out(const char* fn, long ents, long words, long cap_ent, long cap_words, const void* ent_class,
+                     const void* ent_prob, const void* word_offset, const void* word_count, const void* ent_source,
+                     const void* word_rect, const void* word_poly, const void* word_source) {
+  ALM_REQUIRE(cap_ent >= ents && cap_words >= words, ALM_ERR_INVALID,
+              std::string(fn) + ": output capacity below the entities (cap_ent) or their words (cap_words)");
+  ALM_REQUIRE(ents == 0 || (ent_class && ent_prob && word_offset && word_count && ent_source), ALM_ERR_INVALID,
+              std::string(fn) + ": null entity output buffer");
+  ALM_REQUIRE(words == 0 || (word_rect && word_poly && word_source), ALM_ERR_INVALID,
+              std::string(fn) + ": null word output buffer");
+}
+
+}  // namespace
+
 int alm_omni_merge_kie_tiles(alm_ctx* h, const int* heights, const int* widths, int n_pages, const int32_t* turns,
                              int tile, int overlap, int n_tiles, const int* tile_page, const int* tile_origin,
                              const int32_t* n_tok, const int64_t* tokens, const float* tok_prob, int max_tok,
@@ -1136,44 +1192,63 @@ int alm_omni_merge_kie_tiles(alm_ctx* h, const int* heights, const int* widths, 
                 std::string(fn) + ": null argument");
     const std::vector<tile_core::Tile> tiles = merge_plan(fn, heights, widths, n_pages, turns, tile, overlap, margin,
                                                           band, iou, n_tiles, tile_page, tile_origin);
-    // the walk of every tile's token stream: the checks, and the entity table of the merge
-    std::vector<std::vector<kie_tile_core::Entity>> per(static_cast<size_t>(n_tiles));
-    std::vector<int> n_ent(static_cast<size_t>(n_tiles));
-    long ents = 0, words = 0;
-    int max_ent = 1;
-    for (int k = 0; k < n_tiles; ++k) {
-      const std::string at = std::string(fn) + ": tile " + std::to_string(k);
-      ALM_REQUIRE(n_tok[k] >= 0 && n_tok[k] <= max_tok, ALM_ERR_INVALID, at + ": n_tok outside [0, max_tok]");
-      ALM_REQUIRE(n_inst[k] >= 0 && n_inst[k] <= max_inst, ALM_ERR_INVALID, at + ": n_inst outside [0, max_inst]");
-      const long o = static_cast<long>(k) * max_tok;
-      int pairs = 0;
-      const int st = kie_tile_core::walk(tokens + o, tok_prob + o, n_tok[k], inst_pos + static_cast<long>(k) * max_inst,
-                                         n_inst[k], num_bins, class_base, n_classes, &per[static_cast<size_t>(k)],
-                                         &pairs);
-      ALM_REQUIRE(st != kie_tile_core::kWalkBadClass, ALM_ERR_INVALID,
-                  at + ": a token is neither a bin nor an entity class");
-      ALM_REQUIRE(st == kie_tile_core::kWalkOk && pairs == n_inst[k], ALM_ERR_INVALID,
-                  at + ": inst_pos does not match the (x, y) pairs of the token stream");
-      n_ent[static_cast<size_t>(k)] = static_cast<int>(per[static_cast<size_t>(k)].size());
-      max_ent = std::max(max_ent, n_ent[static_cast<size_t>(k)]);
-      ents += n_ent[static_cast<size_t>(k)];
-      for (const kie_tile_core::Entity& e : per[static_cast<size_t>(k)]) words += e.words;
-    }
-    ALM_REQUIRE(static_cast<long>(n_tiles) * max_ent + words <= INT_MAX / 32, ALM_ERR_INVALID,
+    const EntityTable t = walk_readings(fn, "tile", n_tiles, n_tok, tokens, tok_prob, max_tok, n_inst, inst_pos,
+                                        max_inst, num_bins, class_base, n_classes);
+    ALM_REQUIRE(static_cast<long>(n_tiles) * t.max_ent + t.words <= INT_MAX / 32, ALM_ERR_INVALID,
                 std::string(fn) + ": too many entities or words");
-    ALM_REQUIRE(cap_ent >= ents && cap_words >= words, ALM_ERR_INVALID,
-                std::string(fn) + ": output capacity below the entities (cap_ent) or their words (cap_words)");
-    ALM_REQUIRE(ents == 0 || (ent_class && ent_prob && word_offset && word_count && ent_source), ALM_ERR_INVALID,
-                std::string(fn) + ": null entity output buffer");
-    ALM_REQUIRE(words == 0 || (word_rect && word_poly && word_source), ALM_ERR_INVALID,
-                std::string(fn) + ": null word output buffer");
-    std::vector<kie_tile_core::Entity> table(static_cast<size_t>(n_tiles) * max_ent, kie_tile_core::Entity{0, 0.f, 0, 0});
-    for (int k = 0; k < n_tiles; ++k)
-      std::copy(per[static_cast<size_t>(k)].begin(), per[static_cast<size_t>(k)].end(),
-                table.begin() + static_cast<long>(k) * max_ent);
-    kie_merge(&h->c, tiles, n_pages, max_ent, n_ent.data(), table.data(), max_inst, poly, num_bins, margin, iou,
+    require_kie_out(fn, t.ents, t.words, cap_ent, cap_words, ent_class, ent_prob, word_offset, word_count, ent_source,
+                    word_rect, word_poly, word_source);
+    kie_merge(&h->c, tiles, n_pages, t.max_ent, t.n_ent.data(), t.table.data(), max_inst, poly, num_bins, margin, iou,
               page_count, page_offset, ent_class, ent_prob, word_offset, word_count, ent_source, word_rect, word_poly,
               word_source);
+  });
+}
+
+int alm_omni_merge_kie_whole_page(alm_ctx* h, const int* heights, const int* widths, int n_pages, const int32_t* turns,
+                                  int tile, int overlap, double margin, int num_bins, int class_base, int n_classes,
+                                  const int32_t* count, const int32_t* offset, const int32_t* ent_class,
+                                  const float* ent_prob, const int32_t* word_offset, const int32_t* word_count,
+                                  const int32_t* ent_source, const double* word_rect, const double* word_poly,
+                                  const int32_t* word_source, const int32_t* n_tok, const int64_t* tokens,
+                                  const float* tok_prob, int max_tok, const int32_t* n_inst, const int32_t* inst_pos,
+                                  const int64_t* poly, int max_inst, int32_t* page_count, int32_t* page_offset,
+                                  int32_t* ent_class_out, float* ent_prob_out, int32_t* word_offset_out,
+                                  int32_t* word_count_out, int32_t* ent_source_out, long cap_ent,
+                                  double* word_rect_out, double* word_poly_out, int32_t* word_source_out,
+                                  long cap_words) {
+  return guarded(h, [&] {
+    const char* fn = "alm_omni_merge_kie_whole_page";
+    ALM_REQUIRE(pages_ok(heights, widths, n_pages) && tile_core::valid_layout(tile, overlap), ALM_ERR_INVALID,
+                std::string(fn) + ": page sizes, or tile size / overlap (need tile >= 64, 0 <= 2 overlap <= tile)");
+    ALM_REQUIRE(std::isfinite(margin) && margin >= 0.0, ALM_ERR_INVALID,
+                std::string(fn) + ": margin must be finite and >= 0");
+    ALM_REQUIRE(max_tok >= 1 && max_inst >= 1 && num_bins >= 1 && n_classes >= 1, ALM_ERR_INVALID,
+                std::string(fn) + ": max_tok, max_inst, num_bins and n_classes must be >= 1");
+    ALM_REQUIRE(count && offset && n_tok && tokens && tok_prob && n_inst && inst_pos && poly && page_count &&
+                    page_offset,
+                ALM_ERR_INVALID, std::string(fn) + ": null argument");
+    if (turns) require_turns(turns, n_pages, fn);
+    // the tile entities: page rows, then each entity's word rows, both exclusive prefixes of their counts
+    const long E = prefix_total(fn, "page", count, offset, n_pages);
+    ALM_REQUIRE(E == 0 || (ent_class && ent_prob && word_offset && word_count && ent_source), ALM_ERR_INVALID,
+                std::string(fn) + ": null tile entity buffer");
+    ALM_REQUIRE(E <= INT_MAX / 32, ALM_ERR_INVALID, std::string(fn) + ": too many entities");
+    const long W = E ? prefix_total(fn, "entity", word_count, word_offset, E) : 0;
+    ALM_REQUIRE(W == 0 || (word_rect && word_poly && word_source), ALM_ERR_INVALID,
+                std::string(fn) + ": null tile word buffer");
+    const EntityTable t = walk_readings(fn, "page", n_pages, n_tok, tokens, tok_prob, max_tok, n_inst, inst_pos,
+                                        max_inst, num_bins, class_base, n_classes);
+    ALM_REQUIRE(E + static_cast<long>(n_pages) * t.max_ent + W + t.words <= INT_MAX / 32, ALM_ERR_INVALID,
+                std::string(fn) + ": too many entities or words");
+    require_kie_out(fn, E + t.ents, W + t.words, cap_ent, cap_words, ent_class_out, ent_prob_out, word_offset_out,
+                    word_count_out, ent_source_out, word_rect_out, word_poly_out, word_source_out);
+    std::vector<tile_core::Tile> wt(static_cast<size_t>(n_pages));
+    for (int p = 0; p < n_pages; ++p)
+      wt[static_cast<size_t>(p)] = kie_whole_core::whole_tile(p, heights[p], widths[p], turns ? turns[p] : 0);
+    kie_whole_merge(&h->c, wt, tile, overlap, num_bins, margin, count, offset, ent_class, ent_prob, word_offset,
+                    word_count, ent_source, word_rect, word_poly, word_source, t.max_ent, t.n_ent.data(),
+                    t.table.data(), max_inst, poly, page_count, page_offset, ent_class_out, ent_prob_out,
+                    word_offset_out, word_count_out, ent_source_out, word_rect_out, word_poly_out, word_source_out);
   });
 }
 

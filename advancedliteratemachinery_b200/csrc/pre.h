@@ -6,6 +6,7 @@
 #include "alm_internal.h"
 #include "group_core.h"
 #include "kie_tile_core.h"
+#include "kie_whole_core.h"
 #include "rec_box_core.h"
 #include "tile_core.h"
 #include "whole_core.h"
@@ -171,6 +172,22 @@ void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, i
                const kie_tile_core::Entity* ents, int max_inst, const int64_t* poly, int num_bins, double margin,
                double iou, int* page_count, int* page_offset, int* cls_out, float* prob_out, int* word_offset,
                int* word_count, int* ent_src, double* rects, double* polys, int* word_src);
+
+// KIE entities that cross tile seams, recovered from a whole-page KIE reading of each page (tile_merge.cu; rule:
+// kie_whole_core.h, DESIGN 4.22).  Host inputs: wt, each page's whole tile (kie_whole_core::whole_tile); the KIE tile
+// merge's output of the pages (count / offset [n_pages] and word_offset / word_count [E] exclusive prefixes, checked by
+// the caller; cls, prob, ent_src, rects, polys, word_src in the layout alm_omni_merge_kie_tiles writes); the whole
+// readings' entity table (max_ent slots per page, n_ent [n_pages] used; kie_tile_core::walk's rows) and polygons
+// (max_inst slots of [32] bins per page).  Writes page_count / page_offset [n_pages], the kept entities (page order;
+// tile entities, then whole ones) and their words to the host outputs, which hold every input entity and every word.
+// Three launches whatever the counts.
+void kie_whole_merge(Ctx* c, const std::vector<tile_core::Tile>& wt, int T, int ov, int num_bins, double margin,
+                     const int* count, const int* offset, const int* cls, const float* prob, const int* word_offset,
+                     const int* word_count, const int* ent_src, const double* rects, const double* polys,
+                     const int* word_src, int max_ent, const int* n_ent, const kie_tile_core::Entity* ents,
+                     int max_inst, const int64_t* poly, int* page_count, int* page_offset, int* cls_out,
+                     float* prob_out, int* woff_out, int* wcnt_out, int* src_out, double* rects_out, double* polys_out,
+                     int* wsrc_out);
 
 // Character boxes in page pixels (tile_merge.cu; rule: rec_box_core.h, DESIGN 4.20).  Host inputs: N words' page
 // polygons [N][32], rec ids [N][L], locations [N][L][5] and frame index [N] (into frames [F], checked by the caller).

@@ -43,6 +43,20 @@
 //                        of the word counts (no atomics); words mapped back to the upright page as they are written;
 //                        the first block of a page writes its entity count and offset, the last block the word total
 //
+// The recovery of KIE entities that cross tile seams from a whole-page KIE reading (rule: kie_whole_core.h, DESIGN
+// 4.22), three launches whatever the counts.  The whole entity table comes from the host walk that checks the whole
+// readings' token streams.  Blocks are turn_core::blocks over two readings per page: reading 2 p = the page's tile
+// entities, 2 p + 1 = its whole entity slots (rows E + p max_ent .. of one keep array, E = the tile entities):
+//   kie_whole_map_kernel      flat over whole entity slots: box in the turned frame, the separable cut test against
+//                             the page's plan, keep flag, box mapped back to the page
+//   kie_whole_pair_kernel     one 128-thread block per (page, 128 tile entities): each tile entity tests its anchor
+//                             against the page's kept whole boxes, staged 128 at a time in shared memory; blocks of
+//                             whole slots only count theirs; kept entity and word counts per block
+//   kie_whole_compact_kernel  the same blocks: exclusive prefixes of the kept entity and word counts of every earlier
+//                             block, the block's kept entities by a warp ballot and their words after a block scan (no
+//                             atomics); tile entities copied, whole ones written and mapped back to the upright page;
+//                             the first block of a page writes its count and offset, the last block the word total
+//
 // Character boxes in page pixels of words read in tiles (rule: rec_box_core.h, DESIGN 4.20), one launch:
 //   rec_box_kernel       one warp per word: decode_seq's walk over the steps in chunks of 32, a lane per step, the
 //                        kept steps numbered by ballot prefix counts (no atomics: bit-reproducible), each kept step's
@@ -55,6 +69,7 @@
 #include "block_scan.cuh"
 #include "pre.h"
 #include "kie_tile_core.h"
+#include "kie_whole_core.h"
 #include "rec_box_core.h"
 #include "tile_core.h"
 #include "turn_core.h"
@@ -376,6 +391,112 @@ kie_compact_kernel(int max_ent, int max_inst, int nchunk, int num_bins, int n_pa
   }
 }
 
+__global__ void __launch_bounds__(kBlock)
+kie_whole_map_kernel(long S, int max_ent, int max_inst, const tile_core::Tile* __restrict__ wt,
+                     const int* __restrict__ n_ent, const kie_tile_core::Entity* __restrict__ ents,
+                     const int64_t* __restrict__ poly, int T, int ov, int num_bins, double margin,
+                     double* __restrict__ box, uint8_t* __restrict__ keep) {
+  const long g = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (g < S)
+    kie_whole_core::map_entity(g, max_ent, max_inst, wt, n_ent, ents, poly, T, ov, num_bins, margin, box, keep);
+}
+
+// keep: [E] tile entities, then [n_pages max_ent] whole slots (kie_whole_map_kernel's flags); wbox: the whole slots'
+// page boxes.  Kept count and kept word count per block.
+__global__ void __launch_bounds__(kBlock)
+kie_whole_pair_kernel(const turn_core::Blk* __restrict__ blks, const int* __restrict__ count,
+                      const int* __restrict__ offset, long E, int max_ent, const int* __restrict__ word_offset,
+                      const int* __restrict__ word_count, const double* __restrict__ rects,
+                      const kie_tile_core::Entity* __restrict__ ents, const double* __restrict__ wbox,
+                      uint8_t* __restrict__ keep, int* __restrict__ blk_count, int* __restrict__ blk_words) {
+  __shared__ double sbox[kBlock][4];
+  __shared__ int sk[kBlock];
+  __shared__ int red[kWarps];
+  const int blk = blockIdx.x, tid = threadIdx.x;
+  const turn_core::Blk b = blks[blk];
+  const int i = b.row0 + tid;
+  const bool live = i < count[b.reading];
+  const long n = static_cast<long>(offset[b.reading]) + i;
+  bool kp = false;
+  int words = 0;
+  if (b.reading & 1) {  // whole slots: kie_whole_map_kernel's flag; uniform over the block
+    kp = live && keep[n];
+    words = kp ? ents[n - E].words : 0;
+  } else {  // tile entities
+    const int nw = live ? word_count[n] : 0;
+    double ax = 0.0, ay = 0.0;
+    if (nw > 0) kie_whole_core::anchor(rects + 4L * word_offset[n], nw, &ax, &ay);
+    const int cnt = count[b.reading + 1];
+    const uint8_t* wkeep = keep + E + static_cast<long>(b.page) * max_ent;
+    const double* wb = wbox + static_cast<long>(b.page) * max_ent * 4;
+    bool dropped = false;
+    for (int j0 = 0; j0 < cnt; j0 += kBlock) {
+      __syncthreads();
+      const int j = j0 + tid;
+      sk[tid] = j < cnt && wkeep[j];
+      if (sk[tid])
+        for (int q = 0; q < 4; ++q) sbox[tid][q] = wb[4L * j + q];
+      __syncthreads();
+      if (nw > 0 && !dropped) {
+        const int m = min(kBlock, cnt - j0);
+        for (int q = 0; q < m; ++q)
+          if (sk[q] && kie_whole_core::inside(ax, ay, sbox[q])) {
+            dropped = true;
+            break;
+          }
+      }
+    }
+    kp = live && !dropped;
+    if (live) keep[n] = kp;
+    words = kp ? nw : 0;
+  }
+  const int total = block_scan::block_sum<kBlock>(kp ? 1 : 0, red);
+  const int wtotal = block_scan::block_sum<kBlock>(words, red);
+  if (tid == 0) {
+    blk_count[blk] = total;
+    blk_words[blk] = wtotal;
+  }
+}
+
+// o_page: entity count [n_pages], entity offset [n_pages], word total [1]
+__global__ void __launch_bounds__(kBlock)
+kie_whole_compact_kernel(const turn_core::Blk* __restrict__ blks, const int* __restrict__ count,
+                         const int* __restrict__ offset, long E, int max_ent, int max_inst, int num_bins, int n_pages,
+                         const int* __restrict__ blk_count, const int* __restrict__ blk_words,
+                         const uint8_t* __restrict__ keep, const int* __restrict__ cls, const float* __restrict__ prob,
+                         const int* __restrict__ word_offset, const int* __restrict__ word_count,
+                         const int* __restrict__ ent_src, const double* __restrict__ rects,
+                         const double* __restrict__ polys, const int* __restrict__ word_src,
+                         const tile_core::Tile* __restrict__ wt, const kie_tile_core::Entity* __restrict__ ents,
+                         const int64_t* __restrict__ poly, int* __restrict__ cls_out, float* __restrict__ prob_out,
+                         int* __restrict__ woff_out, int* __restrict__ wcnt_out, int* __restrict__ src_out,
+                         double* __restrict__ rects_out, double* __restrict__ polys_out, int* __restrict__ wsrc_out,
+                         int* __restrict__ o_page) {
+  __shared__ int red[kWarps], warp_kept[kWarps];
+  const turn_core::Blk b = blks[blockIdx.x];
+  const int i = b.row0 + threadIdx.x;
+  const long n = static_cast<long>(offset[b.reading]) + i;
+  const bool whole = b.reading & 1, kp = i < count[b.reading] && keep[n];
+  const Place at = place(blk_count, kp, red, warp_kept);
+  const int wbefore = block_scan::range_sum<kBlock>(blk_words, 0, blockIdx.x, red);
+  const int words = kp ? (whole ? ents[n - E].words : word_count[n]) : 0;
+  const int wpos = wbefore + block_scan::block_exclusive<kBlock>(words, red);
+  if (kp) {
+    if (whole)
+      kie_whole_core::put_whole(n - E, at.pos, wpos, max_ent, max_inst, wt, ents, poly, num_bins, cls_out, prob_out,
+                                woff_out, wcnt_out, src_out, rects_out, polys_out, wsrc_out);
+    else
+      kie_whole_core::put_tile(n, at.pos, wpos, cls, prob, word_offset, word_count, ent_src, rects, polys, word_src,
+                               cls_out, prob_out, woff_out, wcnt_out, src_out, rects_out, polys_out, wsrc_out);
+  }
+  if (static_cast<int>(blockIdx.x) == b.blk_first)  // uniform over the block
+    put_page(blk_count, b.blk_first, b.blk_end, at.before, &o_page[b.page], &o_page[n_pages + b.page], red);
+  if (blockIdx.x == gridDim.x - 1) {  // uniform over the block
+    const int last = block_scan::block_sum<kBlock>(words, red);
+    if (threadIdx.x == 0) o_page[2 * n_pages] = wbefore + last;
+  }
+}
+
 // words per block of rec_box_kernel: one warp each
 constexpr int kBoxWords = kBlock / 32;
 
@@ -624,6 +745,89 @@ void kie_merge(Ctx* c, const std::vector<tile_core::Tile>& tiles, int n_pages, i
   st.down(rects, o_rects, kept_words * 4);
   st.down(polys, o_polys, kept_words * 32);
   st.down(word_src, o_wsrc, kept_words * 2);
+  st.sync();
+}
+
+void kie_whole_merge(Ctx* c, const std::vector<tile_core::Tile>& wt, int T, int ov, int num_bins, double margin,
+                     const int* count, const int* offset, const int* cls, const float* prob, const int* word_offset,
+                     const int* word_count, const int* ent_src, const double* rects, const double* polys,
+                     const int* word_src, int max_ent, const int* n_ent, const kie_tile_core::Entity* ents,
+                     int max_inst, const int64_t* poly, int* page_count, int* page_offset, int* cls_out,
+                     float* prob_out, int* woff_out, int* wcnt_out, int* src_out, double* rects_out, double* polys_out,
+                     int* wsrc_out) {
+  const int P = static_cast<int>(wt.size());
+  const long E = static_cast<long>(offset[P - 1]) + count[P - 1];
+  const long W = E ? static_cast<long>(word_offset[E - 1]) + word_count[E - 1] : 0;
+  const long S = static_cast<long>(P) * max_ent, SI = static_cast<long>(P) * max_inst;
+  long words = W;  // the tile entities' words and every whole entity's: an upper bound of the kept ones
+  for (long g = 0; g < S; ++g)
+    if (g % max_ent < n_ent[g / max_ent]) words += ents[g].words;
+  std::vector<int> count2(2 * static_cast<size_t>(P)), offset2(2 * static_cast<size_t>(P));
+  for (int p = 0; p < P; ++p) {
+    count2[2 * p] = count[p];
+    offset2[2 * p] = offset[p];
+    count2[2 * p + 1] = n_ent[p];
+    offset2[2 * p + 1] = static_cast<int>(E + static_cast<long>(p) * max_ent);
+  }
+  const std::vector<turn_core::Blk> blks = turn_core::blocks(P, 2, count2.data());
+  const int nblk = static_cast<int>(blks.size());
+  Staging st(c);
+  const tile_core::Tile* d_wt = st.up(wt.data(), wt.size());
+  const turn_core::Blk* d_blks = st.up(blks.data(), blks.size());
+  const int* d_count = st.up(count2.data(), count2.size());
+  const int* d_offset = st.up(offset2.data(), offset2.size());
+  const int* d_cls = st.up(cls, E);
+  const float* d_prob = st.up(prob, E);
+  const int* d_woff = st.up(word_offset, E);
+  const int* d_wcnt = st.up(word_count, E);
+  const int* d_src = st.up(ent_src, E * 2);
+  const double* d_rects = st.up(rects, W * 4);
+  const double* d_polys = st.up(polys, W * 32);
+  const int* d_wsrc = st.up(word_src, W * 2);
+  const int* d_n = st.up(n_ent, P);
+  const kie_tile_core::Entity* d_ents = st.up(ents, S);
+  const int64_t* d_poly = st.up(poly, SI * 32);
+  double* wbox = st.out<double>(S * 4);
+  uint8_t* keep = st.out<uint8_t>(E + S);
+  int* blk_count = st.out<int>(nblk);
+  int* blk_words = st.out<int>(nblk);
+  int* o_cls = st.out<int>(E + S);
+  float* o_prob = st.out<float>(E + S);
+  int* o_woff = st.out<int>(E + S);
+  int* o_wcnt = st.out<int>(E + S);
+  int* o_src = st.out<int>((E + S) * 2);
+  double* o_rects = st.out<double>(words * 4);
+  double* o_polys = st.out<double>(words * 32);
+  int* o_wsrc = st.out<int>(words * 2);
+  int* o_page = st.out<int>(2 * static_cast<size_t>(P) + 1);  // count, offset [P], word total
+
+  kie_whole_map_kernel<<<static_cast<unsigned>((S + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(
+      S, max_ent, max_inst, d_wt, d_n, d_ents, d_poly, T, ov, num_bins, margin, wbox, keep + E);
+  count_launch(c); check_launch("kie_whole_map");
+  kie_whole_pair_kernel<<<nblk, kBlock, 0, c->stream>>>(d_blks, d_count, d_offset, E, max_ent, d_woff, d_wcnt, d_rects,
+                                                        d_ents, wbox, keep, blk_count, blk_words);
+  count_launch(c); check_launch("kie_whole_pair");
+  kie_whole_compact_kernel<<<nblk, kBlock, 0, c->stream>>>(
+      d_blks, d_count, d_offset, E, max_ent, max_inst, num_bins, P, blk_count, blk_words, keep, d_cls, d_prob, d_woff,
+      d_wcnt, d_src, d_rects, d_polys, d_wsrc, d_wt, d_ents, d_poly, o_cls, o_prob, o_woff, o_wcnt, o_src, o_rects,
+      o_polys, o_wsrc, o_page);
+  count_launch(c); check_launch("kie_whole_compact");
+
+  std::vector<int> hp(2 * static_cast<size_t>(P) + 1);
+  st.down(hp.data(), o_page, hp.size());
+  st.sync();  // also: the pageable uploads above are done
+  std::copy(hp.begin(), hp.begin() + P, page_count);
+  std::copy(hp.begin() + P, hp.begin() + 2 * P, page_offset);
+  const long total = static_cast<long>(page_offset[P - 1]) + page_count[P - 1];
+  const long kept_words = hp[2 * static_cast<size_t>(P)];
+  st.down(cls_out, o_cls, total);
+  st.down(prob_out, o_prob, total);
+  st.down(woff_out, o_woff, total);
+  st.down(wcnt_out, o_wcnt, total);
+  st.down(src_out, o_src, total * 2);
+  st.down(rects_out, o_rects, kept_words * 4);
+  st.down(polys_out, o_polys, kept_words * 32);
+  st.down(wsrc_out, o_wsrc, kept_words * 2);
   st.sync();
 }
 

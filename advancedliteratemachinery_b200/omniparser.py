@@ -484,6 +484,62 @@ def merge_kie_tiles(ctx: _lib.Context, sizes, tile: int, overlap: int, plan, n_t
     return _trim(out, ('rect', 'poly', 'word_source'), int(out['word_count'].sum()))
 
 
+_KIE_ENT = ('cls', 'prob', 'word_offset', 'word_count', 'source')   # merge_kie_tiles' entity and word arrays, in the
+_KIE_WORD = ('rect', 'poly', 'word_source')                         # order of the C arguments
+
+
+def merge_kie_whole_page(ctx: _lib.Context, sizes, tile: int, overlap: int, tiles: dict, n_tok, tokens, tok_prob,
+                         n_inst, inst_pos, poly, num_bins: int, class_base: int, n_classes: int, margin: float = 4.0,
+                         turns=None) -> dict:
+    """KIE entities that cross tile seams recovered from a whole-page KIE reading of every page, on the device
+    (``alm_omni_merge_kie_whole_page``; rule: DESIGN 4.22).  tiles: what ``merge_kie_tiles(ctx, sizes, tile, overlap,
+    ..., margin=margin, turns=turns)`` returned for the pages; n_tok / tokens / tok_prob / n_inst / inst_pos / poly: each
+    page's whole-page KIE reading (``np.rot90(page_p, turns[p])`` decoded as one image) in the layout of
+    ``alm_omni_decode_kie``, one row per page.  A whole-page entity is kept iff it has words and every tile of the
+    page's plan cuts its box (an edge within margin of an interior edge); a tile entity is dropped iff its anchor, the
+    centre of its box, lies inside the box of a kept whole-page entity.
+    Returns merge_kie_tiles' dict: page p's kept tile entities in their order, then its kept whole-page entities in
+    entity order (words mapped to the page), source = (tile, entity) / word_source = (tile, instance) for tile entities
+    and (-1, entity) / (-1, instance) for whole-page ones."""
+    from .preprocess import check_turns
+    margin = float(margin)
+    if not (math.isfinite(margin) and margin >= 0):
+        raise ValueError(f'margin must be finite and >= 0, got {margin}')
+    if turns is not None:
+        turns = check_turns(turns, len(sizes))
+    hs, ws = _size_arrays(sizes)
+    P = len(hs)
+    t = {k: np.ascontiguousarray(tiles[k], dtype=d) for k, d in (
+        ('count', np.int32), ('offset', np.int32), ('cls', np.int32), ('prob', np.float32), ('word_offset', np.int32),
+        ('word_count', np.int32), ('source', np.int32), ('rect', np.float64), ('poly', np.float64),
+        ('word_source', np.int32))}
+    n_tok, n_inst, inst_pos = (np.ascontiguousarray(a, dtype=np.int32) for a in (n_tok, n_inst, inst_pos))
+    tokens, poly = (np.ascontiguousarray(a, dtype=np.int64) for a in (tokens, poly))
+    tok_prob = np.ascontiguousarray(tok_prob, dtype=np.float32)
+    E, N = len(t['cls']), len(t['rect'])
+    if not (t['count'].shape == t['offset'].shape == (P,) and all(t[k].shape[:1] == (E,) for k in _KIE_ENT) and
+            t['source'].shape == (E, 2) and t['rect'].shape == (N, 4) and t['poly'].shape == (N, 32) and
+            t['word_source'].shape == (N, 2) and n_tok.shape == (P,) and tokens.ndim == 2 and
+            tokens.shape[0] == P and tok_prob.shape == tokens.shape and n_inst.shape == (P,) and
+            inst_pos.ndim == 2 and inst_pos.shape[0] == P and poly.shape == inst_pos.shape + (32,)):
+        raise ValueError('merge_kie_whole_page: tile entities or whole-page readings do not match the pages')
+    # every token of a whole reading could close an entity, and every instance belongs to at most one
+    EK, NK = max(E + int(n_tok.clip(min=0).sum()), 1), max(N + int(n_inst.clip(min=0).sum()), 1)
+    out = dict(count=np.zeros(P, np.int32), offset=np.zeros(P, np.int32), cls=np.zeros(EK, np.int32),
+               prob=np.zeros(EK, np.float32), word_offset=np.zeros(EK, np.int32), word_count=np.zeros(EK, np.int32),
+               source=np.zeros((EK, 2), np.int32), rect=np.zeros((NK, 4)), poly=np.zeros((NK, 32)),
+               word_source=np.zeros((NK, 2), np.int32))
+    ctx.check(ctx.lib.alm_omni_merge_kie_whole_page(
+        ctx.h, hs.ctypes.data, ws.ctypes.data, P, None if turns is None else turns.ctypes.data, int(tile),
+        int(overlap), margin, int(num_bins), int(class_base), int(n_classes), t['count'].ctypes.data,
+        t['offset'].ctypes.data, *[t[k].ctypes.data for k in _KIE_ENT + _KIE_WORD], n_tok.ctypes.data,
+        tokens.ctypes.data, tok_prob.ctypes.data, tokens.shape[1], n_inst.ctypes.data, inst_pos.ctypes.data,
+        poly.ctypes.data, inst_pos.shape[1], out['count'].ctypes.data, out['offset'].ctypes.data,
+        *[out[k].ctypes.data for k in _KIE_ENT], EK, *[out[k].ctypes.data for k in _KIE_WORD], NK))
+    _trim(out, _KIE_ENT, int(out['count'].sum()))
+    return _trim(out, _KIE_WORD, int(out['word_count'].sum()))
+
+
 def _tile_of(source_tile, first_tile):
     """A merged row's 'tile' within its page: -1 for a whole-page row (merge_whole_page's source -1)."""
     return -1 if source_tile < 0 else int(source_tile - first_tile)
@@ -1315,7 +1371,8 @@ class OmniParserB200:
             if mode == 'auto':  # the probe at the chosen turn is the whole-page reading
                 whole = tuple(a[4 * np.arange(P) + turns] for a in extra['probe'])
             else:
-                whole = self._read_whole(rpages, rsizes, rturns, tile, max_batch, test_min_size, test_max_size)
+                whole = self._read_whole(rpages, rsizes, rturns, tile, max_batch, test_min_size, test_max_size,
+                                         self._decode_dense_arrays)
             out = merge_whole_page(self.ctx, rsizes, tile, overlap, m, *whole, v.num_bins, margin, turns=rturns)
         # the words of every page, each with its reading and its (tile, instance) in the readings' plan
         if mode == 'mixed':
@@ -1505,7 +1562,7 @@ class OmniParserB200:
     def kie_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                   band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200, test_max_size: int = 1920,
                   orientation='upright', rec_candidates: int = 0, rec_beams: int = 0,
-                  rec_locations: bool = False) -> List[list]:
+                  rec_locations: bool = False, whole_page: bool = False) -> List[list]:
         """KIE of pages larger than the model's input or turned by quarter-turns, read in overlapping tiles (rule:
         DESIGN 4.18).  pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch); the checkpoint must
         be a KIE checkpoint.  Every page is cut into the tiles of ``preprocess.omni_tile_plan(sizes, tile, overlap)``;
@@ -1525,35 +1582,88 @@ class OmniParserB200:
         n_inst, inst_pos, poly, rec, rec_prob) and the merge ('merged': each entity's (tile, entity) source, each word's
         (tile, instance) source, rect and 16-vertex polygon in page pixels, ``decode_pred_seq``'s arithmetic, the input
         of ``group_lines``, ``preprocess.curve_crops`` and ``recognize_polygons``); with an orientation also 'turns',
-        and for 'auto' 'page_scores' and the probe decodes 'probe'.  Recognition candidates, beams and character
-        locations are not offered here."""
+        and for 'auto' 'page_scores' and the probe decodes 'probe'.
+        whole_page (rule: DESIGN 4.22): also read every page larger than one tile whole, at its reading turn, through
+        the validation transform, with the KIE decode ('auto' reuses its probe at the chosen turn, with no extra
+        decode).  ``merge_kie_whole_page`` then keeps the whole-page entities whose box every tile cuts, entities
+        crossing a seam that no tile saw whole, and drops the tile entities whose anchor lies inside one of their
+        boxes.  They follow the page's tile entities; ``last_tiles`` gains 'whole' (the whole-page decode arrays, one
+        row per page) and 'whole_merge' (its merge; 'merged' stays the tile merge).  A page that fits in one tile is not
+        read again and keeps what whole_page=False gives.
+        rec_locations (rule: DESIGN 4.20): every tile decode, 'auto''s probes and the whole-page readings also keep
+        the character locations; each entity word is followed back to its tile instance or whole-page instance, and one
+        ``char_boxes`` call for all pages gives every word ``postprocess.rec_char_boxes``' list (char, centre, cov, box)
+        in pixels of the page as passed in.  Each entity tuple then gains a fifth element, that list per word in
+        ``rects`` order.  ``last_tiles`` gains 'loc', every tile's locations.  Recognition candidates and beams are not
+        offered here."""
         v = self.vocab
         self._check_checkpoint('kie_tiled', kie=True)
-        if rec_candidates or rec_beams or rec_locations:
-            raise ValueError('kie_tiled offers no recognition candidates, beams or character locations')
+        if rec_candidates or rec_beams:
+            raise ValueError('kie_tiled offers no recognition candidates or beams')
+        rec_locations = bool(rec_locations)
         _check_max_batch(max_batch)
         mode, turns = _parse_orientation(orientation, len(pages), ('upright', 'auto'), 'page')
         pages, sizes = self._device_pages(pages)
+        P = len(sizes)
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
+        decode = self._kie_tile_decode(rec_locations)
         extra = {}
         if mode == 'auto':
             turns, extra = self._probe_turns(pages, sizes, tile, overlap, max_batch, test_min_size, test_max_size,
-                                             self._decode_kie_arrays)
-        plan, (n_inst, pos, poly, rec, prob, n_tok, toks, tprob) = self._read_tiles(
-            pages, sizes, turns, extra.get('probe'), tile, overlap, max_batch, test_min_size, test_max_size,
-            self._decode_kie_arrays)
+                                             decode)
+        plan, arrays = self._read_tiles(pages, sizes, turns, extra.get('probe'), tile, overlap, max_batch,
+                                        test_min_size, test_max_size, decode)
+        n_inst, pos, poly, rec, prob, n_tok, toks, tprob = arrays[:8]
         m = merge_kie_tiles(self.ctx, sizes, tile, overlap, plan, n_tok, toks, tprob, n_inst, pos, poly, v.num_bins,
                             v.padding_index + 1, v.vie_categories, margin, band, iou, turns=turns)
+        out, whole = m, None
+        if whole_page and any(max(s) > tile for s in sizes):
+            if mode == 'auto':  # the probe at the chosen turn is the whole-page reading
+                whole = tuple(a[4 * np.arange(P) + turns] for a in extra['probe'])
+            else:
+                whole = self._read_whole(pages, sizes, turns, tile, max_batch, test_min_size, test_max_size, decode)
+            wn_inst, wpos, wpoly, _, _, wn_tok, wtoks, wtprob = whole[:8]
+            out = merge_kie_whole_page(self.ctx, sizes, tile, overlap, m, wn_tok, wtoks, wtprob, wn_inst, wpos, wpoly,
+                                       v.num_bins, v.padding_index + 1, v.vie_categories, margin, turns=turns)
+        # every entity word's rec row and, with locations, its locations and frame: tile words in the plan's tiles,
+        # whole-page words (word_source tile -1) in their page read whole, frame len(plan) + page
+        page_of = np.repeat(np.arange(P), out['count'])
+        word_page = np.repeat(page_of, out['word_count']).astype(np.int64)
+        src = out['word_source'].astype(np.int64).reshape(-1, 2)
+        tw = src[:, 0] >= 0
+        L = rec.shape[-1]
+        wrec = np.zeros((len(src), L), np.int64)
+        wrec[tw] = rec[src[tw, 0], src[tw, 1]]
+        if whole is not None:
+            wrec[~tw] = whole[3][word_page[~tw], src[~tw, 1]]
+        chars = None
+        if rec_locations:
+            from . import preprocess as Pre
+            wloc = np.zeros((len(src), L, 5), np.float32)
+            wloc[tw] = arrays[8][src[tw, 0], src[tw, 1]]
+            if whole is not None:
+                wloc[~tw] = whole[8][word_page[~tw], src[~tw, 1]]
+            read = sizes if turns is None else Pre.turned_sizes(sizes, turns)
+            frames = np.concatenate([plan, [(p, 0, 0) + tuple(read[p]) for p in range(P)]]).astype(np.int64)
+            boxes = char_boxes(self.ctx, sizes, frames, out['poly'], wrec, wloc,
+                               np.where(tw, src[:, 0], len(plan) + word_page), v.recog_pad_index, v.rec_eos_index,
+                               turns=turns)
+            chars = char_dicts(boxes, wrec, v)
         results = []
-        for p in range(len(sizes)):
+        for p in range(P):
             ents = []
-            for r in range(int(m['offset'][p]), int(m['offset'][p]) + int(m['count'][p])):
-                ws = range(int(m['word_offset'][r]), int(m['word_offset'][r]) + int(m['word_count'][r]))
-                text = ' '.join(self._kie_word(rec[t, i]) for t, i in m['word_source'][ws].tolist())
-                ents.append((text, v.classes[int(m['cls'][r])], float(m['prob'][r]), m['rect'][ws].tolist()))
+            for r in range(int(out['offset'][p]), int(out['offset'][p]) + int(out['count'][p])):
+                ws = range(int(out['word_offset'][r]), int(out['word_offset'][r]) + int(out['word_count'][r]))
+                text = ' '.join(self._kie_word(wrec[w]) for w in ws)
+                ent = (text, v.classes[int(out['cls'][r])], float(out['prob'][r]), out['rect'][ws].tolist())
+                ents.append(ent if chars is None else ent + ([chars[w] for w in ws],))
             results.append(ents)
         self.last_tiles = dict(plan=plan, n_tok=n_tok, tokens=toks, probs=tprob, n_inst=n_inst, inst_pos=pos, poly=poly,
                                rec=rec, rec_prob=prob, merged=m)
+        if rec_locations:
+            self.last_tiles.update(loc=arrays[8])
+        if whole is not None:
+            self.last_tiles.update(whole=whole, whole_merge=out)
         if turns is not None:
             self.last_tiles.update(turns=turns, **extra)
         return results
@@ -1598,10 +1708,11 @@ class OmniParserB200:
             outs.append(decode())
         return tuple(np.concatenate(a) for a in zip(*outs))
 
-    def _read_whole(self, pages, sizes, turns, tile, max_batch, test_min_size, test_max_size):
+    def _read_whole(self, pages, sizes, turns, tile, max_batch, test_min_size, test_max_size, decode):
         """Every page larger than one tile read whole at its turn (turns None: upright) as ``_probe_turns`` reads it
-        (one tile no smaller than the page, overlap 0, chunks of max_batch), decoded by decode_dense (grid 'auto') ->
-        decode_dense's arrays, one row per page (no instance on the other pages)."""
+        (one tile no smaller than the page, overlap 0, chunks of max_batch), decoded by decode (spot_tiled:
+        ``_decode_dense_arrays``, grid 'auto'; kie_tiled: its tile decode) -> decode's arrays, one row per page (zeros,
+        so no instance or token, on the other pages)."""
         from . import preprocess as Pre
         P = len(pages)
         big = [p for p in range(P) if max(sizes[p]) > tile]
@@ -1610,7 +1721,7 @@ class OmniParserB200:
         T = max(64, max(max(s) for s in sb))
         plan = Pre.omni_tile_plan(sb if tb is None else Pre.turned_sizes(sb, tb), T, 0)
         sub = self._decode_tiles([pages[p] for p in big], plan, T, 0, tb, max_batch, test_min_size, test_max_size,
-                                 self._decode_dense_arrays)
+                                 decode)
         out = tuple(np.zeros((P,) + a.shape[1:], a.dtype) for a in sub)
         for a, b in zip(out, sub):
             a[big] = b
@@ -1625,6 +1736,14 @@ class OmniParserB200:
             if rec_locations:
                 out += (self.last_rec_locations,)
             return out + (self.last_rec_candidates or self.last_rec_beams or ())
+        return decode
+
+    def _kie_tile_decode(self, rec_locations=False):
+        """The decode of kie_tiled's tiles, probes and whole readings: a function giving ``_decode_kie_arrays``' eight
+        arrays, then with rec_locations the locations f32 [B, max_inst, rec_length, 5] (``decode_kie``'s layout)."""
+        def decode():
+            out = self._decode_kie_arrays(None, 0, 0, 1.0, rec_locations)
+            return out + ((self.last_rec_locations,) if rec_locations else ())
         return decode
 
     def _keep_tile_lists(self, lists, source):

@@ -1071,6 +1071,45 @@ ALM_API int alm_omni_merge_kie_tiles(alm_ctx* ctx, const int* heights, const int
                                      int32_t* page_count, int32_t* page_offset, int32_t* ent_class, float* ent_prob,
                                      int32_t* word_offset, int32_t* word_count, int32_t* ent_source, long cap_ent,
                                      double* word_rect, double* word_poly, int32_t* word_source, long cap_words);
+/* KIE entities that cross tile seams, recovered from a whole-page KIE reading of each page (DESIGN 4.22; the rule in
+ * full is in kie_whole_core.h).  An entity taller or wider than the overlap that crosses a seam is cut in every tile,
+ * so alm_omni_merge_kie_tiles drops it; a reading of the whole page sees it whole.  Page p of upright size heights[p] x
+ * widths[p], read at turns[p] (null = all upright), tiled with (tile, overlap) and merged by alm_omni_merge_kie_tiles.
+ * Inputs, HOST buffers:
+ *   - tile entities: what alm_omni_merge_kie_tiles wrote for the pages: count / offset int32 [n_pages] (offset the
+ *     exclusive prefix sum of count), ent_class int32 [E], ent_prob f32 [E], word_offset / word_count int32 [E]
+ *     (word_offset the exclusive prefix sum of word_count), ent_source int32 [E][2]; word_rect f64 [N][4], word_poly
+ *     f64 [N][32], word_source int32 [N][2], in page pixels;
+ *   - whole readings: each page's whole-page KIE reading (np.rot90(page, turn) decoded as one image, orig_size its
+ *     turned size) in the layout of alm_omni_decode_kie, one row per page: n_tok int32 [n_pages] in [0, max_tok],
+ *     tokens int64 [n_pages][max_tok], tok_prob f32 [..], n_inst int32 [n_pages] in [0, max_inst], inst_pos int32
+ *     [n_pages][max_inst], poly int64 [n_pages][max_inst][32].
+ * Whole entities: alm_omni_merge_kie_tiles' walk (1.) and word rects (2.) with the turned page's size and origin 0, box
+ * the union of the word rects.  A whole entity is kept iff it has words and every tile of the page's plan cuts its box:
+ * an edge within margin (<=) of an interior edge of that tile, in its frame, edges outside the tile included.  Its word
+ * rects then map back to the page corner by corner, min / max re-ordered, its polygons vertex by vertex, as
+ * alm_omni_merge_kie_tiles maps turned words.  A tile entity is dropped iff its anchor (the centre of the union of its
+ * word rects) lies inside the box of a kept whole entity of its page, edges included, in double, in page pixels; a NaN
+ * or non-finite coordinate is never inside, and an entity without words is never dropped.  Whole entities never drop
+ * each other.  Outputs, HOST, in alm_omni_merge_kie_tiles' layout: page p's kept tile entities in input order, then its
+ * kept whole entities in entity order; ent_source_out = ent_source's (tile, entity) for tile entities and (-1, entity)
+ * for whole ones, word_source_out = (tile, instance) and (-1, instance).  A page that fits in one tile keeps its tile
+ * entities and no whole entity.  Three kernel launches whatever the counts; only the kept rows and the per-page counts
+ * are copied back.  ALM_ERR_INVALID, before any device work, for bad pages, tile / overlap, a margin that is negative
+ * or not finite, a turn outside 0..3, max_tok / max_inst / num_bins / n_classes < 1, a null buffer, a negative count,
+ * offsets that are not the exclusive prefix sums of their counts, a whole reading alm_omni_merge_kie_tiles would refuse
+ * as a tile's (n_tok, n_inst, inst_pos, tokens), or cap_ent / cap_words below the tile entities plus the whole
+ * entities / all their words. */
+ALM_API int alm_omni_merge_kie_whole_page(
+    alm_ctx* ctx, const int* heights, const int* widths, int n_pages, const int32_t* turns, int tile, int overlap,
+    double margin, int num_bins, int class_base, int n_classes, const int32_t* count, const int32_t* offset,
+    const int32_t* ent_class, const float* ent_prob, const int32_t* word_offset, const int32_t* word_count,
+    const int32_t* ent_source, const double* word_rect, const double* word_poly, const int32_t* word_source,
+    const int32_t* n_tok, const int64_t* tokens, const float* tok_prob, int max_tok, const int32_t* n_inst,
+    const int32_t* inst_pos, const int64_t* poly, int max_inst, int32_t* page_count, int32_t* page_offset,
+    int32_t* ent_class_out, float* ent_prob_out, int32_t* word_offset_out, int32_t* word_count_out,
+    int32_t* ent_source_out, long cap_ent, double* word_rect_out, double* word_poly_out, int32_t* word_source_out,
+    long cap_words);
 /* Spotted words -> text lines in reading order, each with a 16-point line polygon (DESIGN 4.12; the rule in full is
  * in group_core.h).  Inputs, HOST buffers, in the layout alm_omni_merge_tiles writes: page p's words are rows
  * page_offset[p] .. page_offset[p] + page_count[p] - 1 of polys f64 [N][32], N = the sum of page_count; the rows of
