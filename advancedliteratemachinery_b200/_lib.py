@@ -16,6 +16,7 @@ LIB_PATH = os.environ.get('ALM_OCR_LIB') or os.path.join(_HERE, 'libalm_ocr.so')
 ALM_OK = 0
 MAX_CANDIDATES = 8  # ALM_MAX_CANDIDATES
 MAX_BEAMS = 8  # ALM_MAX_BEAMS
+MAX_CHARSETS = 65536  # ALM_MAX_CHARSETS
 BOX_CROP, BOX_QUAD, BOX_CURVE = 0, 1, 2  # ALM_BOX_*: geometry of alm_mgpstr_forward_boxes
 MAX_LINE_WINDOWS = 8  # ALM_MAX_LINE_WINDOWS
 MODEL_OMNI_SPOT, MODEL_OMNI_KIE, MODEL_MGPSTR = 1, 2, 3
@@ -105,6 +106,7 @@ SIGNATURES = {
     'alm_omni_set_rec_beams': (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     'alm_omni_get_rec_beams': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     'alm_omni_set_rec_locations': (C.c_int, [C.c_void_p, C.c_int]),
+    'alm_omni_set_rec_charset': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]),
     'alm_omni_get_rec_locations': (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     'alm_omni_decode_logits': (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     'alm_omni_vocab': (C.c_int, [C.c_void_p]),

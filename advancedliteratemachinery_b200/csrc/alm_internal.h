@@ -222,6 +222,11 @@ struct Ctx {
   int rec_beams = 0;    // alm_omni_set_rec_beams: 0 = greedy recognition, 1..8 = beam width of the recognition loop
   float beam_alpha = 1.f;  // length penalty of the final beam ranking (score / len^alpha)
   bool rec_locations = false;  // alm_omni_set_rec_locations: also reduce every rec step's last-layer cross-attention
+  // alm_omni_set_rec_charset: rec_cs_sets = 0 (off), else the sets rec_cs_allowed [n_sets][rec_cs_chars] and, when not
+  // empty, the row sets rec_cs_rows [B][cap] of the next alm_omni_decode_at
+  int rec_cs_sets = 0, rec_cs_chars = 0;
+  std::vector<uint8_t> rec_cs_allowed;
+  std::vector<int32_t> rec_cs_rows;
   int attn_impl = 0;   // ViT attention: 0 = fused flash-style mma.sync kernel (attn_tc.cu), 1 = GEMM + softmax + GEMM
   int wattn_impl = 3;  // 3 = persistent TMA-fed mma.sync kernel over head pairs (wattn_ms.cu; odd head counts fall back to 0), 0 = one CTA per (window, head), 1 = fp32 SIMT debug kernel
   // optional per-GEMM event timing (alm_set_option "profile_gemm" 1; read with alm_profile_read)

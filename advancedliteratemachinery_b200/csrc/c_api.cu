@@ -1485,6 +1485,37 @@ int alm_omni_set_rec_locations(alm_ctx* h, int on) {
   });
 }
 
+int alm_omni_set_rec_charset(alm_ctx* h, const uint8_t* allowed, int n_sets, int n_chars, const int32_t* row_set,
+                             size_t n_rows) {
+  return guarded(h, [&] {
+    const std::string fn = "alm_omni_set_rec_charset: ";
+    ALM_REQUIRE(n_sets >= 0 && n_sets <= ALM_MAX_CHARSETS, ALM_ERR_INVALID,
+                fn + "n_sets must be 0.." + std::to_string(ALM_MAX_CHARSETS));
+    Ctx& c = h->c;
+    if (n_sets == 0) {  // off: the default, nothing allocated or launched
+      c.rec_cs_sets = c.rec_cs_chars = 0;
+      c.rec_cs_allowed.clear();
+      c.rec_cs_rows.clear();
+      return;
+    }
+    ALM_REQUIRE(allowed != nullptr && n_chars >= 1, ALM_ERR_INVALID, fn + "allowed must be [n_sets][n_chars], n_chars >= 1");
+    ALM_REQUIRE((row_set == nullptr) == (n_rows == 0), ALM_ERR_INVALID, fn + "row_set and n_rows go together");
+    const size_t n = static_cast<size_t>(n_sets) * n_chars;
+    for (int k = 0; k < n_sets; ++k)
+      ALM_REQUIRE(std::any_of(allowed + static_cast<size_t>(k) * n_chars, allowed + (k + 1) * static_cast<size_t>(n_chars),
+                              [](uint8_t v) { return v != 0; }),
+                  ALM_ERR_INVALID, fn + "set " + std::to_string(k) + " is empty");
+    for (size_t r = 0; r < n_rows; ++r)
+      ALM_REQUIRE(row_set[r] >= 0 && row_set[r] < n_sets, ALM_ERR_INVALID,
+                  fn + "row " + std::to_string(r) + "'s set index is outside [0, n_sets)");
+    c.rec_cs_allowed.resize(n);
+    for (size_t i = 0; i < n; ++i) c.rec_cs_allowed[i] = allowed[i] != 0;
+    c.rec_cs_rows.assign(row_set, row_set + n_rows);
+    c.rec_cs_sets = n_sets;
+    c.rec_cs_chars = n_chars;
+  });
+}
+
 int alm_omni_get_rec_locations(alm_ctx* h, float* out, size_t elems) {
   return guarded(h, [&] {
     ALM_REQUIRE(out, ALM_ERR_INVALID, "null argument");

@@ -974,6 +974,29 @@ void wait_stream(Ctx* c, cudaStream_t s) {
   ALM_CHECK_CUDA(cudaEventSynchronize(c->ev_block));
 }
 
+// The context's character sets (alm_omni_set_rec_charset) against one decode, before any device work: the sets must
+// cover the checkpoint's characters, and row sets are read by alm_omni_decode_at alone, one per row of its B x cap
+// (at_rows; -1 for every other entry).
+void check_rec_charset(const Ctx* c, const alm_decode_cfg& cfg, long at_rows) {
+  if (c->rec_cs_sets == 0) return;
+  const std::string fn = "alm_omni_set_rec_charset: ";
+  ALM_REQUIRE(c->rec_cs_chars == cfg.recog_pad - cfg.num_bins - 1, ALM_ERR_INVALID,
+              fn + "n_chars must be recog_pad - num_bins - 1 = " + std::to_string(cfg.recog_pad - cfg.num_bins - 1) +
+                  ", the checkpoint's characters");
+  for (int k = 0; k < c->rec_cs_sets; ++k) {
+    const uint8_t* a = c->rec_cs_allowed.data() + static_cast<size_t>(k) * c->rec_cs_chars;
+    ALM_REQUIRE(std::any_of(a, a + c->rec_cs_chars, [](uint8_t v) { return v != 0; }), ALM_ERR_INVALID,
+                fn + "set " + std::to_string(k) + " is empty");
+  }
+  if (c->rec_cs_rows.empty()) return;
+  ALM_REQUIRE(at_rows >= 0, ALM_ERR_INVALID, fn + "row sets are read by alm_omni_decode_at only (set them again with "
+                                                  "row_set NULL for the other decodes)");
+  ALM_REQUIRE(static_cast<long>(c->rec_cs_rows.size()) == at_rows, ALM_ERR_INVALID,
+              fn + "n_rows must be B x cap = " + std::to_string(at_rows) + " of this alm_omni_decode_at");
+  for (int32_t k : c->rec_cs_rows)
+    ALM_REQUIRE(k >= 0 && k < c->rec_cs_sets, ALM_ERR_INVALID, fn + "a row's set index is outside [0, n_sets)");
+}
+
 struct HeadArgs {
   bool on = false;
   HeadCfg cfg{};
@@ -1017,7 +1040,8 @@ std::vector<long> step_key(Ctx* c, OmniModel* m, int d, DecodeBufs& u, const int
                            h.cfg.rec_eos, h.cfg.recog_pad, reinterpret_cast<long>(c->trace_buf), h.nsoft, h.cfg.vie, c->xattn_impl, c->gemm_grid_cap, c->small_grid_cap, c->debug_skip, c->xattn_ctas_per_sm, c->sattn_wide, c->xattn_wg, c->fuse_ln_gemv,
                            reinterpret_cast<long>(m->key_len), u.mq_grid, u.mq_parts, h.topk,
                            reinterpret_cast<long>(h.cand_ids), reinterpret_cast<long>(h.cand_probs), h.beams,
-                           reinterpret_cast<long>(h.bscore), reinterpret_cast<long>(u.anc), reinterpret_cast<long>(u.loc)};
+                           reinterpret_cast<long>(h.bscore), reinterpret_cast<long>(u.anc), reinterpret_cast<long>(u.loc),
+                           reinterpret_cast<long>(h.cfg.cs_allowed), reinterpret_cast<long>(h.cfg.cs_set)};
 }
 
 // n replays of one step `body`.  The step (all ~62 launches + the counter increment) is captured once into a CUDA
@@ -1166,13 +1190,15 @@ struct PolyRec {
 
 // Polygon and recognition loops (transformer.py:249-284 ; :153-185 for KIE) of pages img0 .. img0 + pts.size() - 1,
 // Ncap rows per page: row n of page img0 + i is [x, y, sos] of pts[i][n], a dead row 0, 0, sos past pts[i]'s end.  The
-// context's rec_topk / rec_beams / rec_locations add candidates, beam search or locations to the recognition loop.
+// context's rec_topk / rec_beams / rec_locations add candidates, beam search or locations to the recognition loop, and
+// its character sets (rec_cs_sets > 0) restrict the recognition loop's choice: row n of page img0 + i reads with set
+// row_set[(img0 + i) * row_stride + n] (row_set null, and dead rows: set 0).
 // The two loops only depend on the points, not on each other.  With one row per instance they run as one joint pass
 // while both have steps left, then the longer loop finishes alone; otherwise (beams, the fp32 GEMV step, the unfused
 // cross-attention) they run concurrently on two streams.  `done` (if any) is recorded on the caller's stream once every
 // loop is enqueued.
 PolyRec poly_rec(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int img0, const std::vector<Points>& pts, int Ncap,
-                 cudaEvent_t done) {
+                 cudaEvent_t done, const int32_t* row_set = nullptr, int row_stride = 0) {
   OmniModel* m = c->omni;
   Arena& ws = c->ws;
   const int nimg = static_cast<int>(pts.size()), Si = nimg * Ncap;  // poly / rec instances
@@ -1207,6 +1233,25 @@ PolyRec poly_rec(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int img0,
     ALM_CHECK_CUDA(cudaMemcpyAsync(toks[phase], h_prompt[phase].data(), h_prompt[phase].size() * sizeof(int),
                                    cudaMemcpyHostToDevice, s0));
   }
+  // the caller's character sets (alm_omni_set_rec_charset) for the recognition loop's head selection alone: the sets,
+  // and each instance's set when rows differ; nothing is allocated or copied without them
+  HeadCfg rc = hc;
+  std::vector<int> h_cs;
+  if (c->rec_cs_sets > 0) {
+    uint8_t* d_allowed = ws.get<uint8_t>(c->rec_cs_allowed.size());
+    ALM_CHECK_CUDA(cudaMemcpyAsync(d_allowed, c->rec_cs_allowed.data(), c->rec_cs_allowed.size(), cudaMemcpyHostToDevice,
+                                   s0));
+    rc.cs_allowed = d_allowed;
+    if (row_set) {
+      h_cs.assign(Si, 0);
+      for (int b = 0; b < nimg; ++b)
+        for (size_t n = 0; n < pts[b].size(); ++n)
+          h_cs[static_cast<size_t>(b) * Ncap + n] = row_set[static_cast<size_t>(img0 + b) * row_stride + n];
+      int* d_cs = ws.get<int>(Si);
+      ALM_CHECK_CUDA(cudaMemcpyAsync(d_cs, h_cs.data(), h_cs.size() * sizeof(int), cudaMemcpyHostToDevice, s0));
+      rc.cs_set = d_cs;
+    }
+  }
   // rec candidates on the device: [Si sequences][rec_length][K], every entry written by the rec loop
   const size_t cand_n = static_cast<size_t>(Si) * cfg.rec_length * K;
   int* d_cand_ids = K > 0 ? ws.get<int>(cand_n) : nullptr;
@@ -1224,7 +1269,7 @@ PolyRec poly_rec(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int img0,
   float* d_loc = Lc ? ws.get<float>(loc_n) : nullptr;
   auto heads = [&](int phase) {  // head selection of the polygon (1) or recognition (2) loop
     HeadArgs h;
-    h.on = true; h.cfg = hc; h.tokens = toks[phase]; h.tstride = 3 + lens[phase]; h.n_prompt_m1 = 2;
+    h.on = true; h.cfg = phase == 2 ? rc : hc; h.tokens = toks[phase]; h.tstride = 3 + lens[phase]; h.n_prompt_m1 = 2;
     h.probs = prbs[phase]; h.pstride = lens[phase]; h.seqs_per_image = Ncap;
     h.nsoft = m->V - m->vie;  // logits[:, -1, :-vie_categories] (transformer.py:156,176)
     if (phase == 2 && K > 0) { h.topk = K; h.cand_ids = d_cand_ids; h.cand_probs = d_cand_probs; }
@@ -1318,7 +1363,8 @@ PolyRec poly_rec(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int img0,
 // result of entry slot_inst[q][n] of its image.  Writes poly / rec / rec_prob in alm_omni_decode's layout with maxI
 // rows per slot, and keeps the candidate / beam / location lists of the context's settings in the model.
 void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P, int maxI, const std::vector<Points>& uniq,
-                    const std::vector<std::vector<int>>& slot_inst, int64_t* poly, int64_t* rec, float* rec_prob) {
+                    const std::vector<std::vector<int>>& slot_inst, int64_t* poly, int64_t* rec, float* rec_prob,
+                    const int32_t* row_set = nullptr, int row_stride = 0) {
   OmniModel* m = c->omni;
   const int S = static_cast<int>(slot_inst.size()), K = c->rec_topk, Wb = c->rec_beams;
   const size_t L = cfg.rec_length, rows = static_cast<size_t>(S) * maxI;
@@ -1336,7 +1382,7 @@ void poly_rec_loops(Ctx* c, const alm_decode_cfg& cfg, const HeadCfg& hc, int P,
   }
   if (c->rec_locations) lists.rec_loc.assign(rows * L * 5, 0.f);
   if (Ncap > 0) {
-    const PolyRec r = poly_rec(c, cfg, hc, 0, uniq, Ncap, c->ev_t[4]);
+    const PolyRec r = poly_rec(c, cfg, hc, 0, uniq, Ncap, c->ev_t[4], row_set, row_stride);
     c->timing_valid[1] = true;
     const size_t T1 = 3 + cfg.poly_length, T2 = 3 + L;
     for (int q = 0; q < S; ++q)
@@ -1400,6 +1446,7 @@ void omni_decode_impl(Ctx* c, const int64_t* prompts, long page_stride, int P, i
               "the batch was encoded with kv_decoders < 3: only alm_omni_decode_points can run on it");
   ALM_REQUIRE(points_only || cfg.max_instances >= (pt_steps / 2), ALM_ERR_INVALID, "max_instances < pt_seq_length / 2");
   ALM_REQUIRE(points_only || cfg.poly_length == 32, ALM_ERR_UNSUPPORTED, "polygon length is fixed at 32 (transformer.py:254)");
+  if (!points_only) check_rec_charset(c, cfg, -1);
   const int B = m->B;
   Arena& ws = c->ws;
   ws.release(m->ws_mark);
@@ -1633,6 +1680,7 @@ void omni_decode_at(Ctx* c, const int32_t* xy, const int32_t* count, int cap, co
                   "alm_omni_decode_at: page " + std::to_string(b) + " has a bin outside [0, num_bins)");
     }
   }
+  check_rec_charset(c, cfg, static_cast<long>(B) * cap);
   std::vector<std::vector<std::pair<int, int>>> uniq(B);
   std::vector<std::vector<int>> slot_inst(B);
   for (int b = 0; b < B; ++b)
@@ -1653,7 +1701,8 @@ void omni_decode_at(Ctx* c, const int32_t* xy, const int32_t* count, int cap, co
   ALM_CHECK_CUDA(cudaEventRecord(c->ev_t[2], c->stream));
   ALM_CHECK_CUDA(cudaEventRecord(c->ev_t[3], c->stream));
   const HeadCfg hc{cfg.num_bins, cfg.pt_eos, cfg.rec_eos, cfg.recog_pad, m->vie};
-  poly_rec_loops(c, cfg, hc, 1, cap, uniq, slot_inst, poly, rec, rec_prob);
+  poly_rec_loops(c, cfg, hc, 1, cap, uniq, slot_inst, poly, rec, rec_prob,
+                 c->rec_cs_rows.empty() ? nullptr : c->rec_cs_rows.data(), cap);
 }
 
 // Teacher-forced logits for one image: every position of every sequence (Transformer.decode, :74-100).
@@ -1824,6 +1873,7 @@ void omni_decode_dense(Ctx* c, const int64_t* prompt, int n_prompt, const alm_de
   const long most = static_cast<long>(nx ? nx * ny : kMaxWindows) * per_seq;
   ALM_REQUIRE(cap >= 1 && cap >= most, ALM_ERR_INVALID,
               fn + "cap is below what the grid can produce: " + std::to_string(most) + " rows per page");
+  check_rec_charset(c, cfg, -1);  // honoured by every polygon / recognition pass, set 0 on every row
 
   // the preamble of every decode entry: a fresh workspace after the encoded state, and no candidate / n-best / location
   // lists (they describe the last decode or none; dense decoding makes none)

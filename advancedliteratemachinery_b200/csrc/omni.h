@@ -6,6 +6,11 @@ namespace alm {
 
 struct HeadCfg {
   int num_bins, pt_eos, rec_eos, recog_pad, vie;
+  // caller character sets of the rec loop (alm_omni_set_rec_charset), null when none is in force: cs_allowed uint8
+  // [n_sets][recog_pad - num_bins - 1] (1 = chars[i] allowed), cs_set int32 [instance] the set of each instance (null:
+  // set 0 for every instance); the beam rows of an instance share its set
+  const uint8_t* cs_allowed = nullptr;
+  const int* cs_set = nullptr;
 };
 
 struct LNW {

@@ -577,17 +577,26 @@ cross_attn_q1_kernel(const float* __restrict__ q, const bf16* __restrict__ kc_hi
   if (t == 0) counters[pair] = 0;  // ready for the next launch
 }
 
+// The caller's character set of rec instance `inst` (alm_omni_set_rec_charset): one byte per class of chars, null when
+// no set is in force, so the default path reads nothing.
+__device__ __forceinline__ const uint8_t* charset_of(const HeadCfg& cfg, long inst) {
+  if (!cfg.cs_allowed) return nullptr;
+  const long n_chars = cfg.recog_pad - cfg.num_bins - 1;
+  return cfg.cs_allowed + (cfg.cs_set ? cfg.cs_set[inst] : 0) * n_chars;
+}
+
 // One greedy step's reduction, 256 threads: m = max of x[:nsoft], tot = sum exp(x - m) over them, (best, bi) = the
 // largest allowed logit of `mode` (lowest id on ties).  head_select_kernel and head_select_topk_kernel both reduce
 // through here, so the top-k form's candidate 0 carries the greedy step's bits.  LIST: every thread also collects the
-// allowed candidates of its slice.
+// allowed candidates of its slice.  cs (mode 2 only; null: none): the instance's character set, which removes the
+// characters outside it from the allowed classes; the unknown class recog_pad - 1, recog_pad and rec_eos stay.
 struct HeadStep {
   float m, tot, best;
   int bi;
 };
 template <bool LIST>
 __device__ __forceinline__ HeadStep head_reduce(const float* __restrict__ x, int V, int nsoft, int mode, const HeadCfg& cfg,
-                                                float* redf, int* redi, TopkList* l) {
+                                                float* redf, int* redi, TopkList* l, const uint8_t* cs = nullptr) {
   const int t = threadIdx.x;
   float m = -INFINITY;
   for (int j = t; j < nsoft; j += 256) m = fmaxf(m, x[j]);
@@ -606,7 +615,9 @@ __device__ __forceinline__ HeadStep head_reduce(const float* __restrict__ x, int
     bool ok;
     if (mode == 0) ok = j < cfg.num_bins || j == cfg.pt_eos;
     else if (mode == 1) ok = j < cfg.num_bins;
-    else if (mode == 2) ok = (j >= cfg.num_bins && j <= cfg.recog_pad) || j == cfg.rec_eos;
+    else if (mode == 2)
+      ok = ((j >= cfg.num_bins && j <= cfg.recog_pad) || j == cfg.rec_eos) &&
+           (!cs || j >= cfg.recog_pad - 1 || j == cfg.rec_eos || cs[j - cfg.num_bins]);
     else ok = j >= V - cfg.vie;
     if (ok && v > best) { best = v; bi = j; }
     if (LIST && ok) topk_insert(*l, v, j);
@@ -654,7 +665,7 @@ head_select_kernel(const float* __restrict__ logits, int V, int nsoft, int phase
   const int gen_index = pos_t - n_prompt_m1;  // index of the token being generated
   const int tnext = pos_t + 1, pidx = gen_index;
   const HeadStep h = head_reduce<false>(logits + static_cast<long>(s) * V, V, nsoft, head_mode(phase, gen_index, cfg), cfg,
-                                        redf, redi, nullptr);
+                                        redf, redi, nullptr, charset_of(cfg, s));
   if (threadIdx.x == 0) {
     const float prob = expf(h.best - h.m) / h.tot;
     tokens[static_cast<long>(s) * tstride + tnext] = h.bi;
@@ -685,7 +696,8 @@ head_select_topk_kernel(const float* __restrict__ logits, int V, int nsoft, Head
   const int gen_index = pos_t - n_prompt_m1;
   TopkList l;
   topk_init(l);
-  const HeadStep h = head_reduce<true>(logits + static_cast<long>(s) * V, V, nsoft, 2, cfg, redf, redi, &l);
+  const HeadStep h = head_reduce<true>(logits + static_cast<long>(s) * V, V, nsoft, 2, cfg, redf, redi, &l,
+                                       charset_of(cfg, s));
   topk_block_merge(l, cv, ci);
   if (threadIdx.x == 0) {
     const float prob = expf(h.best - h.m) / h.tot;
@@ -728,6 +740,7 @@ beam_select_kernel(const float* __restrict__ logits, int V, int nsoft, HeadCfg c
   const int tid = threadIdx.x;
   const long r0 = static_cast<long>(blockIdx.x) * W;
   const int t = *tptr, gen = t - n_prompt_m1;
+  const uint8_t* cs = charset_of(cfg, blockIdx.x);  // the instance's set, shared by its W rows
   if (tid < W) {
     pscore[tid] = gen == 0 ? (tid == 0 ? 0.f : -INFINITY) : score[r0 + tid];
     plen[tid] = gen == 0 ? 0 : blen[r0 + tid];
@@ -743,7 +756,7 @@ beam_select_kernel(const float* __restrict__ logits, int V, int nsoft, HeadCfg c
     }
     TopkList l;
     topk_init(l);
-    const HeadStep st = head_reduce<true>(logits + (r0 + h) * V, V, nsoft, 2, cfg, redf, redi, &l);
+    const HeadStep st = head_reduce<true>(logits + (r0 + h) * V, V, nsoft, 2, cfg, redf, redi, &l, cs);
     topk_block_merge(l, cv, ci);
     if (tid == 0) {
 #pragma unroll

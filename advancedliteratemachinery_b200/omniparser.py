@@ -189,6 +189,39 @@ def check_rec_args(k, beams, length_penalty, locations):
     return k, beams, lp, locations
 
 
+def check_rec_charset(charset, chars: str, rows: Optional[int] = None):
+    """A rec_charset argument (ValueError otherwise) as the sets ``alm_omni_set_rec_charset`` takes (rule: DESIGN 4.23):
+    None for no set, else (allowed uint8 [n_sets, len(chars)], row_set int32 [rows] or None).  charset: None; a string
+    of characters of `chars`, at least one, for every row (row_set None: set 0); or, where rows is given, a sequence of
+    `rows` such strings or None, one per row (None: the row reads unconstrained, with the full set).  Strings naming
+    the same characters share one set, in order of first appearance; a sequence of None alone is no set."""
+    def one(s, where):
+        if not isinstance(s, str) or not s:
+            raise ValueError(f'rec_charset{where} must be a non-empty string of the vocabulary\'s characters, got {s!r}')
+        bad = sorted(set(s) - set(chars))
+        if bad:
+            raise ValueError(f'rec_charset{where} has characters outside the vocabulary: {"".join(bad)!r}')
+        return frozenset(s)
+    if charset is None:
+        return None
+    if isinstance(charset, str) or rows is None:
+        sets, row_set = [one(charset, '')], None
+    else:
+        items = list(charset)
+        if len(items) != rows:
+            raise ValueError(f'rec_charset must hold one string or None per row: {len(items)} for {rows} rows')
+        if all(s is None for s in items):
+            return None
+        keys = [frozenset(chars) if s is None else one(s, f'[{i}]') for i, s in enumerate(items)]
+        sets = list(dict.fromkeys(keys))
+        index = {k: i for i, k in enumerate(sets)}
+        row_set = np.array([index[k] for k in keys], dtype=np.int32)
+    if len(sets) > _lib.MAX_CHARSETS:
+        raise ValueError(f'rec_charset names {len(sets)} distinct sets; at most {_lib.MAX_CHARSETS}')
+    allowed = np.array([[c in k for c in chars] for k in sets], dtype=np.uint8).reshape(len(sets), len(chars))
+    return allowed, row_set
+
+
 def _check_max_batch(max_batch) -> int:
     """The most tiles or pages a reader encodes at once, >= 1 (ValueError otherwise)."""
     if int(max_batch) < 1:
@@ -811,6 +844,7 @@ class OmniParserB200:
         self._rec_k = 0
         self._rec_beams = (0, 1.0)
         self._rec_loc = False
+        self._rec_cs = False
         self.last_rec_candidates = None
         self.last_rec_beams = None
         self.last_rec_locations = None
@@ -826,8 +860,8 @@ class OmniParserB200:
         return self
 
     def __call__(self, samples, sequence=None, rec_candidates: int = 0, rec_beams: int = 0, length_penalty: float = 1.0,
-                 rec_locations: bool = False):
-        return self.forward(samples, sequence, rec_candidates, rec_beams, length_penalty, rec_locations)
+                 rec_locations: bool = False, rec_charset: Optional[str] = None):
+        return self.forward(samples, sequence, rec_candidates, rec_beams, length_penalty, rec_locations, rec_charset)
 
     # ---------------------------------------------------------------------------------------- stages
     def encode(self, tensors: torch.Tensor, mask: Optional[torch.Tensor] = None):
@@ -951,6 +985,22 @@ class OmniParserB200:
         self.last_rec_beams = None
         self.last_rec_locations = None
 
+    def _set_rec_charset(self, sets=None, row_set=None):
+        """The character sets of the next decode (``alm_omni_set_rec_charset``): sets = ``check_rec_charset``'s
+        (allowed, rows) or None (off); row_set (``decode_at`` only) int32 [B, cap] overrides its rows.  Every decode
+        method sets them, so a call without rec_charset reads unconstrained."""
+        if sets is None:
+            if self._rec_cs:
+                self.ctx.check(self.lib.alm_omni_set_rec_charset(self.ctx.h, None, 0, 0, None, 0))
+                self._rec_cs = False
+            return
+        allowed = np.ascontiguousarray(sets[0], dtype=np.uint8)
+        rows = None if row_set is None else np.ascontiguousarray(row_set, dtype=np.int32)
+        self.ctx.check(self.lib.alm_omni_set_rec_charset(self.ctx.h, allowed.ctypes.data, allowed.shape[0],
+                                                         allowed.shape[1], None if rows is None else rows.ctypes.data,
+                                                         0 if rows is None else rows.size))
+        self._rec_cs = True
+
     def _take_rec_lists(self, rec: np.ndarray):
         """After a decode, the lists switched on by ``_set_rec_candidates``, None for the others:
         last_rec_candidates = (ids int64, probs f32) in the layout of `rec` + [k];
@@ -987,7 +1037,7 @@ class OmniParserB200:
             .contiguous()
 
     def decode(self, pt_prompt: Optional[torch.Tensor] = None, rec_candidates: int = 0, rec_beams: int = 0,
-               length_penalty: float = 1.0, rec_locations: bool = False):
+               length_penalty: float = 1.0, rec_locations: bool = False, rec_charset: Optional[str] = None):
         """Greedy pt / poly / rec decoding of every encoded image (model/transformer.py:234-286).
         Returns per-image reference-shaped outputs (None where no point was produced).
         rec_candidates = k > 0 (up to 8): also keep the k most likely characters of every recognition step as
@@ -1002,12 +1052,17 @@ class OmniParserB200:
         every step (rule: ``alm_omni_set_rec_locations`` in include/alm_ocr.h) as ``last_rec_locations``,
         [B, max_inst, rec_length, 5] = centroid and covariance (cx, cy, sxx, sxy, syy) normalised by the page's
         encoded size like poly / num_bins (``slot_locations`` slices them per image, ``postprocess.rec_char_boxes``
-        turns them into one box per character)."""
+        turns them into one box per character).
+        rec_charset = a string of the vocabulary's characters (rule: DESIGN 4.23, ``alm_omni_set_rec_charset``): every
+        recognition step chooses only among them, the unknown class and the two end tokens, so every returned text is
+        in the set; probabilities stay those of the unconstrained softmax, so a forced word scores lower.  Candidates,
+        beams and locations follow the constrained path.  The setting describes this call only."""
         n_inst, pt, poly, rec, prob = self._decode_arrays(pt_prompt, rec_candidates, rec_beams, length_penalty,
-                                                          rec_locations)
+                                                          rec_locations, rec_charset)
         return [_spotting_result(n_inst[b], pt[b], poly[b], rec[b], prob[b]) for b in range(len(n_inst))]
 
-    def _decode_arrays(self, pt_prompt=None, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False):
+    def _decode_arrays(self, pt_prompt=None, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False,
+                       rec_charset=None):
         """alm_omni_decode's outputs for every encoded image: n_inst int32 [B], pt int64 [B, max_inst, 2], poly
         [B, max_inst, 32], rec [B, max_inst, rec_length], prob f32 [B, max_inst, rec_length]."""
         v = self.vocab
@@ -1020,7 +1075,9 @@ class OmniParserB200:
         rec = np.zeros((B, maxi, v.rec_length), dtype=np.int64)
         prob = np.zeros((B, maxi, v.rec_length), dtype=np.float32)
         cfg = self._cfg(maxi)
+        sets = check_rec_charset(rec_charset, v.chars)
         self._set_rec_candidates(rec_candidates, rec_beams, length_penalty, rec_locations)
+        self._set_rec_charset(sets)
         self.ctx.check(self.lib.alm_omni_decode(self.ctx.h, prompt.data_ptr(), prompt.numel(), C.byref(cfg),
                                                 n_inst.ctypes.data, pt.ctypes.data, poly.ctypes.data, rec.ctypes.data,
                                                 prob.ctypes.data))
@@ -1028,7 +1085,7 @@ class OmniParserB200:
         return n_inst, pt, poly, rec, prob
 
     def read_at(self, points, rec_candidates: int = 0, rec_beams: int = 0, length_penalty: float = 1.0,
-                rec_locations: bool = False):
+                rec_locations: bool = False, rec_charset=None):
         """Read the words at caller points of every encoded page: the polygon and recognition loops prompted with
         [x, y, sos] for each point (model/transformer.py:249-284) without the point loop (``alm_omni_decode_at``).
         points: per encoded page an int array [n, 2] of (x, y) bins in [0, num_bins), the frame of ``decode``'s pt
@@ -1038,11 +1095,15 @@ class OmniParserB200:
         Returns per page what ``decode`` returns, ``([pt, poly, rec], [probs])`` with pt the given points, or None for
         a page without points.  decode's own points give decode's output bit for bit.  rec_candidates, rec_beams /
         length_penalty and rec_locations: as in ``decode``, the lists [B, rows, ...] with row n the page's point n.
+        rec_charset: as in ``decode`` (a string for every point), or per page a sequence of one string or None per
+        point (None: that point reads unconstrained); each point reads with its own set.
         KIE checkpoints are refused: their classes come from the point loop."""
-        n, pt, poly, rec, prob = self._read_at_arrays(points, rec_candidates, rec_beams, length_penalty, rec_locations)
+        n, pt, poly, rec, prob = self._read_at_arrays(points, rec_candidates, rec_beams, length_penalty, rec_locations,
+                                                      rec_charset)
         return [_spotting_result(n[b], pt[b], poly[b], rec[b], prob[b]) for b in range(len(n))]
 
-    def _read_at_arrays(self, points, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False):
+    def _read_at_arrays(self, points, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False,
+                        rec_charset=None):
         """alm_omni_decode_at's outputs at the points of every encoded page: count int32 [B], pt int64 [B, N, 2] (the
         given points), poly [B, N, 32], rec [B, N, rec_length], prob f32 [B, N, rec_length], N = max_instances times
         the number of calls."""
@@ -1064,15 +1125,29 @@ class OmniParserB200:
         maxi = max(1, v.pt_seq_length // 2)
         calls = max(1, -(-int(counts.max(initial=0)) // maxi))
         cfg = self._cfg(maxi)
+        if rec_charset is None or isinstance(rec_charset, str):
+            sets, per_point = check_rec_charset(rec_charset, v.chars), None
+        else:   # one string or None per point of every page: the pages' rows in page order
+            if len(rec_charset) != B:
+                raise ValueError(f'rec_charset: {len(rec_charset)} per-point lists for {B} encoded pages')
+            for b, cs in enumerate(rec_charset):
+                if isinstance(cs, str) or len(cs) != counts[b]:
+                    raise ValueError(f'rec_charset[{b}] must hold one string or None per point of page {b}')
+            sets = check_rec_charset([s_ for cs in rec_charset for s_ in cs], v.chars, int(counts.sum()))
+            per_point = None if sets is None else np.split(sets[1], np.cumsum(counts)[:-1])
         self._set_rec_candidates(rec_candidates, rec_beams, length_penalty, rec_locations)
         outs, lists = [], []
         for k in range(calls):
             xy = np.zeros((B, maxi, 2), dtype=np.int32)
             cnt = np.zeros(B, dtype=np.int32)
+            row_set = None if per_point is None else np.zeros((B, maxi), dtype=np.int32)
             for b, a in enumerate(pts):
                 part = a[k * maxi:(k + 1) * maxi]
                 cnt[b] = len(part)
                 xy[b, :len(part)] = part
+                if row_set is not None:
+                    row_set[b, :len(part)] = per_point[b][k * maxi:(k + 1) * maxi]
+            self._set_rec_charset(sets, row_set)
             poly = np.zeros((B, maxi, 32), dtype=np.int64)
             rec = np.zeros((B, maxi, v.rec_length), dtype=np.int64)
             prob = np.zeros((B, maxi, v.rec_length), dtype=np.float32)
@@ -1090,7 +1165,7 @@ class OmniParserB200:
         return (counts,) + tuple(np.concatenate(a, axis=1) for a in zip(*outs))
 
     def decode_prompts(self, prompts: torch.Tensor, rec_candidates: int = 0, rec_beams: int = 0,
-                       length_penalty: float = 1.0, rec_locations: bool = False):
+                       length_penalty: float = 1.0, rec_locations: bool = False, rec_charset: Optional[str] = None):
         """Several window prompts per encoded image in one batched decode (``alm_omni_decode_prompts``).
         prompts: [P, L] (the same P prompts for every image) or [B, P, L], P <= 16, e.g. rows of
         ``vocab.window_prompt(...)``.  Returns a list over images of lists over prompts; item [b][p] is what the
@@ -1098,7 +1173,8 @@ class OmniParserB200:
         ``([pt, poly, rec], [probs])`` or None.  rec_candidates: as in ``decode``, [B, P, max_inst, rec_length, k].
         rec_beams / length_penalty: as in ``decode``, [B, P, max_inst, W, rec_length]; a point shared by several
         prompts of a page carries its n-best list to each of their slots.  rec_locations: as in ``decode``,
-        [B, P, max_inst, rec_length, 5]; a shared point carries its locations to each slot."""
+        [B, P, max_inst, rec_length, 5]; a shared point carries its locations to each slot.  rec_charset: as in
+        ``decode``."""
         v = self.vocab
         B = len(self.page_shapes())
         p = prompts.to(torch.long).cpu()
@@ -1115,7 +1191,9 @@ class OmniParserB200:
         rec = np.zeros((B, P, maxi, v.rec_length), dtype=np.int64)
         prob = np.zeros((B, P, maxi, v.rec_length), dtype=np.float32)
         cfg = self._cfg(maxi)
+        sets = check_rec_charset(rec_charset, v.chars)
         self._set_rec_candidates(rec_candidates, rec_beams, length_penalty, rec_locations)
+        self._set_rec_charset(sets)
         self.ctx.check(self.lib.alm_omni_decode_prompts(self.ctx.h, p.data_ptr(), P, p.shape[2], C.byref(cfg),
                                                         n_inst.ctypes.data, pt.ctypes.data, poly.ctypes.data,
                                                         rec.ctypes.data, prob.ctypes.data))
@@ -1123,7 +1201,8 @@ class OmniParserB200:
         return [[_spotting_result(n_inst[b, k], pt[b, k], poly[b, k], rec[b, k], prob[b, k]) for k in range(P)]
                 for b in range(B)]
 
-    def decode_dense(self, pt_prompt: Optional[torch.Tensor] = None, grid='auto', iou: float = 0.5):
+    def decode_dense(self, pt_prompt: Optional[torch.Tensor] = None, grid='auto', iou: float = 0.5,
+                     rec_charset: Optional[str] = None):
         """Text spotting of dense pages, with more words than one point sequence holds (``alm_omni_decode_dense``; rule:
         DESIGN 4.16).  grid='auto': every page is read as ``decode`` reads it; a page whose point sequence runs out of
         steps without EOS is read again in the 2 x 2 windows of the training grids, and at 3 x 3 if one of those runs
@@ -1134,11 +1213,11 @@ class OmniParserB200:
         window=[int32 [n] per page: the window of each row], grid=int32 [B, 2] (nx, ny) used, saturated=bool [B, 9]
         per window of that grid: its sequence ran out of steps, so the window may have missed words, loops=int32 [n, 4]
         the window point loops and polygon / recognition passes run beyond level 0, as (kind, first page, pages, per
-        page))."""
-        n_inst, pt, poly, rec, prob = self._decode_dense_arrays(pt_prompt, grid, iou)
+        page)).  rec_charset: as in ``decode``, for every recognition pass."""
+        n_inst, pt, poly, rec, prob = self._decode_dense_arrays(pt_prompt, grid, iou, rec_charset)
         return [_spotting_result(n_inst[b], pt[b], poly[b], rec[b], prob[b]) for b in range(len(n_inst))]
 
-    def _decode_dense_arrays(self, pt_prompt=None, grid='auto', iou=0.5):
+    def _decode_dense_arrays(self, pt_prompt=None, grid='auto', iou=0.5, rec_charset=None):
         v = self.vocab
         if v.vie_categories:
             raise ValueError('decode_dense reads text-spotting checkpoints only')
@@ -1166,7 +1245,9 @@ class OmniParserB200:
         grids = np.zeros((B, 2), dtype=np.int32)
         sat = np.zeros((B, 9), dtype=np.uint8)
         cfg = self._cfg(maxi)
+        sets = check_rec_charset(rec_charset, v.chars)
         self._set_rec_candidates(0)
+        self._set_rec_charset(sets)
         self.ctx.check(self.lib.alm_omni_decode_dense(self.ctx.h, prompt.data_ptr(), prompt.numel(), C.byref(cfg), nx, ny,
                                                       iou, cap, n_inst.ctypes.data, pt.ctypes.data, poly.ctypes.data,
                                                       rec.ctypes.data, prob.ctypes.data, window.ctypes.data,
@@ -1201,15 +1282,17 @@ class OmniParserB200:
         return [(torch.from_numpy(toks[b, :n_tok[b]].copy()), torch.from_numpy(prob[b, :n_tok[b]].copy())) for b in range(B)]
 
     def decode_kie(self, image_sizes, pt_prompt: Optional[torch.Tensor] = None, rec_candidates: int = 0, rec_beams: int = 0,
-                   length_penalty: float = 1.0, rec_locations: bool = False):
+                   length_penalty: float = 1.0, rec_locations: bool = False, rec_charset: Optional[str] = None):
         """KIE decoding of every encoded image (model/transformer.py:143-217): per image the reference's
         ``[(text, class_name, prob, [[x0,y0,x1,y1], ...]), ...]``.  image_sizes: (h, w) per image (seq[3]).
         rec_candidates: as in ``decode``; the candidates of pair n belong to ``last_kie_raw['rec'][b, n]``.
         rec_beams / length_penalty: as in ``decode``; the n-best list of pair n is ``last_rec_beams[...][b, n]``.
-        rec_locations: as in ``decode``; the locations of pair n are ``last_rec_locations[b, n]``."""
+        rec_locations: as in ``decode``; the locations of pair n are ``last_rec_locations[b, n]``.
+        rec_charset: as in ``decode``, for every pair's transcription (the point loop and its classes are unchanged)."""
         v = self.vocab
         n_inst, pos, poly, rec, prob, n_tok, toks, tprob = self._decode_kie_arrays(pt_prompt, rec_candidates, rec_beams,
-                                                                                  length_penalty, rec_locations)
+                                                                                  length_penalty, rec_locations,
+                                                                                  rec_charset)
         self.last_kie_raw = dict(n_tok=n_tok, tokens=toks, probs=tprob, n_inst=n_inst, inst_pos=pos, poly=poly, rec=rec,
                                  rec_prob=prob)
         results = []
@@ -1251,7 +1334,7 @@ class OmniParserB200:
         return ''.join(chars)
 
     def _decode_kie_arrays(self, pt_prompt=None, rec_candidates=0, rec_beams=0, length_penalty=1.0,
-                           rec_locations=False):
+                           rec_locations=False, rec_charset=None):
         """alm_omni_decode_kie's outputs for every encoded image, in _decode_arrays' order with inst_pos in place of
         pt, then the token stream: n_inst int32 [B], inst_pos int32 [B, max_inst], poly int64 [B, max_inst, 32], rec
         [B, max_inst, rec_length], prob f32 [B, max_inst, rec_length], n_tok int32 [B], tokens int64 [B,
@@ -1270,7 +1353,9 @@ class OmniParserB200:
         rec = np.zeros((B, maxi, L), dtype=np.int64)
         prob = np.zeros((B, maxi, L), dtype=np.float32)
         cfg = self._cfg(maxi)
+        sets = check_rec_charset(rec_charset, v.chars)
         self._set_rec_candidates(rec_candidates, rec_beams, length_penalty, rec_locations)
+        self._set_rec_charset(sets)
         self.ctx.check(self.lib.alm_omni_decode_kie(self.ctx.h, prompt.data_ptr(), prompt.numel(), C.byref(cfg),
                                                     n_tok.ctypes.data, toks.ctypes.data, tprob.ctypes.data,
                                                     n_inst.ctypes.data, pos.ctypes.data, poly.ctypes.data, rec.ctypes.data,
@@ -1282,7 +1367,7 @@ class OmniParserB200:
                    band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200,
                    test_max_size: int = 1920, orientation='upright', whole_page: bool = False,
                    rec_locations: bool = False, rec_candidates: int = 0, rec_beams: int = 0,
-                   length_penalty: float = 1.0) -> List[List[dict]]:
+                   length_penalty: float = 1.0, rec_charset: Optional[str] = None) -> List[List[dict]]:
         """Text spotting of pages larger than the model's input, read in overlapping tiles (rule: DESIGN 4.11).
         pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch).  Every page is cut into the tiles
         of ``preprocess.omni_tile_plan(sizes, tile, overlap)``; each tile goes through the reference's validation
@@ -1334,7 +1419,10 @@ class OmniParserB200:
         the point and polygon loops stay greedy and the tile merge decides on boxes and tile edges, so for 'upright'
         and explicit turns the words, points, polygons, 'tile' and 'instance' are those without beams; 'auto' and
         'mixed' choose on hypothesis 0's score.  Candidates combine with rec_locations; beams do not, and neither
-        combines with whole_page (``decode_dense`` offers neither).  Refusals come before any device work."""
+        combines with whole_page (``decode_dense`` offers neither).
+        rec_charset (rule: DESIGN 4.23): a string, as in ``decode``; every tile decode, 'auto''s probes and the
+        whole-page readings read with it, so every returned text is in the set.  Refusals come before any device
+        work."""
         from . import postprocess
         v = self.vocab
         self._check_checkpoint('spot_tiled')
@@ -1345,11 +1433,12 @@ class OmniParserB200:
         if (K or W) and whole_page:
             raise ValueError('rec_candidates and rec_beams cannot be combined with whole_page: whole-page readings '
                              'have neither')
+        check_rec_charset(rec_charset, v.chars)
         mode, turns = _parse_orientation(orientation, len(pages), ('upright', 'auto', 'mixed'), 'page')
         pages, sizes = self._device_pages(pages)
         P = len(sizes)
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
-        decode = self._tile_decode(K, W, lp, rec_locations)
+        decode = self._tile_decode(K, W, lp, rec_locations, rec_charset)
         extra = {}
         if mode == 'auto':
             turns, extra = self._probe_turns(pages, sizes, tile, overlap, max_batch, test_min_size, test_max_size,
@@ -1372,7 +1461,7 @@ class OmniParserB200:
                 whole = tuple(a[4 * np.arange(P) + turns] for a in extra['probe'])
             else:
                 whole = self._read_whole(rpages, rsizes, rturns, tile, max_batch, test_min_size, test_max_size,
-                                         self._decode_dense_arrays)
+                                         lambda: self._decode_dense_arrays(rec_charset=rec_charset))
             out = merge_whole_page(self.ctx, rsizes, tile, overlap, m, *whole, v.num_bins, margin, turns=rturns)
         # the words of every page, each with its reading and its (tile, instance) in the readings' plan
         if mode == 'mixed':
@@ -1411,7 +1500,7 @@ class OmniParserB200:
     def read_regions(self, pages, regions, page_index, kind: str = 'quad', tile: int = 1200, overlap: int = 256,
                      max_batch: int = 16, test_min_size: int = 1200, test_max_size: int = 1920, rec_candidates: int = 0,
                      rec_beams: int = 0, length_penalty: float = 1.0, rec_locations: bool = False,
-                     orientation='upright') -> List[dict]:
+                     orientation='upright', rec_charset=None) -> List[dict]:
         """Read caller-given regions of raw pages of any size (rule: DESIGN 4.19): OmniParser as the recogniser of
         another detector's regions, each word read in place on the page and returned with its 16-point polygon.
         pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch); regions of one kind, in page
@@ -1444,6 +1533,9 @@ class OmniParserB200:
         plan; candidates, beams and 'chars' follow the kept reading.  ``last_regions`` gains 'readings' ((page, turn)
         pairs), 'reading', 'route' and the readings' 'rec' / 'prob' per (region, candidate), 'turns' [R], 'frames' /
         'frame_index' (the frames of ``select_regions``), and for 'auto' 'candidates' [R, 2] and 'scores' f64 [R, 2].
+        rec_charset (rule: DESIGN 4.23): a string for every region, as in ``decode``, or a sequence of R strings or None,
+        one per region (None: read unconstrained), e.g. digits for an amount field and upper case and digits for a
+        plate; 'auto' reads both turns of a region under its set and chooses on the constrained scores.
         Not offered: KIE checkpoints, and any merge or dedupe of overlapping regions -- each region is read as given."""
         from . import postprocess
         from . import preprocess as Pre
@@ -1467,6 +1559,9 @@ class OmniParserB200:
             cand = (np.zeros(R, np.int32) if mode == 'upright' else cand).reshape(R, 1)
         K, W = int(rec_candidates), int(rec_beams)
         self._set_rec_candidates(K, W, length_penalty, rec_locations)   # refused before device work
+        per_region = rec_charset is not None and not isinstance(rec_charset, str)
+        if check_rec_charset(rec_charset, v.chars, R if per_region else None) is None:
+            rec_charset, per_region = None, False
         C = cand.shape[1]
         boxes = region_boxes(regions, kind)
         if mode == 'upright':   # every page a reading at turn 0, the plan and routing of the pages as they are
@@ -1515,7 +1610,8 @@ class OmniParserB200:
                                     turns=rturns[idx])
             self._encode_chunk(nt, [f[2:] for f in frames], test_min_size, test_max_size)
             local = [postprocess.point_bins(tpts[r_] - np.array([f[1], f[0]]), f[2:], nb) for f, r_ in zip(frames, rows)]
-            n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty, rec_locations)
+            cs = [[rec_charset[r_c // C] for r_c in r_] for r_ in rows] if per_region else rec_charset
+            n, xy, pl, rc, pb = self._read_at_arrays(local, K, W, length_penalty, rec_locations, cs)
             for j, r_ in enumerate(rows):
                 k = len(r_)
                 pt[r_], poly[r_], rec[r_], prob[r_] = xy[j, :k], pl[j, :k], rc[j, :k], pb[j, :k]
@@ -1562,7 +1658,7 @@ class OmniParserB200:
     def kie_tiled(self, pages, tile: int = 1200, overlap: int = 256, max_batch: int = 16, margin: float = 4,
                   band: Optional[float] = None, iou: float = 0.5, test_min_size: int = 1200, test_max_size: int = 1920,
                   orientation='upright', rec_candidates: int = 0, rec_beams: int = 0,
-                  rec_locations: bool = False, whole_page: bool = False) -> List[list]:
+                  rec_locations: bool = False, whole_page: bool = False, rec_charset: Optional[str] = None) -> List[list]:
         """KIE of pages larger than the model's input or turned by quarter-turns, read in overlapping tiles (rule:
         DESIGN 4.18).  pages: decoded uint8 RGB pages [h, w, 3] (host numpy / torch or CUDA torch); the checkpoint must
         be a KIE checkpoint.  Every page is cut into the tiles of ``preprocess.omni_tile_plan(sizes, tile, overlap)``;
@@ -1595,18 +1691,20 @@ class OmniParserB200:
         ``char_boxes`` call for all pages gives every word ``postprocess.rec_char_boxes``' list (char, centre, cov, box)
         in pixels of the page as passed in.  Each entity tuple then gains a fifth element, that list per word in
         ``rects`` order.  ``last_tiles`` gains 'loc', every tile's locations.  Recognition candidates and beams are not
-        offered here."""
+        offered here.  rec_charset (rule: DESIGN 4.23): a string, as in ``decode_kie``, for every tile decode, probe
+        and whole-page reading."""
         v = self.vocab
         self._check_checkpoint('kie_tiled', kie=True)
         if rec_candidates or rec_beams:
             raise ValueError('kie_tiled offers no recognition candidates or beams')
+        check_rec_charset(rec_charset, v.chars)
         rec_locations = bool(rec_locations)
         _check_max_batch(max_batch)
         mode, turns = _parse_orientation(orientation, len(pages), ('upright', 'auto'), 'page')
         pages, sizes = self._device_pages(pages)
         P = len(sizes)
         margin, band, iou = check_merge_args(margin, overlap / 4 if band is None else band, iou)
-        decode = self._kie_tile_decode(rec_locations)
+        decode = self._kie_tile_decode(rec_locations, rec_charset)
         extra = {}
         if mode == 'auto':
             turns, extra = self._probe_turns(pages, sizes, tile, overlap, max_batch, test_min_size, test_max_size,
@@ -1727,22 +1825,24 @@ class OmniParserB200:
             a[big] = b
         return out
 
-    def _tile_decode(self, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False):
+    def _tile_decode(self, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False, rec_charset=None):
         """The decode of spot_tiled's tiles and probes: a function giving ``_decode_arrays``' five arrays, then with
         rec_locations the locations f32 [B, max_inst, rec_length, 5], then with rec_candidates the candidates (ids,
-        probs) or with rec_beams the n-best lists (ids, probs, scores), in ``decode``'s layouts."""
+        probs) or with rec_beams the n-best lists (ids, probs, scores), in ``decode``'s layouts; every decode reads
+        with rec_charset."""
         def decode():
-            out = self._decode_arrays(None, rec_candidates, rec_beams, length_penalty, rec_locations)
+            out = self._decode_arrays(None, rec_candidates, rec_beams, length_penalty, rec_locations, rec_charset)
             if rec_locations:
                 out += (self.last_rec_locations,)
             return out + (self.last_rec_candidates or self.last_rec_beams or ())
         return decode
 
-    def _kie_tile_decode(self, rec_locations=False):
+    def _kie_tile_decode(self, rec_locations=False, rec_charset=None):
         """The decode of kie_tiled's tiles, probes and whole readings: a function giving ``_decode_kie_arrays``' eight
-        arrays, then with rec_locations the locations f32 [B, max_inst, rec_length, 5] (``decode_kie``'s layout)."""
+        arrays, then with rec_locations the locations f32 [B, max_inst, rec_length, 5] (``decode_kie``'s layout); every
+        decode reads with rec_charset."""
         def decode():
-            out = self._decode_kie_arrays(None, 0, 0, 1.0, rec_locations)
+            out = self._decode_kie_arrays(None, 0, 0, 1.0, rec_locations, rec_charset)
             return out + ((self.last_rec_locations,) if rec_locations else ())
         return decode
 
@@ -1834,14 +1934,15 @@ class OmniParserB200:
 
     # ---------------------------------------------------------------------------------------- forward
     def forward(self, samples: NestedTensor, sequence=None, rec_candidates: int = 0, rec_beams: int = 0,
-                length_penalty: float = 1.0, rec_locations: bool = False):
+                length_penalty: float = 1.0, rec_locations: bool = False, rec_charset: Optional[str] = None):
         """Reference contract for batch 1 (engine/val.py:22,35): returns
         ``([pt[1,2N], poly[1,32N], rec[1,N,L]], [probs[N,L]])`` or ``None``.
         ``sequence`` = [pt_prompt, poly_prompt, rec_prompt, orig_size]; the poly/rec prompts are the fixed
         sos tokens (val.py:30-31) and are validated, the pt prompt is passed through.
-        rec_candidates, rec_beams, length_penalty, rec_locations: as in ``decode`` (the return value keeps the reference
-        shape)."""
-        outs = self.forward_batch(samples, sequence, rec_candidates, rec_beams, length_penalty, rec_locations)
+        rec_candidates, rec_beams, length_penalty, rec_locations, rec_charset: as in ``decode`` (the return value keeps
+        the reference shape)."""
+        outs = self.forward_batch(samples, sequence, rec_candidates, rec_beams, length_penalty, rec_locations,
+                                  rec_charset)
         if len(outs) != 1:
             raise ValueError('OmniParser.forward keeps the reference batch-1 contract; use forward_batch for B > 1')
         return outs[0]
@@ -1855,36 +1956,43 @@ class OmniParserB200:
         return sequence[0]
 
     def forward_batch(self, samples: NestedTensor, sequence=None, rec_candidates: int = 0, rec_beams: int = 0,
-                      length_penalty: float = 1.0, rec_locations: bool = False) -> List:
+                      length_penalty: float = 1.0, rec_locations: bool = False,
+                      rec_charset: Optional[str] = None) -> List:
         """Padded-batch semantics: every page is encoded on the common canvas with the mask (the reference's
         ``model(samples, seqs)`` for a batch).  forward_pages gives each page its batch-1 result instead."""
         pt_prompt = self._pt_prompt(sequence)
+        check_rec_charset(rec_charset, self.vocab.chars)
         self.encode(samples.tensors, samples.mask)
         return self._decode_all(samples.tensors.shape[0], sequence, pt_prompt, rec_candidates, rec_beams, length_penalty,
-                                rec_locations)
+                                rec_locations, rec_charset)
 
     def forward_pages(self, samples: NestedTensor, sequence=None, rec_candidates: int = 0, rec_beams: int = 0,
-                      length_penalty: float = 1.0, rec_locations: bool = False, dense=None) -> List:
+                      length_penalty: float = 1.0, rec_locations: bool = False, dense=None,
+                      rec_charset: Optional[str] = None) -> List:
         """A batch of pages of different sizes (e.g. from ``preprocess.omni_pages``): a list over pages of what the
         reference's batch-1 ``model(nested_tensor_from_tensor_list([page_b]), seqs)`` returns, text spotting or KIE.
         The page sizes come from the mask (``page_sizes_from_mask``: each page a top-left rectangle, ValueError
         otherwise).  dense='auto' or a grid (nx, ny): text spotting through ``decode_dense(grid=dense)``, so a page with
-        more words than one point sequence holds is read in windows instead of failing (None: ``decode``)."""
+        more words than one point sequence holds is read in windows instead of failing (None: ``decode``).  rec_charset:
+        as in ``decode``, also with dense."""
         pt_prompt = self._pt_prompt(sequence)
+        check_rec_charset(rec_charset, self.vocab.chars)
         if dense is not None and (rec_candidates or rec_beams or rec_locations):
             raise ValueError('dense decoding cannot be combined with rec_candidates, rec_beams or rec_locations')
         sizes = page_sizes_from_mask(samples.mask)
         self.encode_pages(samples.tensors, sizes)
         if dense is not None:
-            return self.decode_dense(pt_prompt, grid=dense)
-        return self._decode_all(len(sizes), sequence, pt_prompt, rec_candidates, rec_beams, length_penalty, rec_locations)
+            return self.decode_dense(pt_prompt, grid=dense, rec_charset=rec_charset)
+        return self._decode_all(len(sizes), sequence, pt_prompt, rec_candidates, rec_beams, length_penalty, rec_locations,
+                                rec_charset)
 
-    def _decode_all(self, B, sequence, pt_prompt, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False):
+    def _decode_all(self, B, sequence, pt_prompt, rec_candidates=0, rec_beams=0, length_penalty=1.0, rec_locations=False,
+                    rec_charset=None):
         if self.vocab.vie_categories:
             if sequence is None or len(sequence) < 4:
                 raise ValueError('KIE needs the original image size as sequence[3] (engine/val.py:33)')
             size = sequence[3]
             sizes = [size] * B if torch.as_tensor(size).dim() == 1 else size
             return self.decode_kie([tuple(float(x) for x in torch.as_tensor(sz).reshape(-1)[:2]) for sz in sizes], pt_prompt,
-                                   rec_candidates, rec_beams, length_penalty, rec_locations)
-        return self.decode(pt_prompt, rec_candidates, rec_beams, length_penalty, rec_locations)
+                                   rec_candidates, rec_beams, length_penalty, rec_locations, rec_charset)
+        return self.decode(pt_prompt, rec_candidates, rec_beams, length_penalty, rec_locations, rec_charset)

@@ -395,6 +395,35 @@ ALM_API int alm_omni_get_rec_beams(alm_ctx* ctx, int64_t* ids, float* probs, flo
 ALM_API int alm_omni_set_rec_locations(alm_ctx* ctx, int on);
 ALM_API int alm_omni_get_rec_locations(alm_ctx* ctx, float* out, size_t elems);
 
+/* Character sets: restrict the recognition loop to caller-given characters, per decode or per row -- an amount, a
+ * date or an ID field (digits and ".,-/"), a licence plate (upper case and digits), a meter reading (digits).  The
+ * choice is constrained at every step, so a wrong first character is never fed back as filtering the text afterwards
+ * would leave it.  The rule:
+ *   - chars are the checkpoint's characters, classes num_bins + i (n_chars = recog_pad - num_bins - 1, 95 by
+ *     default).  A set is a subset of chars with at least one character: allowed uint8 [n_sets][n_chars], nonzero =
+ *     chars[i] in the set.
+ *   - while a set is in force, rec step j of an instance may choose num_bins + i for every chars[i] in the set, the
+ *     unknown class recog_pad - 1, recog_pad and rec_eos: the allowed set of the recognition loop intersected with the
+ *     caller's characters.  A word can still end, and a glyph the set cannot name can still be read as unknown, which
+ *     decode_seq drops, so every character of every returned text is in the set.  The full set gives every output,
+ *     launch and list bit for bit as without a set.
+ *   - a chosen class keeps its probability under the step's softmax over logits[:nsoft] (not renormalised over the
+ *     set), so the decode_pred_seq score of a forced word drops.  Ties go to the lower id.
+ *   - candidates are the k best classes of the constrained set (id -1, probability 0 past its end; candidate 0 is
+ *     rec); beams expand only into it (W = 1 is still the greedy loop up to the terminal token); character locations
+ *     follow the constrained path.  The point and polygon loops are unchanged.
+ * n_sets = 0 turns the setting off (the default: nothing allocated, copied or launched).  With row_set NULL (n_rows 0)
+ * every instance of the following alm_omni_decode / _prompts / _kie / _at / _dense calls uses set 0.  A row_set is
+ * read by alm_omni_decode_at alone: int32 [B][cap] of that call (n_rows = B cap), point n of page b reads with set
+ * row_set[b cap + n].  The setting is copied and stays in force until the next call.
+ * Errors: ALM_ERR_INVALID here, leaving the previous setting, for n_sets outside 0..ALM_MAX_CHARSETS, a null allowed or
+ * n_chars < 1, an empty set, a set index outside [0, n_sets), or row_set and n_rows not given together; ALM_ERR_INVALID
+ * from a decode, before any device work and leaving the context usable, for n_chars other than recog_pad - num_bins -
+ * 1, row sets with any entry other than alm_omni_decode_at, or n_rows other than its B cap. */
+#define ALM_MAX_CHARSETS 65536
+ALM_API int alm_omni_set_rec_charset(alm_ctx* ctx, const uint8_t* allowed, int n_sets, int n_chars,
+                                     const int32_t* row_set, size_t n_rows);
+
 /* Teacher-forced logits: replaces `Transformer.decode(input_seq, memory, mask, pos_embed, input_type)`
  * (transformer.py:74-100) for image `image`: seq int64 [n_seq, len] -> logits f32 [n_seq, len, V].
  * kind: 0 = pt, 1 = poly, 2 = rec. */
